@@ -1,4 +1,4 @@
-"""atom_b200 -- B200 (sm_100a) implementation of the efeslab/Atom W4A4 inference hot path.
+"""atom_b200 -- H100 (sm_90a) implementation of the efeslab/Atom W4A4 inference hot path.
 
     atom_b200.ops       operator API (mirror of punica.ops)
     atom_b200.kvcache   paged INT4 KV pool (mirror of punica.utils.kvcache)

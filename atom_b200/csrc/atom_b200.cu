@@ -17,10 +17,7 @@
 #include <utility>
 
 #include "../../include/atom_b200.h"
-#include "gemm_i4_sm100.cuh"
-#include "gemm_i4_skinny_sm100.cuh"
-#include "gemm_i4_tall_sm100.cuh"
-#include "gemm_i4_wide_sm100.cuh"
+#include "gemm_i4_sm90.cuh"
 #include "kv_kernels.cuh"
 #include "prefill_kernels.cuh"
 #include "comm_kernels.cuh"
@@ -88,7 +85,7 @@ inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 // cudaFuncAttributeMaxDynamicSharedMemorySize is per (function, device): raise it once for each pair, under a lock
 // (the reference calls cudaFuncSetAttribute on every launch, GEMM.cuh:757).
 template <typename F>
-int ensure_dynamic_smem(F* func, int bytes, const char* what, bool max_carveout = false) {
+int ensure_dynamic_smem(F* func, int bytes, const char* what) {
   static std::mutex mu;
   static std::set<std::pair<const void*, int>> done;
   int dev = 0;
@@ -98,10 +95,6 @@ int ensure_dynamic_smem(F* func, int bytes, const char* what, bool max_carveout 
   if (done.count(key)) return ATOM_OK;
   cudaError_t e = cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
   if (e != cudaSuccess) return fail(ATOM_E_CUDA, "%s: cudaFuncSetAttribute(smem=%d): %s", what, bytes, cudaGetErrorString(e));
-  if (max_carveout) {   // two ~100 KB CTAs per SM only fit when the SM's L1/shared split is at its shared-memory maximum
-    e = cudaFuncSetAttribute(func, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
-    if (e != cudaSuccess) return fail(ATOM_E_CUDA, "%s: cudaFuncSetAttribute(carveout): %s", what, cudaGetErrorString(e));
-  }
   done.insert(key);
   return ATOM_OK;
 }
@@ -141,7 +134,7 @@ std::mutex g_map_mu;
 std::unordered_map<MapKey, CUtensorMap, MapKeyHash> g_maps;
 
 // 2-D byte tensor [rows][inner] with row pitch `pitch`; box = box_rows x box_inner bytes; OOB rows read as zero.
-// swizzle: 0 = none, 1 = SWIZZLE_128B, 2 = SWIZZLE_64B
+// swizzle: 0 = none, 1 = SWIZZLE_128B
 int make_map(CUtensorMap* out, const void* ptr, uint64_t inner, uint64_t rows, uint64_t pitch, uint32_t box_inner,
              uint32_t box_rows, int swizzle) {
   MapKey key{ptr, inner, rows, pitch, box_inner, box_rows, (uint32_t)swizzle};
@@ -158,36 +151,9 @@ int make_map(CUtensorMap* out, const void* ptr, uint64_t inner, uint64_t rows, u
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(ptr), dims, strides, box, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  swizzle == 1 ? CU_TENSOR_MAP_SWIZZLE_128B : (swizzle == 2 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_NONE),
+                  swizzle == 1 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(ATOM_E_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
-  std::lock_guard<std::mutex> lk(g_map_mu);
-  if (g_maps.size() > 4096) g_maps.clear();
-  g_maps.emplace(key, *out);
-  return ATOM_OK;
-}
-
-// The same byte matrix viewed as [rows/4][2][2][inner] with the two middle dimensions swapped: a box of `box_rows` rows
-// lands in shared memory in the order 4q+0, 4q+2, 4q+1, 4q+3 (gemm_i4_tall_sm100.cuh: neighbouring accumulator columns
-// then belong to different channel pairs).  rows % 4 == 0; rows beyond the matrix read as zero.
-int make_map_quadswap(CUtensorMap* out, const void* ptr, uint64_t inner, uint64_t rows, uint64_t pitch, uint32_t box_inner,
-                      uint32_t box_rows, int swizzle) {
-  MapKey key{ptr, inner, rows, pitch, box_inner, box_rows, (uint32_t)swizzle | 0x100u};
-  {
-    std::lock_guard<std::mutex> lk(g_map_mu);
-    auto it = g_maps.find(key);
-    if (it != g_maps.end()) { *out = it->second; return ATOM_OK; }
-  }
-  EncodeFn fn = encode_fn();
-  if (!fn) return fail(ATOM_E_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
-  cuuint64_t dims[4] = {inner, 2, 2, (rows + 3) / 4};
-  cuuint64_t strides[3] = {2 * pitch, pitch, 4 * pitch};
-  cuuint32_t box[4] = {box_inner, 2, 2, box_rows / 4};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 4, const_cast<void*>(ptr), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle == 1 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(ATOM_E_CUDA, "cuTensorMapEncodeTiled (4-D) failed with CUresult %d", (int)r);
   std::lock_guard<std::mutex> lk(g_map_mu);
   if (g_maps.size() > 4096) g_maps.clear();
   g_maps.emplace(key, *out);
@@ -197,51 +163,11 @@ int make_map_quadswap(CUtensorMap* out, const void* ptr, uint64_t inner, uint64_
 // ------------------------------------------------------------------------------------------------ GEMM launch
 struct GemmOperands {
   const void *a, *b, *ak, *bk;
-  int64_t M, N, K;
+  int64_t M, N, K;          // N = weight rows
 };
 
-template <bool kSwap, int BN, int GS, int kPack, int kSplit, bool kO4, int kConvWarps, int kEpiWgs>
-int launch_gemm(const GemmOperands& op, const atom::GemmArgs& args, cudaStream_t stream) {
-  using C = atom::GemmCfg<kSwap, BN, GS, kPack, kSplit, kO4, kConvWarps, kEpiWgs>;
-  auto kern = atom::gemm_i4_kernel<kSwap, BN, GS, kPack, kSplit, kO4, kConvWarps, kEpiWgs>;
-  int rc = ensure_dynamic_smem(kern, C::SMEM_BYTES, "gemm_i4");
-  if (rc) return rc;
-  const uint64_t kp = (uint64_t)(op.K - 128) / 2;
-  // MMA-M operand = kSwap ? weights : tokens
-  const void* p4 = kSwap ? op.b : op.a;  const void* q4 = kSwap ? op.a : op.b;
-  const void* p8 = kSwap ? op.bk : op.ak; const void* q8 = kSwap ? op.ak : op.bk;
-  const uint64_t prow = kSwap ? op.N : op.M, qrow = kSwap ? op.M : op.N;
-  CUtensorMap tp4, tq4, tp8, tq8;
-  if ((rc = make_map(&tp4, p4, kp, prow, kp, 64, C::BM, 0))) return rc;
-  if ((rc = make_map(&tq4, q4, kp, qrow, kp, 64, BN, 0))) return rc;
-  if ((rc = make_map(&tp8, p8, 128, prow, 128, 128, C::BM, 1))) return rc;
-  if ((rc = make_map(&tq8, q8, 128, qrow, 128, 128, BN, 1))) return rc;
-
-  const int ch_tile = kSwap ? C::BM : BN, tok_tile = kSwap ? BN : C::BM;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)((op.N + ch_tile - 1) / ch_tile), (unsigned)((op.M + tok_tile - 1) / tok_tile), kSplit);
-  cfg.blockDim = dim3(C::THREADS);
-  cfg.dynamicSmemBytes = C::SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 1; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = kSplit;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  atom::GemmArgs largs = args;
-  if (pdl_enabled()) {
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.numAttrs = 2;
-    largs.pdl = 1;
-  }
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, tp4, tq4, tp8, tq8, largs);
-  if (e != cudaSuccess) return fail(ATOM_E_CUDA, "gemm_i4 launch: %s", cudaGetErrorString(e));
-  return ATOM_OK;
-}
-
-// Decode-shape kernel (gemm_i4_skinny_sm100.cuh): weights expanded into tensor memory, two CTAs per SM, always launched
-// with programmatic stream serialization (the kernel fetches only weights before griddepcontrol.wait).
+// The GEMM is launched with programmatic stream serialization unless ATOM_B200_GEMM_PDL=0: the kernel fetches only weights
+// before griddepcontrol.wait.
 int g_gemm_pdl = -1;
 bool gemm_pdl_enabled() {
   if (g_gemm_pdl < 0) {
@@ -251,26 +177,24 @@ bool gemm_pdl_enabled() {
   return g_gemm_pdl == 1;
 }
 
+// out_channels: channels that get a tile of their own (gate/up: op.N = 2 I weight rows, I output channels)
 template <int BN, int kSplit, int kEpi>
-int launch_skinny(const GemmOperands& op, const atom::GemmArgs& args, cudaStream_t stream, int64_t out_channels = -1) {
-  using C = atom::SkinnyCfg<BN, kSplit, kEpi>;
-  auto kern = atom::gemm_i4_skinny_kernel<BN, kSplit, kEpi>;
-  int rc = ensure_dynamic_smem(kern, C::SMEM_BYTES, "gemm_i4 (skinny)", true);
+int launch_gemm(const GemmOperands& op, const atom::GemmArgs& args, cudaStream_t stream, int64_t out_channels = -1) {
+  using C = atom::GemmCfg<BN, kSplit, kEpi>;
+  auto kern = atom::gemm_i4_kernel<BN, kSplit, kEpi>;
+  int rc = ensure_dynamic_smem(kern, C::SMEM_BYTES, "gemm_i4");
   if (rc) return rc;
   const uint64_t kp = (uint64_t)(op.K - 128) / 2;
-  CUtensorMap tp4, tp8;       // weights only: the token operand is read with plain loads (no descriptor per activation buffer)
-  if ((rc = make_map(&tp4, op.b, kp, op.N, kp, 64, C::BM, 2))) return rc;
-  if ((rc = make_map(&tp8, op.bk, 128, op.N, 128, 128, C::BM, 1))) return rc;
+  CUtensorMap tw4, ta4, tw8, ta8;
+  if ((rc = make_map(&tw4, op.b, kp, op.N, kp, 64, 128, 0))) return rc;
+  if ((rc = make_map(&ta4, op.a, kp, op.M, kp, 64, BN, 0))) return rc;
+  if ((rc = make_map(&tw8, op.bk, 128, op.N, 128, 128, 128, 1))) return rc;
+  if ((rc = make_map(&ta8, op.ak, 128, op.M, 128, 128, BN, 1))) return rc;
+  const int64_t chan = out_channels > 0 ? out_channels : op.N;
   cudaLaunchConfig_t cfg{};
-  const int64_t chan = out_channels > 0 ? out_channels : op.N;       // (gate/up: op.N = 2 I weight rows, I output channel tiles)
-  cfg.gridDim = dim3((unsigned)((chan + C::BM - 1) / C::BM), (unsigned)((op.M + BN - 1) / BN), kSplit);
+  cfg.gridDim = dim3((unsigned)((chan + 127) / 128), (unsigned)((op.M + BN - 1) / BN), kSplit);
   cfg.blockDim = dim3(C::THREADS);
   cfg.dynamicSmemBytes = C::SMEM_BYTES;
-  if (kEpi == atom::EPI_GATEUP && (args.dbg & 2) && C::SMEM_BYTES < 120 * 1024) {     // experiment: one CTA per SM
-    static bool raised = false;
-    if (!raised) { cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 120 * 1024); raised = true; }
-    cfg.dynamicSmemBytes = 120 * 1024;
-  }
   cfg.stream = stream;
   cudaLaunchAttribute attr[2];
   attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -282,157 +206,57 @@ int launch_skinny(const GemmOperands& op, const atom::GemmArgs& args, cudaStream
     attr[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.numAttrs = 2;
   }
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, tp4, tp8, args);
-  if (e != cudaSuccess) return fail(ATOM_E_CUDA, "gemm_i4 (skinny) launch: %s", cudaGetErrorString(e));
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, tw4, ta4, tw8, ta8, args);
+  if (e != cudaSuccess) return fail(ATOM_E_CUDA, "gemm_i4 launch: %s", cudaGetErrorString(e));
   return ATOM_OK;
 }
 
-// Prefill-shape kernel (gemm_i4_tall_sm100.cuh): biased accumulators, packed FP32 epilogue, TMA-permuted weight rows.
-template <bool kO4>
-int launch_tall(const GemmOperands& op, const atom::GemmArgs& args, cudaStream_t stream) {
-  using C = atom::TallCfg<kO4>;
-  auto kern = atom::gemm_i4_tall_kernel<kO4>;
-  int rc = ensure_dynamic_smem(kern, C::SMEM_BYTES, "gemm_i4 (tall)");
-  if (rc) return rc;
-  const uint64_t kp = (uint64_t)(op.K - 128) / 2;
-  CUtensorMap tp4, tq4, tp8, tq8;
-  if ((rc = make_map(&tp4, op.a, kp, op.M, kp, 64, C::BM, 0))) return rc;
-  if ((rc = make_map_quadswap(&tq4, op.b, kp, op.N, kp, 64, C::BN, 0))) return rc;
-  if ((rc = make_map(&tp8, op.ak, 128, op.M, 128, 128, C::BM, 1))) return rc;
-  if ((rc = make_map_quadswap(&tq8, op.bk, 128, op.N, 128, 128, C::BN, 1))) return rc;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)((op.N + C::BN - 1) / C::BN), (unsigned)((op.M + C::BM - 1) / C::BM), 1);
-  cfg.blockDim = dim3(C::THREADS);
-  cfg.dynamicSmemBytes = C::SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  cfg.attrs = attr;
-  cfg.numAttrs = 0;
-  if (gemm_pdl_enabled()) {
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.numAttrs = 1;
-  }
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, tp4, tq4, tp8, tq8, args);
-  if (e != cudaSuccess) return fail(ATOM_E_CUDA, "gemm_i4 (tall) launch: %s", cudaGetErrorString(e));
-  return ATOM_OK;
+// token tile: the smallest that holds a decode batch, 128 from 65 tokens on
+int token_tile(int64_t M, uint32_t flags) {
+  if (flags & ATOM_GEMM_FORCE_TALL) return 128;
+  const int bn = M <= 16 ? 16 : (M <= 32 ? 32 : (M <= 64 ? 64 : 128));
+  return (flags & ATOM_GEMM_FORCE_SKINNY) ? std::min(bn, 64) : bn;
 }
 
-// Prefill-shape kernel with the token operand in tensor memory, 128 x 256 tiles (gemm_i4_wide_sm100.cuh).
-template <bool kO4>
-int launch_wide(const GemmOperands& op, const atom::GemmArgs& args, cudaStream_t stream) {
-  using C = atom::WideCfg<kO4>;
-  auto kern = atom::gemm_i4_wide_kernel<kO4>;
-  int rc = ensure_dynamic_smem(kern, C::SMEM_BYTES, "gemm_i4 (wide)");
-  if (rc) return rc;
-  const uint64_t kp = (uint64_t)(op.K - 128) / 2;
-  CUtensorMap ta4, tb4, ta8, tb8;
-  if ((rc = make_map(&ta4, op.a, kp, op.M, kp, 64, C::BM, 2))) return rc;
-  if ((rc = make_map_quadswap(&tb4, op.b, kp, op.N, kp, 64, C::BH, 0))) return rc;
-  if ((rc = make_map(&ta8, op.ak, 128, op.M, 128, 128, C::BM, 1))) return rc;
-  if ((rc = make_map_quadswap(&tb8, op.bk, 128, op.N, 128, 128, C::BH, 1))) return rc;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)((op.N + C::NH * C::BH - 1) / (C::NH * C::BH)), (unsigned)((op.M + C::BM - 1) / C::BM), 1);
-  cfg.blockDim = dim3(C::THREADS);
-  cfg.dynamicSmemBytes = C::SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  cfg.attrs = attr;
-  cfg.numAttrs = 0;
-  if (gemm_pdl_enabled()) {
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.numAttrs = 1;
-  }
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, ta4, tb4, ta8, tb8, args);
-  if (e != cudaSuccess) return fail(ATOM_E_CUDA, "gemm_i4 (wide) launch: %s", cudaGetErrorString(e));
-  return ATOM_OK;
-}
-
-template <bool kO4, bool kPush = false>
-int skinny_dispatch(const GemmOperands& op, const atom::GemmArgs& args, uint32_t flags, cudaStream_t stream) {
-  constexpr int kEpi = kO4 ? atom::EPI_O4 : (kPush ? atom::EPI_PUSH : atom::EPI_O16);
-  const int64_t ch_tiles = (op.N + 127) / 128;
+template <int kEpi>
+int gemm_dispatch(const GemmOperands& op, const atom::GemmArgs& args, uint32_t flags, cudaStream_t stream, int64_t out_channels = -1) {
+  const int bn = token_tile(op.M, flags);
+  const int64_t tiles = ((out_channels > 0 ? out_channels : op.N) + 127) / 128 * ((op.M + bn - 1) / bn);
   const int groups = args.G + 1;
-  const int bn = op.M <= 16 ? 16 : (op.M <= 32 ? 32 : 64);
-  const int64_t tiles = ch_tiles * ((op.M + bn - 1) / bn);
-  // K split over a cluster (1, 2 or 4 ranks) until the CTAs cover the machine: 148 SMs, two CTAs resident on each for
-  // the 16- and 32-token tiles.  Every rank must keep at least ~4 groups, or the fixed cost per CTA dominates.
+  // K split over a cluster while the output tiles alone leave SMs of the 132 idle: a decode GEMM is a weight stream, and more
+  // CTAs keep more bytes in flight.  The reduction grows with the token tile, so only 16-token tiles split 4-way (two of their
+  // CTAs fit an SM: 264 slots), larger tiles 2-way; every rank keeps at least 4 groups; an 8-way split only runs on request.
+  // Measured on an H100 (80 GB HBM3, 700 W), device time per launch from a CUDA graph over operand sets larger than L2, split
+  // 1 / 2 / 4 / 8: 16 x 4096 x 4096: 23.5 / 15.8 / 12.8 / 16.7 us; 16 x 11008 x 4096: 27.0 / 21.0 / 26.7 / 29.8;
+  // 32 x 5120 x 5120: 29.2 / 19.9 / 26.0 / 30.5; 64 x 4096 x 4096: 27.8 / 18.8 / 28.3 / 35.8; 128 x 4096 x 4096: 38.9 / 35.3 / 47.3 / 55.5.
+  // The quantising epilogues work on FP32 sums in the reference's order and never split.
   int ksplit = 1;
-  if (!kO4 && !(flags & ATOM_GEMM_NO_SPLITK)) {
-    if (flags & ATOM_GEMM_SPLITK2) ksplit = 2;
-    else if (flags & ATOM_GEMM_SPLITK4) ksplit = 4;
-    else if ((flags & ATOM_GEMM_SPLITK8) && bn <= 32) ksplit = 8;
-    else if (groups >= 8) {
-      // The kernel is latency-, not bandwidth-bound: the largest split whose CTAs are all resident at once wins (148 SMs, two
-      // CTAs each for the 16/32-token tiles), as long as every rank keeps >= 4 groups (8-way: from 32 groups on).
-      // Measured (r02_gemm_skinny_v8_shape_table.jsonl): 16x4096x4096 5.9 us at 8 vs 6.3 at 4; 16x11008x4096 10.3 at 2 vs 12.6 at 1
-      // and 12.9 at 4 (344 CTAs: a second wave); 32x13824x5120 19.1 at 2 vs 29.0 at 1.
-      const int64_t slots = bn <= 32 ? 296 : 160;
-      if (bn <= 32 && groups >= 32 && tiles * 8 <= slots) ksplit = 8;
-      else ksplit = tiles * 4 <= slots ? 4 : (tiles * 2 <= slots ? 2 : 1);
+  if constexpr (kEpi == atom::EPI_O16 || kEpi == atom::EPI_PUSH) {
+    if (!(flags & (ATOM_GEMM_NO_SPLITK | ATOM_GEMM_FORCE_TALL))) {
+      if (flags & ATOM_GEMM_SPLITK2) ksplit = 2;
+      else if (flags & ATOM_GEMM_SPLITK4) ksplit = 4;
+      else if (flags & ATOM_GEMM_SPLITK8) ksplit = 8;
+      else if (op.M <= 128 && groups >= 8) {
+        const int64_t slots = bn == 16 ? 264 : 132;
+        ksplit = (bn == 16 && groups >= 16 && tiles * 4 <= slots) ? 4 : (tiles * 2 <= slots ? 2 : 1);
+      }
     }
   }
-  if constexpr (kO4) {
-    if (bn == 16) return launch_skinny<16, 1, kEpi>(op, args, stream);
-    if (bn == 32) return launch_skinny<32, 1, kEpi>(op, args, stream);
-    return launch_skinny<64, 1, kEpi>(op, args, stream);
-  } else {
-#define ATOM_SK(BN_)                                                                 \
-  return ksplit == 4   ? launch_skinny<BN_, 4, kEpi>(op, args, stream)               \
-         : ksplit == 2 ? launch_skinny<BN_, 2, kEpi>(op, args, stream)               \
-                       : launch_skinny<BN_, 1, kEpi>(op, args, stream)
-    if (bn == 16) { if (ksplit == 8) return launch_skinny<16, 8, kEpi>(op, args, stream); ATOM_SK(16); }
-    if (bn == 32) { if (ksplit == 8) return launch_skinny<32, 8, kEpi>(op, args, stream); ATOM_SK(32); }
-    ATOM_SK(64);
-#undef ATOM_SK
-  }
-}
-
-template <bool kO4>
-int gemm_dispatch(const GemmOperands& op, const atom::GemmArgs& args, uint32_t flags, cudaStream_t stream) {
-  // up to 128 tokens the weight-stationary orientation wins (4096^2, M=128: 13.9 us as two 64-token tiles vs 21.3 us for one
-  // wave of 32 128x128 tiles); from 3 token tiles on the 128x128 kernel is faster
-  // (65..128 tokens are two 64-token tiles per channel tile: only while those CTAs still fit one wave of 148 SMs)
-  const bool skinny = (flags & ATOM_GEMM_FORCE_SKINNY) ||
-                      (!(flags & ATOM_GEMM_FORCE_TALL) && (op.M <= 64 || (op.M <= 128 && (op.N + 127) / 128 * 2 <= 148)));
-  // <swap, BN, groups per pipeline stage, packed stages, K split, o4, converter warps, epilogue warpgroups>
-  if (!skinny) {
-    if (flags & ATOM_GEMM_LEGACY_TALL) return launch_gemm<false, 128, 2, 2, 1, kO4, 4, 2>(op, args, stream);
-    // 128 x 128 tiles by default.  The 128 x 256 kernel (token operand in tensor memory) halves the token-side conversion
-    // per MMA but measured slower at every size (4096^3: 704 vs 783-829 TOP/s, its 128-accumulator epilogue spills), so it
-    // only runs on request.
-    return (flags & ATOM_GEMM_FORCE_WIDE) ? launch_wide<kO4>(op, args, stream) : launch_tall<kO4>(op, args, stream);
-  }
-  // 33..64 tokens: the round-1 configuration (one CTA per SM, 8 converter warps) still measures faster than the new
-  // kernel's BN=64 instance (4096^2: 13.0-13.3 vs 15.0 us), which then only runs on request and under the fused epilogues
-  if (op.M <= 64 && !(flags & ATOM_GEMM_LEGACY_SKINNY) && (op.M <= 32 || (flags & ATOM_GEMM_FORCE_SKINNY))) {
-    if constexpr (!kO4) { if (args.ar.bufs != nullptr) return skinny_dispatch<false, true>(op, args, flags, stream); }
-    return skinny_dispatch<kO4>(op, args, flags, stream);
-  }
-  // decode shapes: weights on the MMA-M axis; K split 4-way over a cluster when one wave of CTAs would not
-  // cover the machine (the kernel is HBM-bound on the weights: more CTAs = more bytes in flight)
-  const int64_t ch_tiles = (op.N + 127) / 128;
-  const int groups = args.G + 1;
-  // K split over a cluster (1, 2 or 4 ranks): as many CTAs as it takes to give every SM about one, no more -- each extra
-  // wave of CTAs costs a full pipeline ramp (first TMA tile ~2 us after launch).
-  const int64_t tiles = ch_tiles * ((op.M + 63) / 64);
-  int ksplit = 1;
-  // o4 quantises from the FP32 sums: a K split would reorder them and move INT4 codes by one, so the KV projections
-  // never split (bit-identical codes to the reference kernel on every path)
-  if (!kO4 && !(flags & ATOM_GEMM_NO_SPLITK) && groups >= 8) {
-    if (flags & ATOM_GEMM_SPLITK2) ksplit = 2;
-    else if (flags & ATOM_GEMM_SPLITK4) ksplit = 4;
-    else ksplit = tiles * 4 <= 148 ? 4 : (tiles * 2 <= 148 ? 2 : 1);   // the largest split that still fits one wave of 148 SMs
-  }
-#define ATOM_SKINNY(BN, GS4, GS2, GS1, KP4, KP2, KP1, EW)                                                      \
-  return ksplit == 4   ? launch_gemm<true, BN, GS4, KP4, 4, kO4, 8, EW>(op, args, stream)                      \
-         : ksplit == 2 ? launch_gemm<true, BN, GS2, KP2, 2, kO4, 8, EW>(op, args, stream)                      \
-                       : launch_gemm<true, BN, GS1, KP1, 1, kO4, 8, EW>(op, args, stream)
-  if (op.M <= 16) { ATOM_SKINNY(16, 2, 2, 2, 4, 4, 4, 1); }
-  if (op.M <= 32) { ATOM_SKINNY(32, 2, 2, 2, 4, 4, 4, 1); }
-  ATOM_SKINNY(64, 1, 2, 2, 4, 2, 3, 2);
-#undef ATOM_SKINNY
+#define ATOM_BN(BN_)                                                                                  \
+  do {                                                                                                \
+    if constexpr (kEpi == atom::EPI_O16 || kEpi == atom::EPI_PUSH) {                                  \
+      if (ksplit == 8) return launch_gemm<BN_, 8, kEpi>(op, args, stream, out_channels);              \
+      if (ksplit == 4) return launch_gemm<BN_, 4, kEpi>(op, args, stream, out_channels);              \
+      if (ksplit == 2) return launch_gemm<BN_, 2, kEpi>(op, args, stream, out_channels);              \
+    }                                                                                                 \
+    return launch_gemm<BN_, 1, kEpi>(op, args, stream, out_channels);                                 \
+  } while (0)
+  if (bn == 16) ATOM_BN(16);
+  if (bn == 32) ATOM_BN(32);
+  if (bn == 64) ATOM_BN(64);
+  if constexpr (kEpi == atom::EPI_GATEUP || kEpi == atom::EPI_PUSH) return fail(ATOM_E_UNSUPPORTED, "gemm_i4: decode batches only (M <= 64)");
+  else ATOM_BN(128);
+#undef ATOM_BN
 }
 
 int gemm_common(const void* a, const void* b, const void* a_scale, const void* b_scale, const void* a_keeper,
@@ -451,7 +275,7 @@ int gemm_common(const void* a, const void* b, const void* a_scale, const void* b
     ATOM_REQUIRE(ar->bufs && ar->state && ar->world >= 1 && ar->world <= 32 && ar->rank >= 0 && ar->rank < ar->world && ar->slot % 8 == 0 &&
                  M * N <= ar->slot, "gemm_i4_o16_push: rank=%d world=%d, M x N = %lld must fit a slot of %lld elements", ar->rank, ar->world,
                  (long long)(M * N), (long long)ar->slot);
-    flags = (flags | ATOM_GEMM_FORCE_SKINNY) & ~(ATOM_GEMM_FORCE_TALL | ATOM_GEMM_LEGACY_SKINNY);
+    flags &= ~ATOM_GEMM_FORCE_TALL;
   }
   ATOM_REQUIRE(aligned16(b_scale) && aligned16(b_keeper_scale), "gemm_i4: weight scale pointers must be 16-byte aligned");
   ATOM_REQUIRE((reinterpret_cast<uintptr_t>(a_scale) & 3) == 0 && (reinterpret_cast<uintptr_t>(a_keeper_scale) & 3) == 0,
@@ -463,9 +287,9 @@ int gemm_common(const void* a, const void* b, const void* a_scale, const void* b
   args.a_keeper_scale = (const __half*)a_keeper_scale; args.b_keeper_scale = (const __half*)b_keeper_scale;
   args.d = o4 ? nullptr : (__half*)d; args.d4 = o4 ? (uint8_t*)d : nullptr; args.d_scale = (__half2*)d_scale;
   args.M = (int)M; args.N = (int)N; args.G = (int)(K / 128 - 1); args.lda_scale = atom::scale_size((int)M); args.trace = g_trace;
-  args.a4 = (const uint8_t*)a; args.a8 = (const int8_t*)a_keeper; args.ldb_scale = (int)N;
-  if (ar != nullptr) args.ar = *ar;
-  return o4 ? gemm_dispatch<true>(op, args, flags, (cudaStream_t)stream) : gemm_dispatch<false>(op, args, flags, (cudaStream_t)stream);
+  args.ldb_scale = (int)N;
+  if (ar != nullptr) { args.ar = *ar; return gemm_dispatch<atom::EPI_PUSH>(op, args, flags, (cudaStream_t)stream); }
+  return o4 ? gemm_dispatch<atom::EPI_O4>(op, args, flags, (cudaStream_t)stream) : gemm_dispatch<atom::EPI_O16>(op, args, flags, (cudaStream_t)stream);
 }
 
 int quant_check(const char* what, int seq_len, int hidden, const void* o8, const void* o4, const void* s8, const void* s4) {
@@ -576,7 +400,6 @@ int atom_gemm_i4_o16_push(const void* a, const void* b, const void* a_scale, con
 int atom_gemm_i4_qkv(const void* a, const void* b_qkv, const void* a_scale, const void* b_scale_qkv, const void* a_keeper,
                      const void* b_keeper_qkv, const void* a_keeper_scale, const void* b_keeper_scale_qkv, void* q, void* k,
                      void* k_scale, void* v, void* v_scale, int64_t M, int64_t H, int64_t K, uint32_t flags, void* stream) {
-  (void)flags;
   ATOM_REQUIRE(a && b_qkv && a_scale && b_scale_qkv && a_keeper && b_keeper_qkv && a_keeper_scale && b_keeper_scale_qkv && q && k &&
                k_scale && v && v_scale, "gemm_i4_qkv: null pointer argument");
   ATOM_REQUIRE(M > 0 && H > 0 && H % 128 == 0, "gemm_i4_qkv: M=%lld must be positive, H=%lld a positive multiple of 128", (long long)M, (long long)H);
@@ -584,40 +407,22 @@ int atom_gemm_i4_qkv(const void* a, const void* b_qkv, const void* a_scale, cons
   ATOM_REQUIRE(aligned16(a) && aligned16(b_qkv) && aligned16(a_keeper) && aligned16(b_keeper_qkv) && aligned16(q) && aligned16(b_scale_qkv) &&
                aligned16(b_keeper_scale_qkv), "gemm_i4_qkv: operand pointers must be 16-byte aligned");
   ATOM_REQUIRE(M < (1ll << 31) && 3 * H < (1ll << 31) && K < (1ll << 24), "gemm_i4_qkv: dimension too large");
-  const int64_t N = 3 * H, kp = (K - 128) / 2;
+  const int64_t N = 3 * H;
+  // one launch: 3H/128 channel tiles, the tile index selects the epilogue (q: FP16, k / v: asymmetric INT4 per head)
+  GemmOperands op{a, b_qkv, a_keeper, b_keeper_qkv, M, N, K};
   atom::GemmArgs args{};
   args.a_scale = (const __half*)a_scale; args.a_keeper_scale = (const __half*)a_keeper_scale;
-  args.M = (int)M; args.G = (int)(K / 128 - 1); args.lda_scale = atom::scale_size((int)M); args.trace = g_trace;
-  args.a4 = (const uint8_t*)a; args.a8 = (const int8_t*)a_keeper; args.ldb_scale = (int)N;
-  if (M <= 64) {
-    // one launch: 3H/128 channel tiles, the tile index selects the epilogue (q: FP16, k / v: asymmetric INT4 per head)
-    GemmOperands op{a, b_qkv, a_keeper, b_keeper_qkv, M, N, K};
-    args.b_scale = (const __half*)b_scale_qkv; args.b_keeper_scale = (const __half*)b_keeper_scale_qkv;
-    args.N = (int)N; args.seg_tiles = (int)(H / 128);
-    args.d = (__half*)q; args.d4 = (uint8_t*)k; args.d_scale = (__half2*)k_scale; args.d4_v = (uint8_t*)v; args.d_scale_v = (__half2*)v_scale;
-    if (M <= 16) return launch_skinny<16, 1, atom::EPI_QKV>(op, args, (cudaStream_t)stream);
-    if (M <= 32) return launch_skinny<32, 1, atom::EPI_QKV>(op, args, (cudaStream_t)stream);
-    return launch_skinny<64, 1, atom::EPI_QKV>(op, args, (cudaStream_t)stream);
-  }
-  // prefill sizes: three launches of the tall kernel on the row slices of the fused matrices
-  for (int seg = 0; seg < 3; ++seg) {
-    GemmOperands op{a, (const uint8_t*)b_qkv + (size_t)seg * H * kp, a_keeper, (const int8_t*)b_keeper_qkv + (size_t)seg * H * 128, M, H, K};
-    atom::GemmArgs sa = args;
-    sa.b_scale = (const __half*)b_scale_qkv + (size_t)seg * H; sa.b_keeper_scale = (const __half*)b_keeper_scale_qkv + (size_t)seg * H;
-    sa.N = (int)H;
-    int rc;
-    if (seg == 0) { sa.d = (__half*)q; rc = launch_tall<false>(op, sa, (cudaStream_t)stream); }
-    else { sa.d4 = (uint8_t*)(seg == 1 ? k : v); sa.d_scale = (__half2*)(seg == 1 ? k_scale : v_scale); rc = launch_tall<true>(op, sa, (cudaStream_t)stream); }
-    if (rc) return rc;
-  }
-  return ATOM_OK;
+  args.b_scale = (const __half*)b_scale_qkv; args.b_keeper_scale = (const __half*)b_keeper_scale_qkv;
+  args.M = (int)M; args.N = (int)N; args.G = (int)(K / 128 - 1); args.lda_scale = atom::scale_size((int)M); args.trace = g_trace;
+  args.ldb_scale = (int)N; args.seg_tiles = (int)(H / 128);
+  args.d = (__half*)q; args.d4 = (uint8_t*)k; args.d_scale = (__half2*)k_scale; args.d4_v = (uint8_t*)v; args.d_scale_v = (__half2*)v_scale;
+  return gemm_dispatch<atom::EPI_QKV>(op, args, flags, (cudaStream_t)stream);
 }
 
 int atom_gemm_i4_gateup_act(const void* a, const void* b_gu, const void* a_scale, const void* b_scale_gu, const void* a_keeper,
                             const void* b_keeper_gu, const void* a_keeper_scale, const void* b_keeper_scale_gu, void* o_outliers,
                             void* o_norms, void* outlier_scales, void* norm_scales, int64_t M, int64_t I, int64_t K, uint32_t flags,
                             void* stream) {
-  (void)flags;
   ATOM_REQUIRE(a && b_gu && a_scale && b_scale_gu && a_keeper && b_keeper_gu && a_keeper_scale && b_keeper_scale_gu && o_outliers &&
                o_norms && outlier_scales && norm_scales, "gemm_i4_gateup_act: null pointer argument");
   ATOM_REQUIRE(M > 0 && I >= 256 && I % 128 == 0, "gemm_i4_gateup_act: M=%lld must be positive, I=%lld a multiple of 128 >= 256", (long long)M, (long long)I);
@@ -629,15 +434,12 @@ int atom_gemm_i4_gateup_act(const void* a, const void* b_gu, const void* a_scale
                                               "run the two projections and activate_fp16_i4 for M=%lld", (long long)M);
   GemmOperands op{a, b_gu, a_keeper, b_keeper_gu, M, 2 * I, K};
   atom::GemmArgs args{};
-  { const char* e = getenv("ATOM_B200_GU_MODE"); args.dbg = e ? atoi(e) : 0; }
   args.a_scale = (const __half*)a_scale; args.a_keeper_scale = (const __half*)a_keeper_scale;
   args.b_scale = (const __half*)b_scale_gu; args.b_keeper_scale = (const __half*)b_keeper_scale_gu;
   args.M = (int)M; args.N = (int)(2 * I); args.G = (int)(K / 128 - 1); args.lda_scale = atom::scale_size((int)M); args.trace = g_trace;
-  args.a4 = (const uint8_t*)a; args.a8 = (const int8_t*)a_keeper; args.ldb_scale = (int)(2 * I); args.gu_rows = (int)I;
+  args.ldb_scale = (int)(2 * I); args.gu_rows = (int)I;
   args.q8_out = (int8_t*)o_outliers; args.q4_out = (uint8_t*)o_norms; args.q8_scale = (__half*)outlier_scales; args.q4_scale = (__half*)norm_scales;
-  if (M <= 16) return launch_skinny<16, 2, atom::EPI_GATEUP>(op, args, (cudaStream_t)stream, I);
-  if (M <= 32) return launch_skinny<32, 2, atom::EPI_GATEUP>(op, args, (cudaStream_t)stream, I);
-  return launch_skinny<64, 2, atom::EPI_GATEUP>(op, args, (cudaStream_t)stream, I);
+  return gemm_dispatch<atom::EPI_GATEUP>(op, args, flags & ~(uint32_t)ATOM_GEMM_FORCE_TALL, (cudaStream_t)stream, I);
 }
 
 int atom_gemm_i4_o4(const void* a, const void* b, const void* a_scale, const void* b_scale, const void* a_keeper,

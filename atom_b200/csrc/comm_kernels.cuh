@@ -2,7 +2,7 @@
 //
 // The row-parallel projections (o_proj, down_proj) of a decode step leave an FP16 [batch, hidden] partial on every rank
 // (512 KiB at Llama-65B, batch 32) that must be summed across the ranks: a latency-bound collective (SURVEY.md 8e).
-// The reference has no multi-GPU code at all; round 1 called ncclAllReduce.  This kernel does the exchange itself, with
+// The reference has no multi-GPU code at all.  This kernel does the exchange itself, with
 // no flag round trip and no fence (Lamport-style: the payload is its own arrival signal):
 //   1. every CTA pushes its slice of the local partial into slot [e % 3][my rank] of EVERY rank's receive buffer (plain
 //      16-byte stores through the NVLink peer mappings: fire and forget).  Receive buffers are pre-filled with a sentinel
@@ -15,13 +15,11 @@
 // can write buffer e % 3 again only in call e + 3, which it reaches after my push of call e + 2, i.e. after I finished
 // call e; and buffer (e + 2) % 3 is not written by anybody before call e + 2, which every peer reaches only after my push
 // of call e + 1, i.e. after the reset of call e completed (kernel boundary).
-// An earlier revision (fence + one flag per peer + acquire spin) measured 24.6 us for 512 KiB over 8 GPUs against 31.6 us
-// for ncclAllReduce (profiles/r02_tp_check_n8.jsonl).
 // The two halves also exist fused into their neighbours (tp.py): the row-parallel decode GEMM pushes from its epilogue
-// (gemm_i4_skinny_sm100.cuh, GemmArgs::ar) and rmsnorm_quant_kernel reduces while it loads its row (quant_kernels.cuh);
-// the shared pieces live in ptx_sm100.cuh (ArArgs, ar_*).
+// (gemm_i4_sm90.cuh, GemmArgs::ar) and rmsnorm_quant_kernel reduces while it loads its row (quant_kernels.cuh);
+// the shared pieces live in ptx_sm90.cuh (ArArgs, ar_*).
 #pragma once
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 
 namespace atom {
 

@@ -8,7 +8,7 @@
 //   param f16 [pages][L][2][H][P][2]    (scale, zero);  x = nibble * scale - zero   (quantization.cuh:76)
 // K is stored pre-RoPE; RoPE(theta = 1e4) is applied to q at position len-1 and to k at its index.
 #pragma once
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 
 namespace atom {
 
@@ -67,7 +67,7 @@ append_kv_kernel(KvArgs kv, const uint8_t* __restrict__ k, const uint8_t* __rest
 // the bracket is advanced once per page by a constant rotation (FP32, kept in smem), e^{j t_lo theta} comes from a smem
 // table -- no transcendental per token (the reference evaluates __sincosf per element per token, decode.cuh:39-71).
 // The per-token arithmetic runs in packed half2: one LOP3 turns two nibbles into the halves (1024+n); HSUB2 makes them
-// exact; dequant and rotation are HFMA2 on nibble couples (j, j+4); the q.k products are accumulated in FP32 (FHFMA: FP16
+// exact; dequant and rotation are HFMA2 on nibble couples (j, j+4); the q.k products are accumulated in FP32 (FP16
 // inputs, exact product, FP32 sum); scores, softmax statistics, the page-level rescale and the output accumulators stay
 // FP32 (V is accumulated in half2 only within one page).  An
 // all-FP32 version of this kernel executed 75 M warp instructions per layer, 36 % of them nibble extraction/conversion.
@@ -104,11 +104,9 @@ __device__ __forceinline__ __half2 nib2x(uint32_t w, uint32_t w8, int q) {
   return __hsub2(*reinterpret_cast<const __half2*>(&u), __half2half2(__ushort_as_half(0x6400)));
 }
 
-// acc += a * b with FP16 inputs, an exact product and FP32 accumulation (one FHFMA; .H0 / .H1 operand selectors are free)
-__device__ __forceinline__ float fhfma(__half a, __half b, float acc) {
-  asm("fma.rn.f32.f16 %0, %1, %2, %0;" : "+f"(acc) : "h"(__half_as_ushort(a)), "h"(__half_as_ushort(b)));
-  return acc;
-}
+// acc += a * b with FP16 inputs, an exact product and FP32 accumulation: Hopper has no mixed-precision scalar FMA, so the
+// halves are widened first (the FP32 product of two halves is exact inside the fma, one rounding in all)
+__device__ __forceinline__ float fhfma(__half a, __half b, float acc) { return fmaf(__half2float(a), __half2float(b), acc); }
 
 // kMaxTpl: tokens per lane per page = P / 8 <= kMaxTpl.  kP: page size as a compile-time constant (16 / 32: the sizes the harness
 // uses -- all table strides and the token loops become immediates) or 0 = read it from the arguments.

@@ -12,10 +12,10 @@
 // all later query tiles of its prompt; prefill_attn_kernel is the attention proper.
 // Tiling: CTA = 64 query rows of one (prompt, head), 4 warps x 16 rows; K/V in 64-token tiles through shared memory
 // (K row-major [token][dim], V transposed [dim][token] so both B fragments are contiguous 32-bit loads, padded
-// pitches => conflict-free).  The MMA is mma.sync.m16n8k16 (the warp-level tensor path); a tcgen05 variant (S tile in
-// tensor memory) is the next step for this kernel (DESIGN.md).
+// pitches => conflict-free).  The MMA is mma.sync.m16n8k16 (the warp-level tensor path); a wgmma variant is the
+// next step for this kernel.
 #pragma once
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 
 namespace atom {
 

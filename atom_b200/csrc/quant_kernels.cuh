@@ -8,7 +8,7 @@
 // 11008, and the work decomposition is one warp per 128-channel quantisation group: a lane owns 4 consecutive
 // reordered channels, so INT4 output is one coalesced 64-B warp store and INT8 one 128-B store.
 #pragma once
-#include "gemm_i4_sm100.cuh"  // scale_index / scale_size
+#include "gemm_i4_sm90.cuh"  // scale_index / scale_size
 
 namespace atom {
 

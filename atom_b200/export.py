@@ -1,6 +1,6 @@
 """Simulated (model/) layer -> real-INT4 serving layer (e2e/).  No reference equivalent: the reference's e2e harness runs
 random INT4 weights (e2e/README.md) and its accuracy simulator never leaves FP16; this module is the missing bridge, so
-a layer calibrated with the model/ surface (QLlamaDecoderLayer) can be served by the sm_100a kernels.
+a layer calibrated with the model/ surface (QLlamaDecoderLayer) can be served by the sm_90a kernels.
 
 Operand conventions are the kernels' (include/atom_b200.h; e2e/punica-atom/punica/models/llama.py:35-58):
   weight_int4 u8 [out, (in-128)/2]   reordered input channel 2j in the low nibble of byte j

@@ -1,7 +1,7 @@
 """Paged INT4 KV cache: page pool, per-sequence page lists and the per-step page table.
 
 API-compatible with /root/reference/e2e/punica-atom/punica/utils/kvcache.py:6-127 (class, property and method names are
-what punica/models/llama.py and the benchmark harness touch), laid out for the B200 kernels:
+what punica/models/llama.py and the benchmark harness touch), laid out for the CUDA kernels:
 
     pool.buf    uint8   [pages, num_layers, 2 (K|V), num_heads, block_len, head_dim // 2]   two INT4 per byte
     pool.param  float16 [pages, num_layers, 2,       num_heads, block_len, 2]               (scale, zero): x = nibble*scale - zero

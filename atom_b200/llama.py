@@ -1,4 +1,4 @@
-"""Real-INT4 Llama layers on the B200 kernels -- the operator surface of
+"""Real-INT4 Llama layers on the CUDA kernels -- the operator surface of
 /root/reference/e2e/punica-atom/punica/models/llama.py:35-364 (LinearInt4, LlamaMLP, LlamaAttention, LlamaRMSNormInt4,
 LlamaDecoderLayer, LlamaModel, LlamaForCausalLM): same constructor arguments, parameter names / shapes and
 forward(hidden_states, blen, prefill_kv, decode_kv) contract, so the reference's bench_textgen harness can drive it.

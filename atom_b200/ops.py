@@ -1,5 +1,5 @@
 """Operator API -- mirrors /root/reference/e2e/punica-atom/punica/ops/__init__.py (names, argument order,
-output allocation and return tuples) on top of the sm_100a kernels in libatom_b200.so.
+output allocation and return tuples) on top of the sm_90a kernels in libatom_b200.so.
 
 Differences from the reference (all widening, none changes a result):
   * kernels run on torch's current CUDA stream (the reference uses the legacy default stream);
@@ -17,9 +17,9 @@ __all__ = [
 
 GEMM_AUTO, GEMM_NO_SPLITK, GEMM_FORCE_TALL, GEMM_FORCE_SKINNY = 0, 1, 2, 4
 GEMM_SPLITK2, GEMM_SPLITK4 = 16, 32
-GEMM_FORCE_WIDE, GEMM_NO_WIDE = 512, 1024   # prefill shapes: 128 x 256 tiles with the token operand in tensor memory / never
-GEMM_LEGACY_TALL = 256    # prefill shapes: the round-1 kernel, kept for A/B timing
-GEMM_LEGACY_SKINNY = 128  # decode shapes: the round-1 kernel, kept for A/B timing
+GEMM_FORCE_WIDE, GEMM_NO_WIDE = 512, 1024   # kernel selectors of earlier versions: accepted and ignored
+GEMM_LEGACY_TALL = 256    # kernel selector of earlier versions: accepted and ignored
+GEMM_LEGACY_SKINNY = 128  # kernel selector of earlier versions: accepted and ignored
 
 
 def _stream(t):

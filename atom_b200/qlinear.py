@@ -1,6 +1,6 @@
 """QLinearLayer -- the surface of /root/reference/model/qLinearLayer.py:16-86 (constructor, buffers `weight`/`bias`, `args`,
 `.quant()`, `.reorder()`, `.to()`, `.forward()`), plus the step the reference lacks: `.pack()` converts the quantised
-weight into the real-INT4 operands of the B200 GEMM, after which `forward()` runs
+weight into the real-INT4 operands of the W4A4 GEMM, after which `forward()` runs
     reorder_fp16_i4 (dynamic per-group activation quantise)  ->  dense_layer_gemm_i4_fp16
 on the GPU instead of F.linear on fake-quantised FP16 weights.
 

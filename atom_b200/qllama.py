@@ -14,7 +14,7 @@ the per-module sizes or a `.config` carrying them), so a transformers LlamaDecod
 ToyLlamaDecoderLayer below (used by the CPU tests -- there is no network for checkpoints) both work.
 
 `QLlamaDecoderLayer.to_int4()` is the bridge the reference does not have: it turns the simulated layer into the real
-INT4 serving layer (atom_b200.llama.LlamaDecoderLayer: fused norm+quantise, INT4 tcgen05 GEMMs, INT4 paged KV).
+INT4 serving layer (atom_b200.llama.LlamaDecoderLayer: fused norm+quantise, W4A4 wgmma GEMMs, INT4 paged KV).
 """
 import math
 from typing import Optional, Tuple

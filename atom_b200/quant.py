@@ -4,7 +4,7 @@ quantize_attn_{k,v}_wrapper :234-257, Quantizer :259-304), integer uniform-affin
 formats are out of scope, DESIGN.md section 7).
 
 In addition to the fake-quant ("quantise then dequantise") functions the reference has, `quantize_weight_int` returns the
-INTEGER codes and scales themselves: that is what `QLinearLayer.pack()` turns into the real-INT4 operands of the B200
+INTEGER codes and scales themselves: that is what `QLinearLayer.pack()` turns into the real-INT4 operands of the
 GEMM -- the bridge between model/ and e2e/ that the reference lacks.
 """
 from functools import partial

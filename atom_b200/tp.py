@@ -1,4 +1,4 @@
-"""Tensor parallelism for the W4A4 layers (BASELINE config #5: Llama-65B over 8 B200s).  NEW functionality: the reference
+"""Tensor parallelism for the W4A4 layers (BASELINE config #5: Llama-65B over 8 GPUs).  NEW functionality: the reference
 has no NCCL / torch.distributed code at all (SURVEY.md section 0.3), so there is nothing to be drop-in with; the layout
 follows Megatron: one process per GPU, column-parallel q/k/v/gate/up (no communication), row-parallel o_proj/down_proj
 followed by ONE all-reduce (NCCL over NVLink/NVSwitch) per column->row pair -- two per decoder layer.

@@ -2,7 +2,7 @@
 """bench.py -- the reference's headline benchmark (BASELINE.json configs[1]): gemm_i4_o16, M=16, N=K=4096,
 group 128, INT8 keeper 128, on synthetic random-quantised operands.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--m M]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--m M] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Besides the headline line this also reports, in the same JSON object:
@@ -13,12 +13,16 @@ Besides the headline line this also reports, in the same JSON object:
            layer INSIDE the timed region -> tokens/s at 80 layers (strong scaling: the work is fixed, N grows).
 
 One "step" = one pass of the hot path over one batch of synthetic input: `gemms_per_step` independent GEMM problems
-(distinct operand sets, together larger than the 126 MB L2, so every launch streams its weights from HBM), launched
+(distinct operand sets, together larger than the H100's 50 MB L2, so every launch streams its weights from HBM), launched
 back to back from one CUDA graph.  `value` = whole-job TOP/s with operands resident in HBM (OP = 2*M*N*K, the
 reference's convention, bench_dense_layer_gemm_i4_o16.cu:40-42); multi-GPU runs give every rank its own batch (weak
 scaling, no data-path collective: GEMM problems are independent units).  `e2e` = the same metric through the public
 operator (atom_b200.ops.dense_layer_gemm_i4_fp16) with HOST activations: per step one pinned H2D copy of the quantised
 activation tuple, the GEMM, and a D2H read of the FP16 result.
+
+--dump-outputs DIR writes what the timed path computed in its last step -- the FP16 results of the step's GEMMs, as float32
+[gemms_per_step, M, N] in DIR/gemm_i4_o16.npy (a fixed seeded sample of the flattened array when that exceeds 32 MB).  The
+operands are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -33,7 +37,11 @@ import torch
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-L2_BYTES = 126e6
+L2_BYTES = 50e6               # H100
+# NVIDIA's data sheet for the H100 SXM (700 W): the denominators of the roofline fractions.  A power-limited card clocks lower.
+H100_HBM_GBS = 3350.0
+H100_INT8_TOPS = 1979.0
+DUMP_MAX_BYTES = 32 << 20
 
 # BASELINE.md section 1: the reference's published bench_gemm_i4_o16 numbers (RTX 4090, figures/bench_gemm.png), TOP/s by M
 PUBLISHED_TOPS = {16: 20.079, 32: 38.334, 64: 78.997, 128: 151.281, 256: 312.242, 512: 546.035, 1024: 630.779,
@@ -48,7 +56,7 @@ def algorithmic_bytes(m, n, k):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / power limit / throttle reasons DURING the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -105,15 +113,6 @@ def cpu_baseline(m, n, k, budget_s=12.0):
             "sample": f"{it} forwards of the fake-quant W4A4 linear (fp32 torch, act quant + F.linear) at M={m}, N={n}, K={k} in {el:.1f} s"}
 
 
-def ncu_traffic(m):
-    """DRAM bytes per launch of the dominant kernel from the committed ncu capture (profiles/), or None."""
-    p = os.path.join(ROOT, "profiles", "ncu_summary.json")
-    try:
-        return json.load(open(p)).get(f"gemm_m{m}", {}).get("dram_bytes_per_launch")
-    except (OSError, ValueError):
-        return None
-
-
 def graph_time_us(fn, nsets, launches, reps, dev):
     """Median device time per launch: `launches` calls of fn(i) captured in one CUDA graph, replayed `reps` times."""
     st = torch.cuda.Stream(dev)
@@ -137,12 +136,11 @@ def graph_time_us(fn, nsets, launches, reps, dev):
     return ts[len(ts) // 2]
 
 
-def gemm_sweep(dev, peaks, ms=(16, 256, 1024, 4096), n=4096, k=4096):
+def gemm_sweep(dev, ms=(16, 256, 1024, 4096), n=4096, k=4096):
     """bench_gemm_i4_o16 axis: device time per GEMM (graph replay over operand sets larger than L2) and the roofline
-    fraction against min(HBM, tensor) with the measured denominators."""
+    fraction against min(HBM, tensor) with the data-sheet denominators."""
     from atom_b200 import ops, synth
-    hbm = peaks.get("hbm_gbs", 6650.0)
-    tc = 2.0 * peaks.get("bf16_tflops", 1590.0)
+    hbm, tc = H100_HBM_GBS, H100_INT8_TOPS
     out = []
     for m in ms:
         one = synth.gemm_operands(m, n, k, dev, seed=99 + m)
@@ -159,7 +157,7 @@ def gemm_sweep(dev, peaks, ms=(16, 256, 1024, 4096), n=4096, k=4096):
         out.append(rec)
         del sets
         torch.cuda.empty_cache()
-    return {"shape": f"N={n} K={k}", "peaks": {"hbm_gbs": hbm, "int8_tensor_tops": tc, "int8_peak_is": "2 x measured bf16 cuBLAS burst"},
+    return {"shape": f"N={n} K={k}", "peaks": {"hbm_gbs": hbm, "int8_tensor_tops": tc, "source": "H100 SXM data sheet (700 W)"},
             "points": out}
 
 
@@ -233,7 +231,7 @@ def tp_decode_layer(rank, world, dev, hidden=8192, inter=22016, heads=64, batch=
            "launch": f"one CUDA graph per step over {copies} chained layer copies ({(w_bytes + kv_bytes) * copies / 1e6:.0f} MB of weights + KV per rank > L2), "
                      "collectives captured inside, device time, max over ranks",
            "hbm_bytes_per_layer_per_rank": int(w_bytes + kv_bytes),
-           "hbm_frac": round((w_bytes + kv_bytes) / (us * 1e-6) * 1e-9 / 6573.2, 3)}
+           "hbm_frac": round((w_bytes + kv_bytes) / (us * 1e-6) * 1e-9 / H100_HBM_GBS, 3)}
     g = None                 # a captured NCCL graph must be gone before the communicator is torn down
     del mods, kvs
     torch.cuda.synchronize()
@@ -251,6 +249,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-sweep", action="store_true")
     ap.add_argument("--no-tp", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's results to DIR/<name>.npy")
     a = ap.parse_args()
     M, N, K = a.m, 4096, 4096
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
@@ -273,7 +272,7 @@ def main():
     if ref_mode:
         from oracle import ref_gpu as R
         if not R.available():
-            # no compiled reference on this box: time the CPU port instead (rank 0 only)
+            # no compiled reference here: time the CPU port instead (rank 0 only)
             if rank == 0:
                 cb = cpu_baseline(M, N, K, budget_s=20.0)
                 print(json.dumps({"impl": "reference", "metric": "gemm_i4_o16_throughput", "value": cb["value"], "unit": "TOP/s",
@@ -296,14 +295,14 @@ def main():
     stream = torch.cuda.default_stream(dev) if ref_mode else torch.cuda.Stream(dev)
 
     def run_batch():
+        """One step; returns the results a caller would receive (under graph capture: the buffers every replay fills)."""
         if ref_mode:   # the reference launches on the legacy default stream (GEMM.cuh:763): not capturable, plain loop
             for i in range(R_sets):
                 R.gemm_i4_o16(*sets[i], d=outs[i], sync=0)
-        else:
-            for i in range(R_sets):
-                ops.dense_layer_gemm_i4_fp16(*sets[i])
+            return outs
+        return [ops.dense_layer_gemm_i4_fp16(*sets[i]) for i in range(R_sets)]
 
-    graph = None
+    graph = step_outs = None
     with torch.cuda.stream(stream):
         run_batch()
         stream.synchronize()
@@ -311,15 +310,15 @@ def main():
         if not ref_mode:
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph, stream=stream):
-                run_batch()
+                step_outs = run_batch()
 
     launch_desc = "one CUDA graph replay per step" if graph is not None else "python loop on the legacy stream (reference launcher)"
 
     def step():
         if graph is not None:
             graph.replay()
-        else:
-            run_batch()
+            return step_outs
+        return run_batch()
 
     def barrier():
         if world > 1:
@@ -341,8 +340,9 @@ def main():
         barrier()
         w0 = time.perf_counter()
         e0.record(stream)
+        last = None
         for _ in range(a.steps):
-            step()
+            last = step()
         e1.record(stream)
         barrier()
         wall_ms = (time.perf_counter() - w0) * 1e3
@@ -351,6 +351,13 @@ def main():
         # of the host's wall clock between the two synchronising barriers; a large gap means they did not bracket the work
         assert ms >= 0.7 * wall_ms - 1.0, f"timing contract broken: events {ms:.3f} ms vs wall clock {wall_ms:.3f} ms"
     clocks = sampler.stop() if rank == 0 else None
+    if a.dump_outputs and rank == 0 and last is not None:
+        import numpy as np
+        os.makedirs(a.dump_outputs, exist_ok=True)
+        d = torch.stack([t.float() for t in last]).cpu().numpy()
+        if d.nbytes > DUMP_MAX_BYTES:
+            d = d.reshape(-1)[np.sort(np.random.default_rng(0).choice(d.size, DUMP_MAX_BYTES // 4, replace=False))]
+        np.save(os.path.join(a.dump_outputs, "gemm_i4_o16.npy"), d)
     t = torch.tensor([ms], device=dev)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -425,15 +432,10 @@ def main():
     assert ms_per_step * 1e3 / R_sets <= e2e_us_per_step * 1.05, \
         f"timing contract broken: {ms_per_step * 1e3 / R_sets:.2f} us per launch (events) > {e2e_us_per_step:.2f} us per e2e step"
 
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except (OSError, ValueError):
-        pass
     # ------------------------------------------------------------------ config #5: tensor-parallel decode layer (all ranks)
     tp_rec = None
     if not ref_mode and not a.no_tp:
-        graph = e2e_graphs = None          # the captured graphs reference the operand sets freed next
+        graph = e2e_graphs = step_outs = last = None          # the captured graphs reference the operand sets freed next
         del sets, outs
         torch.cuda.empty_cache()
         try:
@@ -449,33 +451,31 @@ def main():
     sweep = None
     if not ref_mode and not a.no_sweep:
         try:
-            sweep = gemm_sweep(dev, peaks)
+            sweep = gemm_sweep(dev)
         except Exception as e:  # noqa: BLE001
             sweep = {"error": str(e)[:300]}
     # ------------------------------------------------------------------ roofline of the dominant kernel
-    hbm_peak = peaks.get("hbm_gbs", 6650.0)
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    hbm_peak, peak_src = H100_HBM_GBS, "H100 SXM data sheet (700 W)"
     us_per_launch = ms_per_step * 1e3 / R_sets
     alg = algorithmic_bytes(M, N, K)
     # HBM-bound up to the crossover M*~200 (BASELINE.md section 2); tensor-bound above it
-    int8_peak_tops = 2.0 * peaks.get("bf16_tflops", 1590.0)
+    int8_peak_tops = H100_INT8_TOPS
     t_hbm, t_tc = alg / (hbm_peak * 1e9), op_count / (int8_peak_tops * 1e12)
     if t_hbm >= t_tc:
         ach = alg / (us_per_launch * 1e-6) * 1e-9
-        roof = {"bound": "hbm", "achieved": ach, "peak": hbm_peak, "unit": "GB/s", "frac": ach / hbm_peak, "traffic": ncu_traffic(M),
+        roof = {"bound": "hbm", "achieved": ach, "peak": hbm_peak, "unit": "GB/s", "frac": ach / hbm_peak,
                 "algorithmic_bytes_per_launch": alg, "us_per_launch": us_per_launch, "peak_source": peak_src}
     else:
         ach = op_count / (us_per_launch * 1e-6) * 1e-12
         roof = {"bound": "tensor", "achieved": ach, "peak": int8_peak_tops, "unit": "TOP/s", "frac": ach / int8_peak_tops,
-                "traffic": ncu_traffic(M), "us_per_launch": us_per_launch,
-                "peak_source": "2 x measured bf16 cuBLAS burst (INT8 tcgen05 = 2x bf16 rate; Blackwell has no INT4 MMA)"}
+                "us_per_launch": us_per_launch, "peak_source": peak_src + ", dense INT8 (Hopper's wgmma has no INT4 type)"}
     line = {
         "metric": "gemm_i4_o16_throughput", "value": value, "unit": "TOP/s", "n_gpus": a.gpus, "steps": a.steps, "warmup": max(a.warmup, 3),
         "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak",
-        "vs_baseline": (value / PUBLISHED_TOPS[M]) if M in PUBLISHED_TOPS else None, "dtype": "s4 x s4 -> s32 (via tcgen05 kind::i8), fp16 out",
+        "vs_baseline": (value / PUBLISHED_TOPS[M]) if M in PUBLISHED_TOPS else None, "dtype": "s4 x s4 -> s32 (via wgmma s8), fp16 out",
         "data": "synthetic", "impl": a.impl,
         "config": {"workload": f"gemm_i4_o16 M={M} N={N} K={K} (K incl. 128 INT8 keeper) group_size=128", "gemms_per_step": R_sets,
-                   "l2": f"{R_sets} distinct operand sets per step = {R_sets * per_set / 1e6:.0f} MB > 126 MB L2 (inputs larger than L2)",
+                   "l2": f"{R_sets} distinct operand sets per step = {R_sets * per_set / 1e6:.0f} MB > 50 MB L2 (inputs larger than L2)",
                    "launch": launch_desc,
                    "parallelism": f"dp{world} for the GEMM line (independent GEMM problems per rank, no collective); "
                                   f"tp{world} with two all-reduces per layer for the `tp` record",
@@ -488,7 +488,7 @@ def main():
     }
     if ref_mode:
         line["cpu_baseline"] = {"value": value, "unit": "TOP/s", "cores": 0, "kind": "reference",
-                                "sample": "the reference's own CUDA kernel (oracle/_ref, compiled unmodified for sm_100a) on this GPU; "
+                                "sample": "the reference's own CUDA kernel (oracle/_ref, compiled unmodified for sm_90a) on this GPU; "
                                           "its CPU path is the fake-quant simulator, see cpu_baseline of the main arm"}
         line["gpu_launches"] = 0   # none of OUR kernels ran in this arm
     elif world == 1 and not a.no_cpu_baseline:

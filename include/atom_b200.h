@@ -1,8 +1,8 @@
 /*
- * atom_b200.h -- C ABI of libatom_b200.so: the B200 (sm_100a) implementation of the efeslab/Atom W4A4 hot path.
+ * atom_b200.h -- C ABI of libatom_b200.so: the H100 (sm_90a) implementation of the efeslab/Atom W4A4 hot path.
  *
  * One entry point per function that the reference binds into Python through
- * pybind11 (/root/reference/e2e/punica-atom/punica/ops/csrc/punica_ops.cc:270-279).  Plain pointers and sizes only;
+ * pybind11 (e2e/punica-atom/punica/ops/csrc/punica_ops.cc:270-279 of the reference).  Plain pointers and sizes only;
  * every pointer is a DEVICE pointer owned by the caller, outputs are pre-allocated by the caller (exactly as
  * punica/ops/__init__.py:21-219 does with torch.empty) and the library keeps no reference to them.
  *
@@ -38,15 +38,16 @@ extern "C" {
 /* gemm flags */
 #define ATOM_GEMM_AUTO 0u
 #define ATOM_GEMM_NO_SPLITK 1u   /* bit-exact accumulation order (groups 0..G-1 then keeper) even for small M */
-#define ATOM_GEMM_FORCE_TALL 2u  /* tokens on the MMA-M axis regardless of M */
-#define ATOM_GEMM_FORCE_SKINNY 4u /* channels on the MMA-M axis (requires M <= 128 per tile; any M works) */
+#define ATOM_GEMM_FORCE_TALL 2u  /* 128-token tiles regardless of M; never splits K */
+#define ATOM_GEMM_FORCE_SKINNY 4u /* token tiles of at most 64 regardless of M */
 #define ATOM_GEMM_SPLITK2 16u     /* decode shapes: force a 2-way K split (default: chosen from the tile count) */
 #define ATOM_GEMM_SPLITK4 32u     /* decode shapes: force a 4-way K split */
-#define ATOM_GEMM_SPLITK8 64u     /* decode shapes, M <= 32: force an 8-way K split (cluster of 8) */
-#define ATOM_GEMM_FORCE_WIDE 512u    /* prefill shapes: 128 x 256 tiles, token operand in tensor memory (opt-in: measured slower than 128 x 128) */
-#define ATOM_GEMM_NO_WIDE 1024u      /* prefill shapes: always 128 x 128 tiles (the default; kept for callers that pass it) */
-#define ATOM_GEMM_LEGACY_TALL 256u   /* prefill shapes: the round-1 kernel (I2F + FFMA epilogue), kept for A/B timing */
-#define ATOM_GEMM_LEGACY_SKINNY 128u /* decode shapes: the round-1 kernel (weights expanded into shared memory), kept for A/B timing */
+#define ATOM_GEMM_SPLITK8 64u     /* force an 8-way K split (cluster of 8) */
+/* kernel selectors of earlier versions: accepted for callers that pass them, ignored (there is one GEMM kernel) */
+#define ATOM_GEMM_FORCE_WIDE 512u
+#define ATOM_GEMM_NO_WIDE 1024u
+#define ATOM_GEMM_LEGACY_TALL 256u
+#define ATOM_GEMM_LEGACY_SKINNY 128u
 
 ATOM_API int atom_version(void);
 ATOM_API const char* atom_last_error(void);
@@ -103,8 +104,8 @@ ATOM_API int atom_gemm_i4_o4(const void* a, const void* b, const void* a_scale, 
  * (punica/models/llama.py:146-156: dense_layer_gemm_i4_fp16 for q, dense_layer_gemm_i4_o4 for k and v, same input) as ONE
  * launch over row-concatenated weights  b_qkv u8 [3H,(K-128)/2], b_scale_qkv f16 [K/128-1, 3H], b_keeper_qkv i8 [3H,128],
  * b_keeper_scale_qkv f16 [3H]  (rows [0,H) = q, [H,2H) = k, [2H,3H) = v).  Outputs are bit-identical to the three separate
- * calls: q f16 [M,H]; k, v u8 [M,H/2] with k_scale, v_scale f16 [M,H/128,2].  M <= 64: one decode-kernel launch whose
- * channel tile selects the epilogue; larger M: three launches on the row slices. */
+ * calls: q f16 [M,H]; k, v u8 [M,H/2] with k_scale, v_scale f16 [M,H/128,2].  One launch whose channel tile selects the
+ * epilogue. */
 ATOM_API int atom_gemm_i4_qkv(const void* a, const void* b_qkv, const void* a_scale, const void* b_scale_qkv, const void* a_keeper,
                      const void* b_keeper_qkv, const void* a_keeper_scale, const void* b_keeper_scale_qkv, void* q, void* k,
                      void* k_scale, void* v, void* v_scale, int64_t M, int64_t H, int64_t K, uint32_t flags, void* stream);
@@ -121,10 +122,10 @@ ATOM_API int atom_gemm_i4_gateup_act(const void* a, const void* b_gu, const void
                             void* stream);
 
 /* Debug aid (no reference counterpart): when non-NULL, every GEMM CTA writes 128 clock64() stamps of its pipeline
- * stages to device_buffer[cta*128 ...] (layout in gemm_i4_sm100.cuh).  NULL switches tracing off. */
+ * phases to device_buffer[cta*128 ...] (layout in gemm_i4_sm90.cuh).  NULL switches tracing off. */
 ATOM_API int atom_gemm_set_trace(void* device_buffer);
 
-/* EXPERIMENTAL (no reference counterpart; not yet run on hardware): programmatic dependent launch.  When enabled (also via
+/* EXPERIMENTAL (no reference counterpart): programmatic dependent launch.  When enabled (also via
  * ATOM_B200_PDL=1 in the environment) every kernel is launched with programmatic stream serialization: its prologue -- for
  * the GEMM including the first weight tiles -- overlaps the tail of the preceding kernel; everything that reads that
  * kernel's output waits on griddepcontrol.wait.  Results are unchanged.  Off by default. */

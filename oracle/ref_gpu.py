@@ -1,5 +1,5 @@
 """ctypes front-end of oracle/_ref/libatom_ref.so: the REFERENCE's own CUDA kernels, compiled unmodified from
-/root/reference by oracle/Makefile for sm_100a.  TEST / BENCH INFRASTRUCTURE ONLY (live GPU oracle and the
+the reference tree by oracle/Makefile for sm_90a.  TEST / BENCH INFRASTRUCTURE ONLY (live GPU oracle and the
 `--impl reference` timing arm); never imported by atom_b200/.
 
 All launches go to the legacy default stream, as in the reference (Reorder.cuh:219, GEMM.cuh:763).

@@ -1,4 +1,4 @@
-"""Regenerates tests/golden/*.npz from the reference tree (build container only).
+"""Regenerates tests/golden/*.npz from the reference tree (needs the reference tree: ATOM_REFERENCE).
 
 Two sources, both the reference's own code, neither copied into this repo:
   * the CPU golden functions of test_Reorder.cu / test_RMSNorm.cu / test_activate.cu
@@ -19,7 +19,7 @@ CSRC = os.path.join(REF, "e2e/punica-atom/punica/ops/csrc")
 def cpp_golden(kind, seq_len, hidden):
     tmp = tempfile.mkdtemp()
     exe, out = os.path.join(tmp, "gen"), os.path.join(tmp, "out.bin")
-    subprocess.check_call(["nvcc", "-w", "-O1", "-std=c++17", "-arch=sm_100a", f"-DGEN_{kind.upper()}",
+    subprocess.check_call(["nvcc", "-w", "-O1", "-std=c++17", "-arch=sm_90a", f"-DGEN_{kind.upper()}",
                            f"-I{CSRC}", os.path.join(HERE, "gen_ref_golden.cu"), "-o", exe])
     subprocess.check_call([exe, str(seq_len), str(hidden), out])
     raw = open(out, "rb").read()

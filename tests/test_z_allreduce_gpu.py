@@ -3,7 +3,7 @@ so the full protocol runs (push into slot [e % 3][0], reset of the previous buff
 call counter) and the result must equal the input bit for bit (-0.0 arrives as +0.0) -- eagerly, with sizes that grow and
 shrink between calls and leave CTAs without work, and across CUDA-graph replays (the buffer rotation is driven by the
 device-side counter).  The N >= 2 behaviour is covered by tools/tp_check.py under torchrun
-(profiles/r02_tp_check_n{2,8}.jsonl) and the host logic by tests/test_tp_gloo.py."""
+(several GPUs) and the host logic by tests/test_tp_gloo.py."""
 import pytest
 import torch
 

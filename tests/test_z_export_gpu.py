@@ -1,5 +1,5 @@
 """GPU suite (-m gpu), sorted last on purpose: a layer calibrated with the model/ surface (QLlamaDecoderLayer: reorder ->
-RTN quantise -> activation quantisers), exported with .to_int4(), must give on the sm_100a kernels what the oracle's
+RTN quantise -> activation quantisers), exported with .to_int4(), must give on the sm_90a kernels what the oracle's
 restatement of the kernel chain gives on the same exported operands, and stay within quantisation noise of the simulator."""
 import numpy as np
 import pytest

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """CLI of the continuous-batching harness: the reference's `python -m benchmarks.bench_textgen --system punica`
-(e2e/punica-atom/benchmarks/bench_textgen.py:488-528) on the B200 kernels.  Same flags, same request set, same report
+(e2e/punica-atom/benchmarks/bench_textgen.py:488-528) on the H100 kernels.  Same flags, same request set, same report
 lines, plus one JSON line.  Random INT4 weights of the named architecture (the reference's e2e run does the same,
 e2e/README.md), synthetic token ids.  Needs a GPU; there is no CPU path.
 

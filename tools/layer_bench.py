@@ -1,6 +1,6 @@
 """Decode-step timing of one W4A4 Llama decoder layer (BASELINE configs #3 / #4), one CUDA graph per step.
 python tools/layer_bench.py [--hidden 4096 --inter 11008 --heads 32 --batch 16 --kvlen 2048 --layers 32]
-Prints JSON: us per layer-step, tokens/s extrapolated to `layers` layers, per-kernel shares when run under ncu."""
+Prints JSON: us per layer-step, tokens/s extrapolated to `layers` layers."""
 import argparse, json, os, sys
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -53,4 +53,4 @@ kv_bytes = a.batch * a.heads * (a.kvlen + 1) * 136
 print(json.dumps({"layer_decode_step": {"hidden": a.hidden, "inter": a.inter, "heads": a.heads, "batch": a.batch, "kv_len": a.kvlen},
                   "us_per_layer": round(us, 2), "tokens_per_s_at_layers": {str(a.layers): round(a.batch / (us * a.layers * 1e-6), 1)},
                   "hbm_bytes_per_layer": int(w_bytes + kv_bytes), "hbm_GBps": round((w_bytes + kv_bytes) / us * 1e-3, 1),
-                  "frac_of_measured_hbm_6573": round((w_bytes + kv_bytes) / us * 1e-3 / 6573.2, 3)}))
+                  "frac_of_h100_datasheet_hbm_3350": round((w_bytes + kv_bytes) / us * 1e-3 / 3350.0, 3)}))
