@@ -23,11 +23,14 @@ _SIGNATURES = {
     "atom_gemm_i4_o16": (_I, [_P] * 9 + [_I64, _I64, _I64, _U32, _P]),
     "atom_gemm_i4_o4": (_I, [_P] * 10 + [_I64, _I64, _I64, _U32, _P]),
     "atom_gemm_i4_qkv": (_I, [_P] * 13 + [_I64, _I64, _I64, _U32, _P]),
+    "atom_gemm_i4_qkv_gqa": (_I, [_P] * 13 + [_I64, _I64, _I64, _I64, _U32, _P]),
     "atom_gemm_i4_gateup_act": (_I, [_P] * 12 + [_I64, _I64, _I64, _U32, _P]),
     "atom_gemm_set_trace": (_I, [_P]),
     "atom_set_pdl": (_I, [_I]),
     "atom_batch_decode_i4": (_I, [_P] * 7 + [_I] * 5 + [_P]),
+    "atom_batch_decode_gqa_i4": (_I, [_P] * 7 + [_I] * 6 + [_F, _P]),
     "atom_prefill_attention_i4": (_I, [_P] * 11 + [_I] * 4 + [_P]),
+    "atom_prefill_attention_gqa_i4": (_I, [_P] * 11 + [_I] * 5 + [_P]),
     "atom_allreduce_push_f16": (_I, [_P] * 4 + [_I64, _I64, _I, _I, _P]),
     "atom_allreduce_state_words": (_I, []),
     "atom_gemm_i4_o16_push": (_I, [_P] * 10 + [_I64, _I, _I, _I64, _I64, _I64, _U32, _P]),

@@ -4,7 +4,8 @@ only ever runs random weights and its simulator never leaves FP16).
 One `.safetensors` file holding the module's state_dict verbatim -- for every LinearInt4 the four kernel operands
 (`weight_int4` u8, `weight_int8` i8, `scale_int4` f16, `scale_int8` f16, shapes as punica/models/llama.py:44-58), the fp16
 norm weights, the int16 reorder indices, and for a full model the embedding / lm_head -- plus a JSON header in the file
-metadata: format tag, the LlamaConfig fields and which class was saved.  Loading rebuilds the module on the meta device
+metadata: format tag, the LlamaConfig fields and which class was saved (files written before `num_key_value_heads` /
+`rope_theta` joined the config lack them and load with the defaults: multi-head attention, base 1e4).  Loading rebuilds the module on the meta device
 and assigns the tensors (no random init, no second copy), so a 65B shard loads at file-read speed.
 """
 import dataclasses
@@ -25,7 +26,9 @@ def _config_of(module) -> LlamaConfig:
         at = module.self_attn
         c = LlamaConfig(hidden_size=at.hidden_size, intermediate_size=module.mlp.intermediate_size,
                         num_attention_heads=at.num_heads, num_hidden_layers=1,
-                        rms_norm_eps=module.input_layernorm.variance_epsilon)
+                        rms_norm_eps=module.input_layernorm.variance_epsilon,
+                        num_key_value_heads=None if at.num_kv_heads == at.num_heads else at.num_kv_heads,
+                        rope_theta=at.rope_theta)
     fields = {f.name for f in dataclasses.fields(LlamaConfig)}
     return LlamaConfig(**{k: getattr(c, k) for k in fields if hasattr(c, k)})
 

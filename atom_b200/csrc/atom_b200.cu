@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdarg>
 #include <cstdlib>
 #include <cstdio>
@@ -397,26 +398,47 @@ int atom_gemm_i4_o16_push(const void* a, const void* b, const void* a_scale, con
                      stream, false, &ar);
 }
 
-int atom_gemm_i4_qkv(const void* a, const void* b_qkv, const void* a_scale, const void* b_scale_qkv, const void* a_keeper,
-                     const void* b_keeper_qkv, const void* a_keeper_scale, const void* b_keeper_scale_qkv, void* q, void* k,
-                     void* k_scale, void* v, void* v_scale, int64_t M, int64_t H, int64_t K, uint32_t flags, void* stream) {
+// q rows [0, Hq), k rows [Hq, Hq + Hkv), v the rest: one launch, (Hq + 2 Hkv) / 128 channel tiles, the tile index selects the
+// epilogue (q: FP16, k / v: asymmetric INT4 per head)
+static int gemm_qkv(const char* what, const void* a, const void* b_qkv, const void* a_scale, const void* b_scale_qkv, const void* a_keeper,
+                    const void* b_keeper_qkv, const void* a_keeper_scale, const void* b_keeper_scale_qkv, void* q, void* k,
+                    void* k_scale, void* v, void* v_scale, int64_t M, int64_t Hq, int64_t Hkv, int64_t K, uint32_t flags, void* stream) {
   ATOM_REQUIRE(a && b_qkv && a_scale && b_scale_qkv && a_keeper && b_keeper_qkv && a_keeper_scale && b_keeper_scale_qkv && q && k &&
-               k_scale && v && v_scale, "gemm_i4_qkv: null pointer argument");
-  ATOM_REQUIRE(M > 0 && H > 0 && H % 128 == 0, "gemm_i4_qkv: M=%lld must be positive, H=%lld a positive multiple of 128", (long long)M, (long long)H);
-  ATOM_REQUIRE(K >= 256 && K % 128 == 0, "gemm_i4_qkv: K=%lld must be a multiple of 128 and >= 256", (long long)K);
+               k_scale && v && v_scale, "%s: null pointer argument", what);
+  ATOM_REQUIRE(K >= 256 && K % 128 == 0, "%s: K=%lld must be a multiple of 128 and >= 256", what, (long long)K);
   ATOM_REQUIRE(aligned16(a) && aligned16(b_qkv) && aligned16(a_keeper) && aligned16(b_keeper_qkv) && aligned16(q) && aligned16(b_scale_qkv) &&
-               aligned16(b_keeper_scale_qkv), "gemm_i4_qkv: operand pointers must be 16-byte aligned");
-  ATOM_REQUIRE(M < (1ll << 31) && 3 * H < (1ll << 31) && K < (1ll << 24), "gemm_i4_qkv: dimension too large");
-  const int64_t N = 3 * H;
-  // one launch: 3H/128 channel tiles, the tile index selects the epilogue (q: FP16, k / v: asymmetric INT4 per head)
+               aligned16(b_keeper_scale_qkv), "%s: operand pointers must be 16-byte aligned", what);
+  const int64_t N = Hq + 2 * Hkv;
+  ATOM_REQUIRE(M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 24), "%s: dimension too large", what);
   GemmOperands op{a, b_qkv, a_keeper, b_keeper_qkv, M, N, K};
   atom::GemmArgs args{};
   args.a_scale = (const __half*)a_scale; args.a_keeper_scale = (const __half*)a_keeper_scale;
   args.b_scale = (const __half*)b_scale_qkv; args.b_keeper_scale = (const __half*)b_keeper_scale_qkv;
   args.M = (int)M; args.N = (int)N; args.G = (int)(K / 128 - 1); args.lda_scale = atom::scale_size((int)M); args.trace = g_trace;
-  args.ldb_scale = (int)N; args.seg_tiles = (int)(H / 128);
+  args.ldb_scale = (int)N; args.seg_tiles = (int)(Hq / 128); args.kv_tiles = (int)(Hkv / 128);
   args.d = (__half*)q; args.d4 = (uint8_t*)k; args.d_scale = (__half2*)k_scale; args.d4_v = (uint8_t*)v; args.d_scale_v = (__half2*)v_scale;
   return gemm_dispatch<atom::EPI_QKV>(op, args, flags, (cudaStream_t)stream);
+}
+
+int atom_gemm_i4_qkv(const void* a, const void* b_qkv, const void* a_scale, const void* b_scale_qkv, const void* a_keeper,
+                     const void* b_keeper_qkv, const void* a_keeper_scale, const void* b_keeper_scale_qkv, void* q, void* k,
+                     void* k_scale, void* v, void* v_scale, int64_t M, int64_t H, int64_t K, uint32_t flags, void* stream) {
+  ATOM_REQUIRE(M > 0 && H > 0 && H % 128 == 0, "gemm_i4_qkv: M=%lld must be positive, H=%lld a positive multiple of 128", (long long)M, (long long)H);
+  return gemm_qkv("gemm_i4_qkv", a, b_qkv, a_scale, b_scale_qkv, a_keeper, b_keeper_qkv, a_keeper_scale, b_keeper_scale_qkv, q, k, k_scale,
+                  v, v_scale, M, H, H, K, flags, stream);
+}
+
+int atom_gemm_i4_qkv_gqa(const void* a, const void* b_qkv, const void* a_scale, const void* b_scale_qkv, const void* a_keeper,
+                         const void* b_keeper_qkv, const void* a_keeper_scale, const void* b_keeper_scale_qkv, void* q, void* k,
+                         void* k_scale, void* v, void* v_scale, int64_t M, int64_t Hq_dim, int64_t Hkv_dim, int64_t K, uint32_t flags,
+                         void* stream) {
+  ATOM_REQUIRE(M > 0 && Hq_dim > 0 && Hq_dim % 128 == 0 && Hkv_dim > 0 && Hkv_dim % 128 == 0,
+               "gemm_i4_qkv_gqa: M=%lld must be positive, Hq_dim=%lld and Hkv_dim=%lld positive multiples of 128", (long long)M,
+               (long long)Hq_dim, (long long)Hkv_dim);
+  ATOM_REQUIRE(Hq_dim % Hkv_dim == 0, "gemm_i4_qkv_gqa: Hq_dim=%lld must be a multiple of Hkv_dim=%lld (whole query heads per KV head)",
+               (long long)Hq_dim, (long long)Hkv_dim);
+  return gemm_qkv("gemm_i4_qkv_gqa", a, b_qkv, a_scale, b_scale_qkv, a_keeper, b_keeper_qkv, a_keeper_scale, b_keeper_scale_qkv, q, k,
+                  k_scale, v, v_scale, M, Hq_dim, Hkv_dim, K, flags, stream);
 }
 
 int atom_gemm_i4_gateup_act(const void* a, const void* b_gu, const void* a_scale, const void* b_scale_gu, const void* a_keeper,
@@ -449,27 +471,44 @@ int atom_gemm_i4_o4(const void* a, const void* b, const void* a_scale, const voi
                      flags, stream, true);
 }
 
-int atom_prefill_attention_i4(const void* q, const void* k, const void* k_param, const void* v, const void* v_param,
-                              const void* seqlen_indptr, const void* pos_of_token, const void* rope_table, void* k_f16, void* v_f16,
-                              void* out, int total_tokens, int batch_size, int max_len, int num_heads, void* stream) {
+static int prefill_attention(const char* what, const void* q, const void* k, const void* k_param, const void* v, const void* v_param,
+                             const void* seqlen_indptr, const void* pos_of_token, const void* rope_table, void* k_f16, void* v_f16,
+                             void* out, int total_tokens, int batch_size, int max_len, int num_heads, int num_kv_heads, void* stream) {
   ATOM_REQUIRE(q && k && k_param && v && v_param && seqlen_indptr && pos_of_token && rope_table && k_f16 && v_f16 && out,
-               "prefill_attention_i4: null pointer argument");
-  ATOM_REQUIRE(batch_size > 0 && num_heads > 0 && max_len > 0, "prefill_attention_i4: batch_size=%d num_heads=%d max_len=%d must be positive",
+               "%s: null pointer argument", what);
+  ATOM_REQUIRE(batch_size > 0 && num_heads > 0 && max_len > 0, "%s: batch_size=%d num_heads=%d max_len=%d must be positive", what,
                batch_size, num_heads, max_len);
+  ATOM_REQUIRE(num_kv_heads > 0 && num_heads % num_kv_heads == 0, "%s: num_q_heads=%d must be a positive multiple of num_kv_heads=%d", what,
+               num_heads, num_kv_heads);
   ATOM_REQUIRE(aligned16(q) && aligned16(k) && aligned16(v) && aligned16(k_f16) && aligned16(v_f16) && aligned16(out),
-               "prefill_attention_i4: pointers must be 16-byte aligned");
+               "%s: pointers must be 16-byte aligned", what);
   if (total_tokens <= 0) return ATOM_OK;
-  const long long th = (long long)total_tokens * num_heads;
+  const long long th = (long long)total_tokens * num_kv_heads;
   atom::kv_dequant_rope_kernel<<<(unsigned)((th + 3) / 4), 256, 0, (cudaStream_t)stream>>>(
       (const uint8_t*)k, (const __half2*)k_param, (const uint8_t*)v, (const __half2*)v_param, (const int32_t*)pos_of_token,
-      (const float2*)rope_table, (__half*)k_f16, (__half*)v_f16, th, num_heads);
+      (const float2*)rope_table, (__half*)k_f16, (__half*)v_f16, th, num_kv_heads);
   int rc = check_launch("prefill_attention_i4 (dequant + RoPE)");
   if (rc) return rc;
   const dim3 grid((unsigned)((max_len + atom::PF_BQ - 1) / atom::PF_BQ), (unsigned)batch_size, (unsigned)num_heads);
   atom::prefill_attn_kernel<<<grid, atom::PF_THREADS, 0, (cudaStream_t)stream>>>(
       (const __half*)q, (const __half*)k_f16, (const __half*)v_f16, (const int32_t*)seqlen_indptr, (const float2*)rope_table,
-      (__half*)out, num_heads, 0.08838834764831845f * 1.4426950408889634f);
-  return check_launch("prefill_attention_i4");
+      (__half*)out, num_heads, num_kv_heads, 0.08838834764831845f * 1.4426950408889634f);
+  return check_launch(what);
+}
+
+int atom_prefill_attention_i4(const void* q, const void* k, const void* k_param, const void* v, const void* v_param,
+                              const void* seqlen_indptr, const void* pos_of_token, const void* rope_table, void* k_f16, void* v_f16,
+                              void* out, int total_tokens, int batch_size, int max_len, int num_heads, void* stream) {
+  return prefill_attention("prefill_attention_i4", q, k, k_param, v, v_param, seqlen_indptr, pos_of_token, rope_table, k_f16, v_f16, out,
+                           total_tokens, batch_size, max_len, num_heads, num_heads, stream);
+}
+
+int atom_prefill_attention_gqa_i4(const void* q, const void* k, const void* k_param, const void* v, const void* v_param,
+                                  const void* seqlen_indptr, const void* pos_of_token, const void* rope_table, void* k_f16, void* v_f16,
+                                  void* out, int total_tokens, int batch_size, int max_len, int num_q_heads, int num_kv_heads,
+                                  void* stream) {
+  return prefill_attention("prefill_attention_gqa_i4", q, k, k_param, v, v_param, seqlen_indptr, pos_of_token, rope_table, k_f16, v_f16,
+                           out, total_tokens, batch_size, max_len, num_q_heads, num_kv_heads, stream);
 }
 
 int atom_allreduce_push_f16(const void* in, void* out, const void* peer_buffers, void* state, int64_t numel, int64_t slot_elems,
@@ -517,6 +556,50 @@ int atom_batch_decode_i4(void* o, const void* q, const void* kv_data, const void
   if (page_size <= 32) ATOM_DECODE(4, 0);
   ATOM_DECODE(8, 0);
 #undef ATOM_DECODE
+}
+
+int atom_batch_decode_gqa_i4(void* o, const void* q, const void* kv_data, const void* kv_param, const void* kv_indptr,
+                             const void* kv_indices, const void* last_page_offset, int num_layers, int layer_idx,
+                             int num_q_heads, int num_kv_heads, int page_size, int batch_size, float rope_theta, void* stream) {
+  int rc = kv_check("batch_decode_gqa_i4", kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx,
+                    num_kv_heads, page_size, batch_size);
+  if (rc) return rc;
+  ATOM_REQUIRE(o && q, "batch_decode_gqa_i4: null q/o");
+  ATOM_REQUIRE(num_q_heads > 0 && num_q_heads % num_kv_heads == 0,
+               "batch_decode_gqa_i4: num_q_heads=%d must be a positive multiple of num_kv_heads=%d", num_q_heads, num_kv_heads);
+  ATOM_REQUIRE(rope_theta > 1.f && rope_theta < 1e30f, "batch_decode_gqa_i4: rope_theta=%g must be a finite base above 1", (double)rope_theta);
+  const int group = num_q_heads / num_kv_heads;
+  // multi-head attention with the reference's RoPE base: the kernel every existing caller runs, untouched
+  if (group == 1 && rope_theta == 10000.f)
+    return atom_batch_decode_i4(o, q, kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx, num_kv_heads,
+                                page_size, batch_size, stream);
+  if (group != 1 && group != 2 && group != 4 && group != 8)
+    return fail(ATOM_E_UNSUPPORTED, "batch_decode_gqa_i4: %d query heads per KV head (num_q_heads=%d, num_kv_heads=%d); supported group "
+                                    "sizes are 1, 2, 4 and 8", group, num_q_heads, num_kv_heads);
+  ATOM_REQUIRE(page_size % 8 == 0 && page_size <= 64, "batch_decode_gqa_i4: page_size=%d must be a multiple of 8, at most 64", page_size);
+  ATOM_REQUIRE(aligned16(kv_data) && aligned16(kv_param), "batch_decode_gqa_i4: KV pool must be 16-byte aligned");
+  atom::KvArgs kv{(uint8_t*)kv_data, (__half2*)kv_param, (const int32_t*)kv_indptr, (const int32_t*)kv_indices,
+                  (const int32_t*)last_page_offset, num_layers, layer_idx, num_kv_heads, page_size, batch_size};
+  const size_t smem = atom::batch_decode_gqa_smem_bytes(page_size);
+  const float log2_theta = log2f(rope_theta);
+#define ATOM_DECODE_GQA(G_, TPL, PG)                                                                                         \
+  do {                                                                                                                       \
+    if ((rc = ensure_dynamic_smem(atom::batch_decode_gqa_kernel<G_, TPL, PG>, 100 * 1024, "batch_decode_gqa_i4"))) return rc; \
+    return launch_k("batch_decode_gqa_i4", atom::batch_decode_gqa_kernel<G_, TPL, PG>, dim3(batch_size, num_kv_heads),       \
+                    dim3(atom::GQA_THREADS), smem, (cudaStream_t)stream, (__half*)o, (const __half*)q, kv, log2_theta);      \
+  } while (0)
+#define ATOM_DECODE_GQA_P(G_)                    \
+  do {                                           \
+    if (page_size == 16) ATOM_DECODE_GQA(G_, 2, 16); \
+    if (page_size == 32) ATOM_DECODE_GQA(G_, 4, 32); \
+    ATOM_DECODE_GQA(G_, 8, 0);                   \
+  } while (0)
+  if (group == 1) ATOM_DECODE_GQA(1, 8, 0);       // multi-head attention with another RoPE base: eight page stripes, any page size
+  if (group == 2) ATOM_DECODE_GQA_P(2);
+  if (group == 4) ATOM_DECODE_GQA_P(4);
+  ATOM_DECODE_GQA_P(8);
+#undef ATOM_DECODE_GQA_P
+#undef ATOM_DECODE_GQA
 }
 
 int atom_append_kv_i4(void* kv_data, void* kv_param, const void* kv_indptr, const void* kv_indices,

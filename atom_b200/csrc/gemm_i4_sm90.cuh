@@ -36,9 +36,9 @@ struct GemmArgs {
   __half* d;                     // o16: [M][N]
   uint8_t* d4;                   // o4 : [M][N/2]
   __half2* d_scale;              // o4 : [M][N/128] (scale, zero)
-  uint8_t* d4_v;                 // fused q/k/v projection (EPI_QKV): channel tiles [0, seg_tiles) are q -> d (o16),
-  __half2* d_scale_v;            //   [seg_tiles, 2 seg_tiles) are k -> d4 / d_scale (o4), the rest v -> d4_v / d_scale_v (o4)
-  int seg_tiles;
+  uint8_t* d4_v;                 // fused q/k/v projection (EPI_QKV): channel tiles [0, seg_tiles) are q -> d (o16), the next
+  __half2* d_scale_v;            //   kv_tiles are k -> d4 / d_scale (o4), the last kv_tiles v -> d4_v / d_scale_v (o4)
+  int seg_tiles, kv_tiles;       //   (multi-head attention: kv_tiles == seg_tiles; grouped-query: fewer KV heads)
   // fused gate/up projection + SiLU(gate)*up + dynamic quantisation (EPI_GATEUP): the activation 4-tuple that
   // activate_fp16_i4 would have produced (Activate.cuh:67-180); gu_rows = intermediate size I (up rows start at I)
   int8_t* q8_out; uint8_t* q4_out; __half* q8_scale; __half* q4_scale; int gu_rows;
@@ -347,9 +347,11 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
 
     // ------------------------------------------------------------ output: one warp per token row, 4 channels per lane
     constexpr float kInv = 1.0f / 256.0f;   // exact: removes the 16 * 16 operand factor
-    const int seg = kEpi == EPI_QKV ? (int)blockIdx.x / args.seg_tiles : 0;
-    const int otile = kEpi == EPI_QKV ? (int)blockIdx.x % args.seg_tiles : (int)blockIdx.x;
-    const int n_out_dim = kEpi == EPI_QKV ? args.seg_tiles * 128 : args.N;       // row length of the output this tile writes
+    // q/k/v: tiles [0, seg_tiles) are q, the next kv_tiles k, the last kv_tiles v (kv_tiles == seg_tiles: three equal parts)
+    const int bx = (int)blockIdx.x;
+    const int seg = kEpi == EPI_QKV ? (bx < args.seg_tiles ? 0 : (bx < args.seg_tiles + args.kv_tiles ? 1 : 2)) : 0;
+    const int otile = kEpi == EPI_QKV ? (seg == 0 ? bx : bx - args.seg_tiles - (seg - 1) * args.kv_tiles) : bx;
+    const int n_out_dim = kEpi == EPI_QKV ? (seg == 0 ? args.seg_tiles : args.kv_tiles) * 128 : args.N;   // row length of the output this tile writes
     const int n_out = otile * 128 + lane * 4;
     const bool o16 = kEpi == EPI_O16 || kEpi == EPI_PUSH || (kEpi == EPI_QKV && seg == 0);
     for (int tk = cw; tk < BN; tk += 8) {

@@ -59,12 +59,12 @@ kv_dequant_rope_kernel(const uint8_t* __restrict__ k4, const __half2* __restrict
   vo[i + 64] = __float2half_rn((float)((vb[32 + (i >> 1)] >> sh) & 0xF) * vp.x - vp.y);
 }
 
-// q f16 [T, H*128] (pre-RoPE, the q projection's output); kf, vf from kv_dequant_rope_kernel; indptr i32 [B+1]: prompt b
-// owns tokens [indptr[b], indptr[b+1]); out f16 [T, H*128]
+// q f16 [T, H*128] (pre-RoPE, the q projection's output); kf, vf f16 [T, Hkv*128] from kv_dequant_rope_kernel (H % Hkv == 0);
+// indptr i32 [B+1]: prompt b owns tokens [indptr[b], indptr[b+1]); out f16 [T, H*128]
 __global__ void __launch_bounds__(PF_THREADS)
 prefill_attn_kernel(const __half* __restrict__ q, const __half* __restrict__ kf, const __half* __restrict__ vf,
                     const int32_t* __restrict__ indptr, const float2* __restrict__ rope, __half* __restrict__ out, int H,
-                    float scale_log2) {
+                    int Hkv, float scale_log2) {
   __shared__ __align__(16) __half Ks[PF_BK * PF_KPITCH];
   __shared__ __align__(16) __half Vt[128 * PF_VPITCH];
   const int b = blockIdx.y, h = blockIdx.z, qt = blockIdx.x;
@@ -73,6 +73,8 @@ prefill_attn_kernel(const __half* __restrict__ q, const __half* __restrict__ kf,
   if (q0 >= L) return;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
   const size_t row_pitch = (size_t)H * 128;
+  const size_t kv_pitch = (size_t)Hkv * 128;          // grouped-query attention: query head h reads KV head h / (H / Hkv)
+  const int hk = h / (H / Hkv);
 
   // ---- Q fragments of this warp's 16 rows, rotated (FP32 math, rounded to FP16 like `rotary_pos_emb(...).to(q.dtype)`)
   uint32_t qa[8][4];
@@ -116,7 +118,7 @@ prefill_attn_kernel(const __half* __restrict__ q, const __half* __restrict__ kf,
       const int c = tid + it * PF_THREADS, tok = c >> 4, ch = c & 15, pos = k0 + tok;
       uint4 kv = make_uint4(0, 0, 0, 0), vv = make_uint4(0, 0, 0, 0);        // beyond the prompt: zeros (masked below anyway)
       if (pos < L) {
-        const size_t off = (size_t)(t0 + pos) * row_pitch + h * 128 + ch * 8;
+        const size_t off = (size_t)(t0 + pos) * kv_pitch + hk * 128 + ch * 8;
         kv = *reinterpret_cast<const uint4*>(kf + off);
         vv = *reinterpret_cast<const uint4*>(vf + off);
       }

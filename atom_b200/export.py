@@ -1,6 +1,7 @@
 """Simulated (model/) layer -> real-INT4 serving layer (e2e/).  No reference equivalent: the reference's e2e harness runs
 random INT4 weights (e2e/README.md) and its accuracy simulator never leaves FP16; this module is the missing bridge, so
-a layer calibrated with the model/ surface (QLlamaDecoderLayer) can be served by the sm_90a kernels.
+a layer calibrated with the model/ surface (QLlamaDecoderLayer) can be served by the sm_90a kernels -- multi-head or
+grouped-query attention (Llama-2-70B, Llama-3 shapes: fewer k/v rows, a KV cache of KV heads), with the layer's RoPE base.
 
 Operand conventions are the kernels' (include/atom_b200.h; e2e/punica-atom/punica/models/llama.py:35-58):
   weight_int4 u8 [out, (in-128)/2]   reordered input channel 2j in the low nibble of byte j
@@ -40,15 +41,22 @@ def _index_i16(idx, n):
 @torch.no_grad()
 def int4_decoder_layer(qlayer, device="cuda", layer_idx=0):
     """QLlamaDecoderLayer -> atom_b200.llama.LlamaDecoderLayer with identical quantised weights and reorder indices.
-    MHA only (num_key_value_heads == num_heads), head_dim 128 -- the shapes the INT4 KV kernels support."""
+    Multi-head or grouped-query attention (num_heads / num_key_value_heads in {1, 2, 4, 8}: the group sizes the INT4 paged-KV
+    decode kernel serves), head_dim 128; the layer's RoPE base (`rope_theta` of the attention module or its config, default 1e4)
+    is carried into the exported config."""
     at = qlayer.self_attn
-    assert at.num_key_value_heads == at.num_heads, "the INT4 paged-KV kernels are MHA (as the reference's)"
+    if at.num_heads % at.num_key_value_heads or at.num_heads // at.num_key_value_heads not in (1, 2, 4, 8):
+        raise ValueError(f"{at.num_heads} query heads over {at.num_key_value_heads} KV heads: the INT4 paged-KV decode kernel serves "
+                         f"1, 2, 4 or 8 query heads per KV head")
     assert at.head_dim == 128, "head_dim must be 128 (KV quantisation group)"
+    theta = getattr(at, "rope_theta", None) or getattr(getattr(at, "config", None), "rope_theta", None) or 10000.0
     hidden = at.hidden_size
     inter = qlayer.mlp.gate_proj.weight.shape[0]
     norm = qlayer.input_layernorm.originalNorm
     cfg = LlamaConfig(hidden_size=hidden, intermediate_size=inter, num_attention_heads=at.num_heads, num_hidden_layers=1,
-                      rms_norm_eps=float(getattr(norm, "variance_epsilon", getattr(norm, "eps", 1e-6))))
+                      rms_norm_eps=float(getattr(norm, "variance_epsilon", getattr(norm, "eps", 1e-6))),
+                      num_key_value_heads=None if at.num_key_value_heads == at.num_heads else int(at.num_key_value_heads),
+                      rope_theta=float(theta))
     layer = LlamaDecoderLayer(cfg, layer_idx)
     for name in ("q_proj", "k_proj", "v_proj", "o_proj"):
         fill_linear_int4(getattr(layer.self_attn, name), getattr(at, name))

@@ -12,6 +12,7 @@ Differences (documented in DESIGN.md):
 """
 import math
 from dataclasses import dataclass
+from typing import Optional
 
 import torch
 from torch import nn
@@ -30,6 +31,8 @@ class LlamaConfig:
     rms_norm_eps: float = 1e-6
     vocab_size: int = 32000
     pad_token_id: int = 0
+    num_key_value_heads: Optional[int] = None      # None = multi-head attention (one KV head per query head)
+    rope_theta: float = 10000.0
 
 
 def rotate_half(x):
@@ -37,10 +40,10 @@ def rotate_half(x):
     return torch.cat((-x2, x1), dim=-1)
 
 
-def rotary_pos_emb(q, k, beg):
-    """llama.py:18-32"""
+def rotary_pos_emb(q, k, beg, theta=10000):
+    """llama.py:18-32 (`theta`: the RoPE base, 1e4 there)"""
     bsz, nhead, seqlen, dim = q.shape
-    inv_freq = 1.0 / (10000 ** (torch.arange(0, dim, 2, device=q.device).float() / dim))
+    inv_freq = 1.0 / (theta ** (torch.arange(0, dim, 2, device=q.device).float() / dim))
     t = torch.arange(beg, beg + seqlen, device=q.device, dtype=torch.float32)
     freqs = torch.einsum("i,j->ij", t, inv_freq)
     emb = torch.cat((freqs, freqs), dim=-1)[None, None]
@@ -183,10 +186,16 @@ class LlamaAttention(nn.Module):
         if self.head_dim * self.num_heads != self.hidden_size:
             raise ValueError(f"hidden_size must be divisible by num_heads (got `hidden_size`: {self.hidden_size}"
                              f" and `num_heads`: {self.num_heads}).")
+        # grouped-query attention: fewer KV heads than query heads (Llama-2-70B, Llama-3, Mixtral); None = multi-head
+        self.num_kv_heads = getattr(config, "num_key_value_heads", None) or self.num_heads
+        self.rope_theta = float(getattr(config, "rope_theta", 10000.0))
+        if self.num_heads % self.num_kv_heads:
+            raise ValueError(f"num_attention_heads ({self.num_heads}) must be a multiple of num_key_value_heads ({self.num_kv_heads})")
         h = self.num_heads * self.head_dim
+        hkv = self.num_kv_heads * self.head_dim
         self.q_proj = LinearInt4(self.hidden_size, h, out_dtype="fp16")
-        self.k_proj = LinearInt4(self.hidden_size, h, out_dtype="int4")
-        self.v_proj = LinearInt4(self.hidden_size, h, out_dtype="int4")
+        self.k_proj = LinearInt4(self.hidden_size, hkv, out_dtype="int4")
+        self.v_proj = LinearInt4(self.hidden_size, hkv, out_dtype="int4")
         self.o_proj = LinearInt4(h, self.hidden_size, out_dtype="fp16")
         self.reorder_index = nn.Parameter(torch.randperm(self.hidden_size, dtype=torch.int16), requires_grad=False)
         self._qkv = None       # fused [q; k; v] operands, built by fuse()
@@ -204,12 +213,14 @@ class LlamaAttention(nn.Module):
         if self._qkv is not None:
             outlier, norms, outlier_scales, norm_scales = hidden_states
             w4, s4, w8, s8 = self._qkv
-            q_proj, k_proj, v_proj = ops.dense_layer_gemm_i4_qkv(norms, w4, norm_scales, s4, outlier, w8, outlier_scales, s8)
+            kv_rows = None if self.num_kv_heads == self.num_heads else self.num_kv_heads * self.head_dim
+            q_proj, k_proj, v_proj = ops.dense_layer_gemm_i4_qkv(norms, w4, norm_scales, s4, outlier, w8, outlier_scales, s8,
+                                                                 kv_rows=kv_rows)
         else:
             q_proj, k_proj, v_proj = run_concurrently([self.q_proj, self.k_proj, self.v_proj], hidden_states)
         nvtx.range_pop()
         stack = []
-        nh, hd = self.num_heads, self.head_dim
+        nq, nh, hd = self.num_heads, self.num_kv_heads, self.head_dim      # nh: heads of k / v and of the cache
         if len(blen.prefills) > 0:
             nvtx.range_push("init_kv")
             assert prefill_kv is not None
@@ -219,10 +230,11 @@ class LlamaAttention(nn.Module):
             nvtx.range_pop()
             nvtx.range_push("prefill_attention")
             stack.append(ops.prefill_attention_i4(q_proj[:blen.doff], k_proj[0][:blen.doff], k_proj[1][:blen.doff],
-                                                  v_proj[0][:blen.doff], v_proj[1][:blen.doff], blen.indptr, seqlens=list(blen.prefills)))
+                                                  v_proj[0][:blen.doff], v_proj[1][:blen.doff], blen.indptr, seqlens=list(blen.prefills),
+                                                  rope_theta=self.rope_theta))
             nvtx.range_pop()
         if blen.decode > 0:
-            q = q_proj[blen.doff:].view(blen.decode, nh, hd)
+            q = q_proj[blen.doff:].view(blen.decode, nq, hd)
             k = k_proj[0][blen.doff:].view(blen.decode, nh, hd // 2)
             v = v_proj[0][blen.doff:].view(blen.decode, nh, hd // 2)
             ks = k_proj[1][blen.doff:].view(blen.decode, nh, hd // 128 * 2)
@@ -232,7 +244,8 @@ class LlamaAttention(nn.Module):
             ops.append_kv_i4(decode_kv, k.contiguous(), v.contiguous(), ks.contiguous(), vs.contiguous(), self.layer_idx)
             nvtx.range_pop()
             nvtx.range_push("batch_decode")
-            stack.append(ops.batch_decode_i4(q.contiguous(), decode_kv, self.layer_idx).view(blen.decode, self.hidden_size))
+            stack.append(ops.batch_decode_i4(q.contiguous(), decode_kv, self.layer_idx, rope_theta=self.rope_theta)
+                         .view(blen.decode, self.hidden_size))
             nvtx.range_pop()
         attn = stack[0] if len(stack) == 1 else torch.cat(stack, dim=0)
         nvtx.range_push("o_proj")

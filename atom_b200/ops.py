@@ -215,14 +215,20 @@ def dense_layer_gemm_i4_o4(a, b, a_scale, b_scale, a_keeper, b_keeper, a_keeper_
     return d, d_scale
 
 
-def dense_layer_gemm_i4_qkv(a, b_qkv, a_scale, b_scale_qkv, a_keeper, b_keeper_qkv, a_keeper_scale, b_keeper_scale_qkv, flags=GEMM_AUTO):
+def dense_layer_gemm_i4_qkv(a, b_qkv, a_scale, b_scale_qkv, a_keeper, b_keeper_qkv, a_keeper_scale, b_keeper_scale_qkv, flags=GEMM_AUTO,
+                            kv_rows=None):
     """EXTENSION: q (fp16), k and v (o4) projections of one input over row-concatenated weights [3H, ...] in one launch for
-    decode batches.  Returns (q, (k, k_scale), (v, v_scale)), bit-identical to the three separate operator calls."""
+    decode batches.  Returns (q, (k, k_scale), (v, v_scale)), bit-identical to the three separate operator calls.
+    kv_rows (grouped-query attention): rows of the k part (= of the v part) of `b_qkv`; the q part is the rest.  None = three
+    equal parts."""
     _req_width("dense_layer_gemm_i4_qkv", a_1=a, b_qkv_1=b_qkv, f16_a_scale_2=a_scale, f16_b_scale_qkv_2=b_scale_qkv, a_keeper_1=a_keeper,
                b_keeper_qkv_1=b_keeper_qkv, f16_a_keeper_scale_2=a_keeper_scale, f16_b_keeper_scale_qkv_2=b_keeper_scale_qkv)
     _req_cuda(a, b_qkv, a_scale, b_scale_qkv, a_keeper, b_keeper_qkv, a_keeper_scale, b_keeper_scale_qkv)
     m, n3 = a.size(0), b_qkv.size(0)
     k = a.size(1) * 2 + a_keeper.size(1)
+    if kv_rows is not None:
+        return _gemm_i4_qkv_gqa(a, b_qkv, a_scale, b_scale_qkv, a_keeper, b_keeper_qkv, a_keeper_scale, b_keeper_scale_qkv, flags,
+                                int(kv_rows), m, n3, k)
     if n3 % 384 != 0 or b_scale_qkv.numel() < (k // 128 - 1) * n3 or b_keeper_qkv.size(0) != n3:
         raise RuntimeError("dense_layer_gemm_i4_qkv: weights must be the row concatenation [q; k; v] with H % 128 == 0")
     h = n3 // 3
@@ -236,6 +242,24 @@ def dense_layer_gemm_i4_qkv(a, b_qkv, a_scale, b_scale_qkv, a_keeper, b_keeper_q
                                                a_keeper.data_ptr(), b_keeper_qkv.data_ptr(), a_keeper_scale.data_ptr(),
                                                b_keeper_scale_qkv.data_ptr(), q.data_ptr(), kk.data_ptr(), ks.data_ptr(), vv.data_ptr(),
                                                vs.data_ptr(), m, h, k, flags, _stream(a)), "dense_layer_gemm_i4_qkv")
+    return q, (kk, ks), (vv, vs)
+
+
+def _gemm_i4_qkv_gqa(a, b_qkv, a_scale, b_scale_qkv, a_keeper, b_keeper_qkv, a_keeper_scale, b_keeper_scale_qkv, flags, kv_rows, m, n3, k):
+    hq = n3 - 2 * kv_rows
+    if kv_rows <= 0 or hq <= 0 or kv_rows % 128 or hq % 128 or b_scale_qkv.numel() < (k // 128 - 1) * n3 or b_keeper_qkv.size(0) != n3:
+        raise RuntimeError("dense_layer_gemm_i4_qkv: weights must be the row concatenation [q; k; v] with kv_rows rows of k and of v, "
+                           "q and kv_rows multiples of 128")
+    q = torch.empty((m, hq), dtype=torch.float16, device=a.device)
+    kk = torch.empty((m, kv_rows // 2), dtype=torch.uint8, device=a.device)
+    vv = torch.empty((m, kv_rows // 2), dtype=torch.uint8, device=a.device)
+    ks = torch.empty((m, kv_rows // 128 * 2), dtype=torch.float16, device=a.device)
+    vs = torch.empty((m, kv_rows // 128 * 2), dtype=torch.float16, device=a.device)
+    with torch.cuda.device(a.device):
+        _lib.check(_lib.lib().atom_gemm_i4_qkv_gqa(a.data_ptr(), b_qkv.data_ptr(), a_scale.data_ptr(), b_scale_qkv.data_ptr(),
+                                                   a_keeper.data_ptr(), b_keeper_qkv.data_ptr(), a_keeper_scale.data_ptr(),
+                                                   b_keeper_scale_qkv.data_ptr(), q.data_ptr(), kk.data_ptr(), ks.data_ptr(), vv.data_ptr(),
+                                                   vs.data_ptr(), m, hq, kv_rows, k, flags, _stream(a)), "dense_layer_gemm_i4_qkv (gqa)")
     return q, (kk, ks), (vv, vs)
 
 
@@ -270,14 +294,22 @@ def _kv_dims(kv):
     return kv.data.size(1), kv.data.size(3), kv.data.size(4)
 
 
-def batch_decode_i4(q, kv, layer_idx):
-    """ops/__init__.py:21-32"""
+def batch_decode_i4(q, kv, layer_idx, rope_theta=10000.0):
+    """ops/__init__.py:21-32.  EXTENSION (grouped-query attention): q may hold G = 2, 4 or 8 query heads per head of the cache
+    (query head h attends KV head h // G), and `rope_theta` is the RoPE base; one query head per KV head at the default base
+    is the reference's operator."""
     _req_cuda(q, kv.data, kv.param, kv.indptr, kv.indicies, kv.last_page_offset)
     L, H, P = _kv_dims(kv)
-    if q.dim() != 3 or q.size(1) != H or q.size(2) != 128 or kv.indptr.size(0) != q.size(0) + 1 or \
-            kv.last_page_offset.size(0) != q.size(0):
+    if q.dim() != 3 or q.size(2) != 128 or kv.indptr.size(0) != q.size(0) + 1 or kv.last_page_offset.size(0) != q.size(0):
         raise RuntimeError("batch_decode_i4: shape mismatch")
     o = torch.empty(q.shape, dtype=q.dtype, device=q.device)
+    if q.size(1) != H or float(rope_theta) != 10000.0:
+        with torch.cuda.device(q.device):
+            _lib.check(_lib.lib().atom_batch_decode_gqa_i4(o.data_ptr(), q.data_ptr(), kv.data.data_ptr(), kv.param.data_ptr(),
+                                                           kv.indptr.data_ptr(), kv.indicies.data_ptr(),
+                                                           kv.last_page_offset.data_ptr(), L, layer_idx, q.size(1), H, P, q.size(0),
+                                                           float(rope_theta), _stream(q)), "batch_decode_i4 (gqa)")
+        return o
     with torch.cuda.device(q.device):
         _lib.check(_lib.lib().atom_batch_decode_i4(o.data_ptr(), q.data_ptr(), kv.data.data_ptr(), kv.param.data_ptr(),
                                                    kv.indptr.data_ptr(), kv.indicies.data_ptr(),
@@ -289,29 +321,33 @@ def batch_decode_i4(q, kv, layer_idx):
 _rope_tables = {}
 
 
-def rope_table(max_len, device):
-    """(cos, sin)(pos * theta_i) for pos < max_len, i < 64, theta_i = 1e4^(-i/64), float32 [max_len, 64, 2] -- the factors of
-    punica/models/llama.py:18-32 (`rotary_pos_emb`), computed the same way and cached per device."""
+def rope_table(max_len, device, theta=10000.0):
+    """(cos, sin)(pos * theta_i) for pos < max_len, i < 64, theta_i = theta^(-i/64), float32 [max_len, 64, 2] -- the factors of
+    punica/models/llama.py:18-32 (`rotary_pos_emb`), computed the same way and cached per (device, base)."""
     size = max(256, 1 << (int(max_len) - 1).bit_length())
-    key = (str(device), size)
+    key = (str(device), size) if float(theta) == 10000.0 else (str(device), size, float(theta))
     t = _rope_tables.get(key)
     if t is None:
-        inv_freq = 1.0 / (10000 ** (torch.arange(0, 128, 2, device=device).float() / 128))
+        base = 10000 if float(theta) == 10000.0 else float(theta)
+        inv_freq = 1.0 / (base ** (torch.arange(0, 128, 2, device=device).float() / 128))
         freqs = torch.einsum("i,j->ij", torch.arange(0, size, device=device, dtype=torch.float32), inv_freq)
         t = torch.stack((freqs.cos(), freqs.sin()), dim=-1).contiguous()
         _rope_tables[key] = t
     return t
 
 
-def prefill_attention_i4(q, k, k_param, v, v_param, seqlen_indptr, seqlens=None):
+def prefill_attention_i4(q, k, k_param, v, v_param, seqlen_indptr, seqlens=None, rope_theta=10000.0):
     """EXTENSION: causal prefill attention of every prompt over its own quantised K/V (the o4 projection outputs) with RoPE,
-    one launch for all prompts and heads.  q f16 [T, H*128]; k, v u8 [T, H*64]; k_param, v_param f16 [T, H*2];
-    seqlen_indptr i32 [B+1] (device); seqlens: the prompt lengths as host ints (avoids a device read).  Returns f16 [T, H*128]."""
+    one launch for all prompts and heads.  q f16 [T, H*128]; k, v u8 [T, Hkv*64]; k_param, v_param f16 [T, Hkv*2] (Hkv = H, or
+    a divisor of it for grouped-query attention: taken from k's shape); seqlen_indptr i32 [B+1] (device); seqlens: the prompt
+    lengths as host ints (avoids a device read); rope_theta: the RoPE base.  Returns f16 [T, H*128]."""
     _req_width("prefill_attention_i4", f16_q_2=q, k_1=k, f16_k_param_2=k_param, v_1=v, f16_v_param_2=v_param)
     _req_cuda(q, k, k_param, v, v_param, seqlen_indptr)
     t, hd = q.shape
     h = hd // 128
-    if hd % 128 or k.shape != (t, h * 64) or v.shape != k.shape or k_param.numel() != t * h * 2 or v_param.numel() != t * h * 2:
+    hkv = k.shape[1] // 64 if k.dim() == 2 else 0
+    if hd % 128 or k.dim() != 2 or k.shape != (t, hkv * 64) or hkv == 0 or v.shape != k.shape or k_param.numel() != t * hkv * 2 or \
+            v_param.numel() != t * hkv * 2:
         raise RuntimeError("prefill_attention_i4: shape mismatch (head_dim must be 128)")
     if seqlens is None:
         ip = seqlen_indptr.cpu()
@@ -320,7 +356,16 @@ def prefill_attention_i4(q, k, k_param, v, v_param, seqlen_indptr, seqlens=None)
     if sum(seqlens) != t or seqlen_indptr.numel() != b + 1:
         raise RuntimeError("prefill_attention_i4: seqlen_indptr does not cover the tokens")
     pos = torch.cat([torch.arange(n, dtype=torch.int32) for n in seqlens]).to(q.device, non_blocking=True)
-    table = rope_table(max_len, q.device)
+    table = rope_table(max_len, q.device, rope_theta)
+    if hkv != h:
+        kf = torch.empty((t, hkv * 128), dtype=q.dtype, device=q.device)
+        vf, out = torch.empty_like(kf), torch.empty_like(q)
+        with torch.cuda.device(q.device):
+            _lib.check(_lib.lib().atom_prefill_attention_gqa_i4(q.data_ptr(), k.data_ptr(), k_param.data_ptr(), v.data_ptr(),
+                                                                v_param.data_ptr(), seqlen_indptr.data_ptr(), pos.data_ptr(),
+                                                                table.data_ptr(), kf.data_ptr(), vf.data_ptr(), out.data_ptr(), t, b,
+                                                                max_len, h, hkv, _stream(q)), "prefill_attention_i4 (gqa)")
+        return out
     kf, vf, out = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
     with torch.cuda.device(q.device):
         _lib.check(_lib.lib().atom_prefill_attention_i4(q.data_ptr(), k.data_ptr(), k_param.data_ptr(), v.data_ptr(), v_param.data_ptr(),

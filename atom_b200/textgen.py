@@ -60,11 +60,19 @@ class ModelConfig:
     intermediate_size: int
     dtype: str = "float16"
     device: str = "cuda:0"
+    num_kv_heads: Optional[int] = None     # None = multi-head attention; the KV pool has this many heads
+    rope_theta: float = 10000.0
+
+    @property
+    def kv_heads(self) -> int:
+        return self.num_kv_heads or self.num_heads
 
 
 MODEL_CFGS = {
     "7b": ModelConfig(num_layers=32, num_heads=32, hidden_size=4096, intermediate_size=11008),
     "13b": ModelConfig(num_layers=40, num_heads=40, hidden_size=5120, intermediate_size=13824),
+    "70b": ModelConfig(num_layers=80, num_heads=64, hidden_size=8192, intermediate_size=28672, num_kv_heads=8),
+    "llama3-8b": ModelConfig(num_layers=32, num_heads=32, hidden_size=4096, intermediate_size=14336, num_kv_heads=8, rope_theta=5e5),
 }
 
 

@@ -98,7 +98,8 @@ class RowParallelLinearInt4(nn.Module):
 
 class TPLlamaDecoderLayer(nn.Module):
     """One Llama decoder layer over `world` ranks: heads and MLP channels are sharded, hidden states replicated.
-    forward(hidden, decode_kv) runs a decode step (one token per sequence); KV cache pools are per rank (local heads)."""
+    forward(hidden, decode_kv) runs a decode step (one token per sequence); KV cache pools are per rank (local KV heads:
+    with grouped-query attention a rank holds num_key_value_heads / world of them and their query heads)."""
 
     def __init__(self, config, layer_idx, rank, world, group=None, allreduce=None):
         super().__init__()
@@ -106,12 +107,16 @@ class TPLlamaDecoderLayer(nn.Module):
         h, nh = config.hidden_size, config.num_attention_heads
         if nh % world:
             raise ValueError("num_attention_heads must be divisible by the tensor-parallel size")
+        nkv = getattr(config, "num_key_value_heads", None) or nh
+        if nkv % world:      # KV heads are sharded with the query heads of their groups; they are not replicated
+            raise ValueError("num_key_value_heads must be divisible by the tensor-parallel size")
         self.rank, self.world, self.layer_idx = rank, world, layer_idx
-        self.local_heads = nh // world
-        hl = self.local_heads * 128
+        self.local_heads, self.local_kv_heads = nh // world, nkv // world
+        self.rope_theta = float(getattr(config, "rope_theta", 10000.0))
+        hl, hkvl = self.local_heads * 128, self.local_kv_heads * 128
         self.q_proj = LinearInt4(h, hl, "fp16")
-        self.k_proj = LinearInt4(h, hl, "int4")
-        self.v_proj = LinearInt4(h, hl, "int4")
+        self.k_proj = LinearInt4(h, hkvl, "int4")
+        self.v_proj = LinearInt4(h, hkvl, "int4")
         self.o_proj = RowParallelLinearInt4(h, h, rank, world, group, allreduce=allreduce)
         assert self.o_proj.k1 - self.o_proj.k0 == hl, "head slices and o_proj K-slices must coincide"
         self.inter_sizes = split_sizes(config.intermediate_size, world)
@@ -155,15 +160,16 @@ class TPLlamaDecoderLayer(nn.Module):
         fused = getattr(self, "_qkv", None) is not None and b <= 64
         if fused:
             w4, s4, w8, s8 = self._qkv
-            q, (k, ks), (v, vs) = ops.dense_layer_gemm_i4_qkv(x[1], w4, x[3], s4, x[0], w8, x[2], s8)
+            kv_rows = None if self.local_kv_heads == self.local_heads else self.local_kv_heads * 128
+            q, (k, ks), (v, vs) = ops.dense_layer_gemm_i4_qkv(x[1], w4, x[3], s4, x[0], w8, x[2], s8, kv_rows=kv_rows)
             q = q.view(b, self.local_heads, 128)
         else:
             q = self.q_proj(x).view(b, self.local_heads, 128)
             k, ks = self.k_proj(x)
             v, vs = self.v_proj(x)
-        ops.append_kv_i4(decode_kv, k.view(b, self.local_heads, 64), v.view(b, self.local_heads, 64),
-                         ks.view(b, self.local_heads, 2), vs.view(b, self.local_heads, 2), self.layer_idx)
-        attn = ops.batch_decode_i4(q, decode_kv, self.layer_idx).view(b, self.local_heads * 128)
+        ops.append_kv_i4(decode_kv, k.view(b, self.local_kv_heads, 64), v.view(b, self.local_kv_heads, 64),
+                         ks.view(b, self.local_kv_heads, 2), vs.view(b, self.local_kv_heads, 2), self.layer_idx)
+        attn = ops.batch_decode_i4(q, decode_kv, self.layer_idx, rope_theta=self.rope_theta).view(b, self.local_heads * 128)
         o_in = ops.reorder_fp16_i4(attn, self.attn_reorder_index)
         o = self.o_proj.forward_push(o_in) if self.o_proj.can_push(b) else self.o_proj(o_in)                  # all-reduce #1
         hidden_states, x = self.post_attention_layernorm.forward_add(o, hidden_states)                        # residual add (+ reduce) folded into the norm

@@ -110,6 +110,15 @@ ATOM_API int atom_gemm_i4_qkv(const void* a, const void* b_qkv, const void* a_sc
                      const void* b_keeper_qkv, const void* a_keeper_scale, const void* b_keeper_scale_qkv, void* q, void* k,
                      void* k_scale, void* v, void* v_scale, int64_t M, int64_t H, int64_t K, uint32_t flags, void* stream);
 
+/* EXTENSION (grouped-query attention): atom_gemm_i4_qkv with fewer KV heads than query heads.  Rows [0,Hq_dim) of the
+ * concatenated weights are q, [Hq_dim, Hq_dim+Hkv_dim) k, the last Hkv_dim v (Hq_dim = query heads * 128, Hkv_dim = KV heads * 128,
+ * Hq_dim % Hkv_dim == 0).  q f16 [M,Hq_dim]; k, v u8 [M,Hkv_dim/2] with k_scale, v_scale f16 [M,Hkv_dim/128,2]; bit-identical to
+ * the three separate calls.  Hq_dim == Hkv_dim is atom_gemm_i4_qkv. */
+ATOM_API int atom_gemm_i4_qkv_gqa(const void* a, const void* b_qkv, const void* a_scale, const void* b_scale_qkv, const void* a_keeper,
+                         const void* b_keeper_qkv, const void* a_keeper_scale, const void* b_keeper_scale_qkv, void* q, void* k,
+                         void* k_scale, void* v, void* v_scale, int64_t M, int64_t Hq_dim, int64_t Hkv_dim, int64_t K, uint32_t flags,
+                         void* stream);
+
 /* EXTENSION (launch-count reduction, SURVEY.md 8 f4): LlamaMLP's gate_proj, up_proj and activate_fp16_i4
  * (punica/models/llama.py:85-87) as ONE launch for decode batches (M <= 64; ATOM_E_UNSUPPORTED above): weights
  * row-concatenated  b_gu u8 [2I,(K-128)/2] (rows [0,I) = gate, [I,2I) = up), b_scale_gu f16 [K/128-1, 2I], b_keeper_gu
@@ -138,6 +147,16 @@ ATOM_API int atom_batch_decode_i4(void* o, const void* q, const void* kv_data, c
                          const void* kv_indices, const void* last_page_offset, int num_layers, int layer_idx,
                          int num_heads, int page_size, int batch_size, void* stream);
 
+/* EXTENSION (grouped-query attention): batch_decode_i4 for num_q_heads = G * num_kv_heads query heads over a cache of
+ * num_kv_heads heads -- the same layout with H = num_kv_heads; query head h attends KV head h / G.
+ *   o,q f16 [B,num_q_heads,128]  kv_data u8 [pages,L,2,num_kv_heads,P,64]  kv_param f16 [pages,L,2,num_kv_heads,P,2]
+ * One CTA per (sequence, KV head) reads every page of that head once and serves its G query heads.  rope_theta is the RoPE base
+ * (1e4 for Llama-1/2, 5e5 for Llama-3, 1e6 for Mixtral).  G in {2, 4, 8}; G = 1 with rope_theta = 1e4 IS atom_batch_decode_i4
+ * (same kernel, same bits), G = 1 with another base is supported; any other ratio returns ATOM_E_UNSUPPORTED. */
+ATOM_API int atom_batch_decode_gqa_i4(void* o, const void* q, const void* kv_data, const void* kv_param, const void* kv_indptr,
+                             const void* kv_indices, const void* last_page_offset, int num_layers, int layer_idx,
+                             int num_q_heads, int num_kv_heads, int page_size, int batch_size, float rope_theta, void* stream);
+
 /* EXTENSION (SURVEY.md 8 f3): the prefill attention the reference leaves as a placeholder
  * (punica/models/llama.py:171-190, SDPA over torch.randn K/V): causal attention of every prompt over its own just-quantised
  * K/V -- the o4 outputs of the k/v projections, x = nibble * scale - zero (quantization.cuh:76) -- with RoPE(theta 1e4) on q
@@ -148,6 +167,14 @@ ATOM_API int atom_batch_decode_i4(void* o, const void* q, const void* kv_data, c
 ATOM_API int atom_prefill_attention_i4(const void* q, const void* k, const void* k_param, const void* v, const void* v_param,
                               const void* seqlen_indptr, const void* pos_of_token, const void* rope_table, void* k_f16, void* v_f16,
                               void* out, int total_tokens, int batch_size, int max_len, int num_heads, void* stream);
+
+/* EXTENSION (grouped-query attention): atom_prefill_attention_i4 with num_kv_heads <= num_q_heads (num_q_heads % num_kv_heads == 0).
+ *   q, out f16 [T, num_q_heads*128]; k, v u8 [T, num_kv_heads*64]; k_param, v_param f16 [T, num_kv_heads, 2];
+ *   k_f16, v_f16 f16 [T, num_kv_heads*128] scratch; rope_table built for the model's RoPE base.  Everything else as above. */
+ATOM_API int atom_prefill_attention_gqa_i4(const void* q, const void* k, const void* k_param, const void* v, const void* v_param,
+                                  const void* seqlen_indptr, const void* pos_of_token, const void* rope_table, void* k_f16, void* v_f16,
+                                  void* out, int total_tokens, int batch_size, int max_len, int num_q_heads, int num_kv_heads,
+                                  void* stream);
 
 /* EXTENSION (SURVEY.md 8e; the reference has no multi-GPU code): one-shot all-reduce (sum) of an FP16 vector over NVLink peer
  * memory for the tensor-parallel row-parallel projections.  peer_buffers: DEVICE array of `world` pointers to every rank's

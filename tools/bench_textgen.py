@@ -26,7 +26,8 @@ def build_model(mc: tg.ModelConfig, layers: int):
     try:
         with device:
             model = LlamaForCausalLM(LlamaConfig(hidden_size=mc.hidden_size, num_attention_heads=mc.num_heads,
-                                                 intermediate_size=mc.intermediate_size, num_hidden_layers=layers))
+                                                 intermediate_size=mc.intermediate_size, num_hidden_layers=layers,
+                                                 num_key_value_heads=mc.num_kv_heads, rope_theta=mc.rope_theta))
     finally:
         torch.set_default_dtype(default)
     model = model.to(device)
@@ -60,7 +61,7 @@ def main():
     model = build_model(mc, layers)
     rs = tg.generate_request_set(args.batch_size * args.num_batches, args.maxlen)
     cfg = tg.TextGenConfig(args.batch_size)
-    pool = KvPoolInt4(layers, mc.num_heads, mc.hidden_size // mc.num_heads,
+    pool = KvPoolInt4(layers, mc.kv_heads, mc.hidden_size // mc.num_heads,     # the cache holds KV heads (grouped-query: fewer)
                       tg.pool_capacity(args.batch_size, args.maxlen, args.block_len), args.block_len, device)
     runner = None if args.no_cuda_graphs else tg.DecodeGraphRunner(
         model, pool, device, max_pages_per_seq=(args.maxlen + args.block_len - 1) // args.block_len + 1)
