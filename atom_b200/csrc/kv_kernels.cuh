@@ -109,6 +109,22 @@ __device__ __forceinline__ __half2 nib2x(uint32_t w, uint32_t w8, int q) {
 // halves are widened first (the FP32 product of two halves is exact inside the fma, one rounding in all)
 __device__ __forceinline__ float fhfma(__half a, __half b, float acc) { return fmaf(__half2float(a), __half2float(b), acc); }
 
+// A lane accumulates the V sums of at most DEC_FP16_RUN of its tokens in half2 before adding them to its FP32 accumulators.
+// Each token adds at most 15 * p * (V scale), with p <= 2^6 under the lazy rescale, so a run stays below 4 * 960 * scale: finite
+// for V scales below 17 at every page size (P <= 32 has at most four tokens per lane and page; P > 32 flushes after four).
+constexpr int DEC_FP16_RUN = 4;
+
+// couple u of word w holds elements (8w + q, 8w + q + 4): move the half2 V sums of a run into the FP32 accumulators
+__device__ __forceinline__ void flush_pv(float (&acc)[32], __half2 (&pv)[16]) {
+#pragma unroll
+  for (int u = 0; u < 16; ++u) {
+    const float2 f = __half22float2(pv[u]);
+    acc[8 * (u >> 2) + (u & 3)] += f.x;
+    acc[8 * (u >> 2) + (u & 3) + 4] += f.y;
+    pv[u] = __half2half2(__ushort_as_half(0));
+  }
+}
+
 // kMaxTpl: tokens per lane per page = P / 8 <= kMaxTpl.  kP: page size as a compile-time constant (16 / 32: the sizes the harness
 // uses -- all table strides and the token loops become immediates) or 0 = read it from the arguments.
 template <int kMaxTpl, int kP>
@@ -276,10 +292,11 @@ batch_decode_kernel(__half* __restrict__ o, const __half* __restrict__ q, KvArgs
         if (tl < valid) xmax = fmaxf(xmax, x[i]);
       }
     }
-    // ---- one rescale per page, then p * v with the dequant folded; V partial sums of the page in half2
+    // ---- one rescale per page, then p * v with the dequant folded; V partial sums of the page in half2, DEC_FP16_RUN tokens at most
     // The running maximum only moves when it is exceeded by more than 2^6: any m gives the same softmax, the weights then reach
-    // at most 64 (times the V scale: far inside FP16 for the per-page half2 sums), and with 32 lanes per warp "some lane saw a new
-    // maximum" would otherwise be true on almost every page -- the 34-FMUL rescale below now runs a few times per sequence.
+    // at most 64 (times 15 x the V scale per token: inside FP16 for a run of four tokens up to V scales of 17), and with 32 lanes
+    // per warp "some lane saw a new maximum" would otherwise be true on almost every page -- the 34-FMUL rescale below now runs a
+    // few times per sequence.
     const float m_new = (xmax > m + 6.f) ? xmax : m;
     const float sc = exp2f(m - m_new);
     m = m_new;
@@ -308,14 +325,9 @@ batch_decode_kernel(__half* __restrict__ o, const __half* __restrict__ q, KvArgs
           for (int u = 0; u < 16; ++u) pv[u] = __hfma2(nib2x(w4[u >> 2], w8[u >> 2], u & 3), (u & 1) ? ps2o : ps2, pv[u]);
         }
       }
+      if (kMaxTpl > DEC_FP16_RUN && i % DEC_FP16_RUN == DEC_FP16_RUN - 1 && i + 1 < tpl) flush_pv(acc, pv);   // P > 32
     }
-    // couple u of word w holds elements (8w + q, 8w + q + 4)
-#pragma unroll
-    for (int u = 0; u < 16; ++u) {
-      const float2 f = __half22float2(pv[u]);
-      acc[8 * (u >> 2) + (u & 3)] += f.x;
-      acc[8 * (u >> 2) + (u & 3) + 4] += f.y;
-    }
+    flush_pv(acc, pv);
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[s]);
   }
@@ -554,7 +566,7 @@ batch_decode_gqa_kernel(__half* __restrict__ o, const __half* __restrict__ q, Kv
         if (tl < valid) xmax = fmaxf(xmax, x[i]);
       }
     }
-    // ---- one (lazy, 2^6) rescale per page, then p * v with the dequant folded; V partial sums of the page in half2
+    // ---- one (lazy, 2^6) rescale per page, then p * v with the dequant folded; V partial sums in half2 runs (DEC_FP16_RUN)
     const float m_new = (xmax > m + 6.f) ? xmax : m;
     const float sc = exp2f(m - m_new);
     m = m_new;
@@ -583,14 +595,9 @@ batch_decode_gqa_kernel(__half* __restrict__ o, const __half* __restrict__ q, Kv
           for (int u = 0; u < 16; ++u) pv[u] = __hfma2(nib2x(w4[u >> 2], w8[u >> 2], u & 3), (u & 1) ? ps2o : ps2, pv[u]);
         }
       }
+      if (kMaxTpl > DEC_FP16_RUN && i % DEC_FP16_RUN == DEC_FP16_RUN - 1 && i + 1 < tpl) flush_pv(acc, pv);   // P > 32
     }
-    // couple u of word w holds elements (8w + q, 8w + q + 4)
-#pragma unroll
-    for (int u = 0; u < 16; ++u) {
-      const float2 f = __half22float2(pv[u]);
-      acc[8 * (u >> 2) + (u & 3)] += f.x;
-      acc[8 * (u >> 2) + (u & 3) + 4] += f.y;
-    }
+    flush_pv(acc, pv);
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[s]);          // the G-th arrival frees the stage
   }

@@ -167,7 +167,8 @@ class _KV:
 
 
 @pytest.mark.parametrize("B,H,P,lens", [(3, 2, 16, [1, 37, 64]), (7, 4, 16, [5, 499, 16, 17, 250, 333, 32]),
-                                        (2, 3, 32, [2048, 777]), (4, 2, 8, [8, 9, 1, 100])])
+                                        (2, 3, 32, [2048, 777]), (4, 2, 8, [8, 9, 1, 100]), (4, 2, 24, [1, 23, 25, 500]),
+                                        (4, 2, 64, [1, 63, 65, 1000])])
 def test_batch_decode(B, H, P, lens):
     from atom_b200 import ops
     rng = np.random.default_rng(B * 100 + P)
@@ -179,7 +180,9 @@ def test_batch_decode(B, H, P, lens):
         o = ops.batch_decode_i4(T(q), kv, layer).cpu().numpy()
         ref = O.batch_decode_i4(q, data, param, indptr, indices, last, layer)
         # FP16 output of an FP32 softmax-attention with approximate-vs-exact transcendental differences:
-        # rtol/atol 5e-4: the bound the reference's own test intends (test_batch_decode_int4.py:9-14), SURVEY.md 8(c) policy (4)
+        # rtol/atol 5e-4: the bound the reference's own test intends (test_batch_decode_int4.py:9-14), SURVEY.md 8(c) policy (4).
+        # This fixture's softmax is flat (logit spread ~0.25 nats, V scales <= 0.05), where the kernel's FP16 score and V paths
+        # hardly matter; its error in peaked, long or large-V regimes is bounded in test_z_attention_accuracy_gpu.py instead.
         err = np.abs(o.astype(np.float32) - ref.astype(np.float32)) - 5e-4 * np.abs(ref.astype(np.float32))
         assert err.max() <= 5e-4, f"layer {layer}: worst excess over rtol*|ref| = {err.max():.2e} (atol 5e-4)"
 

@@ -149,7 +149,9 @@ def test_gemm_o4_equals_reference_kernel(m, flags):
 def test_batch_decode_at_least_as_close_to_the_oracle_as_the_reference_kernel():
     """Both kernels approximate transcendentals (the reference: __powf / __sincosf per element; ours: a rotation table and
     packed FP16 dequantisation), so neither is the other's bit pattern.  Judge both against the CPU oracle (float math,
-    decode.cuh:480-689 restated): ours must meet rtol = atol = 5e-4 and must not be further from it than the reference is."""
+    decode.cuh:480-689 restated): ours must meet rtol = atol = 5e-4 and must not be further from it than the reference is.
+    That holds on this flat fixture (logit spread ~0.25 nats, V scales <= 0.05); peaked, long-context and large-V inputs move
+    the kernel further, within the bound that test_z_attention_accuracy_gpu.py asserts against a float64 reference."""
     from atom_b200 import ops
     from tests.test_gpu_parity import _kv_fixture, _KV
     rng = np.random.default_rng(0xabc)

@@ -49,7 +49,7 @@ def _lens(P):
 
 # ------------------------------------------------------------------------------------------------ 1. decode vs the oracle
 @pytest.mark.parametrize("theta", [1e4, 5e5, 1e6])
-@pytest.mark.parametrize("P", [8, 16, 32])
+@pytest.mark.parametrize("P", [8, 16, 24, 32, 64])
 @pytest.mark.parametrize("hq,hkv", [(4, 2), (8, 2), (8, 1), (64, 8)])
 def test_gqa_decode_matches_oracle(hq, hkv, P, theta):
     from atom_b200 import ops
