@@ -37,6 +37,12 @@ _SIGNATURES = {
     "atom_reduce_add_rmsnorm_fp16_i4": (_I, [_P, _P, _I64, _I, _I, _P, _P, _P, _F, _P, _I, _I, _P, _P, _P, _P, _P]),
     "atom_append_kv_i4": (_I, [_P] * 9 + [_I] * 5 + [_P]),
     "atom_init_kv_i4": (_I, [_P] * 10 + [_I] * 6 + [_P]),
+    "atom_moe_route_f16": (_I, [_P, _P, _F, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P]),
+    "atom_moe_plan": (_I, [_P, _I, _I, _I, _I, _I, _P, _P, _P]),
+    "atom_moe_gather_i4": (_I, [_P] * 4 + [_I, _I, _I, _P, _I] + [_P] * 5),
+    "atom_gemm_i4_gateup_act_grouped": (_I, [_P] * 13 + [_I, _I, _I64, _I64, _I64, _I64, _P]),
+    "atom_gemm_i4_o16_grouped": (_I, [_P] * 10 + [_I, _I, _I64, _I64, _I64, _I64, _P]),
+    "atom_moe_combine_f16": (_I, [_P] * 4 + [_I, _I, _I, _P, _P]),
 }
 
 _lib = None

@@ -23,6 +23,7 @@
 #include "prefill_kernels.cuh"
 #include "comm_kernels.cuh"
 #include "quant_kernels.cuh"
+#include "moe_kernels.cuh"
 
 namespace {
 
@@ -179,8 +180,10 @@ bool gemm_pdl_enabled() {
 }
 
 // out_channels: channels that get a tile of their own (gate/up: op.N = 2 I weight rows, I output channels)
+// token_tiles: grid.y when it is not the tiles of op.M (grouped mode: the length of the token-tile table)
 template <int BN, int kSplit, int kEpi>
-int launch_gemm(const GemmOperands& op, const atom::GemmArgs& args, cudaStream_t stream, int64_t out_channels = -1) {
+int launch_gemm(const GemmOperands& op, const atom::GemmArgs& args, cudaStream_t stream, int64_t out_channels = -1,
+                int64_t token_tiles = -1) {
   using C = atom::GemmCfg<BN, kSplit, kEpi>;
   auto kern = atom::gemm_i4_kernel<BN, kSplit, kEpi>;
   int rc = ensure_dynamic_smem(kern, C::SMEM_BYTES, "gemm_i4");
@@ -193,7 +196,7 @@ int launch_gemm(const GemmOperands& op, const atom::GemmArgs& args, cudaStream_t
   if ((rc = make_map(&ta8, op.ak, 128, op.M, 128, 128, BN, 1))) return rc;
   const int64_t chan = out_channels > 0 ? out_channels : op.N;
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)((chan + 127) / 128), (unsigned)((op.M + BN - 1) / BN), kSplit);
+  cfg.gridDim = dim3((unsigned)((chan + 127) / 128), (unsigned)(token_tiles > 0 ? token_tiles : (op.M + BN - 1) / BN), kSplit);
   cfg.blockDim = dim3(C::THREADS);
   cfg.dynamicSmemBytes = C::SMEM_BYTES;
   cfg.stream = stream;
@@ -633,6 +636,148 @@ int atom_init_kv_i4(void* kv_data, void* kv_param, const void* kv_indptr, const 
   return launch_k("init_kv_i4", atom::append_kv_kernel, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, (cudaStream_t)stream, kv,
                   (const uint8_t*)k, (const uint8_t*)v, (const __half2*)k_param, (const __half2*)v_param,
                   (const int32_t*)seqlen_indptr, total_tokens);
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------ sparse MoE block
+namespace {
+
+int64_t moe_tiles_max(int64_t slots, int64_t E, int bn) { return std::min(slots, (slots + E * (bn - 1)) / bn); }
+
+
+// both grouped GEMMs: weights stacked over the experts, expert_rows rows each; a = the permuted activations of rows_cap rows
+int gemm_grouped_check(const char* what, const void* a, const void* b, const void* a_scale, const void* b_scale,
+                              const void* a_keeper, const void* b_keeper, const void* a_keeper_scale, const void* b_keeper_scale,
+                              const void* tiles, int num_tiles, int token_tile, int64_t rows_cap, int64_t num_experts,
+                              int64_t expert_rows, int64_t K) {
+  ATOM_REQUIRE(a && b && a_scale && b_scale && a_keeper && b_keeper && a_keeper_scale && b_keeper_scale && tiles,
+               "%s: null pointer argument", what);
+  ATOM_REQUIRE(token_tile == 16 || token_tile == 32 || token_tile == 64, "%s: token_tile=%d must be 16, 32 or 64", what, token_tile);
+  ATOM_REQUIRE(num_tiles > 0 && rows_cap == (int64_t)num_tiles * token_tile,
+               "%s: rows_cap=%lld must be num_tiles=%d x token_tile=%d", what, (long long)rows_cap, num_tiles, token_tile);
+  ATOM_REQUIRE(num_experts >= 1 && num_experts <= atom::MOE_MAX_EXPERTS, "%s: num_experts=%lld must be in [1, 64]", what,
+               (long long)num_experts);
+  ATOM_REQUIRE(K >= 256 && K % 128 == 0, "%s: K=%lld must be a multiple of 128 and >= 256", what, (long long)K);
+  ATOM_REQUIRE(aligned16(a) && aligned16(b) && aligned16(a_keeper) && aligned16(b_keeper) && aligned16(b_scale) && aligned16(b_keeper_scale) &&
+               aligned16(tiles), "%s: operand pointers must be 16-byte aligned", what);
+  ATOM_REQUIRE((reinterpret_cast<uintptr_t>(a_scale) & 3) == 0 && (reinterpret_cast<uintptr_t>(a_keeper_scale) & 3) == 0,
+               "%s: activation scale pointers must be 4-byte aligned", what);
+  ATOM_REQUIRE(num_experts * expert_rows < (1ll << 31) && rows_cap < (1ll << 31) && K < (1ll << 24), "%s: dimension too large", what);
+  return ATOM_OK;
+}
+
+template <int kEpi>
+int gemm_grouped_dispatch(const GemmOperands& op, const atom::GemmArgs& args, int token_tile, int num_tiles, int64_t out_channels,
+                                 cudaStream_t stream) {
+  if (token_tile == 16) return launch_gemm<16, 1, kEpi | atom::EPI_GROUPED>(op, args, stream, out_channels, num_tiles);
+  if (token_tile == 32) return launch_gemm<32, 1, kEpi | atom::EPI_GROUPED>(op, args, stream, out_channels, num_tiles);
+  return launch_gemm<64, 1, kEpi | atom::EPI_GROUPED>(op, args, stream, out_channels, num_tiles);
+}
+
+}  // namespace
+
+extern "C" {
+
+int atom_moe_route_f16(const void* hidden, const void* norm_weight, float eps, const void* reorder_index, const void* router_weight,
+                       int seq_len, int hidden_dim, int num_experts, int top_k, void* topk_ids, void* topk_weights,
+                       void* router_logits, void* normed, void* stream) {
+  ATOM_REQUIRE(hidden && norm_weight && reorder_index && router_weight && topk_ids && topk_weights, "moe_route_f16: null pointer argument");
+  ATOM_REQUIRE(seq_len > 0, "moe_route_f16: seq_len=%d must be positive", seq_len);
+  ATOM_REQUIRE(hidden_dim >= 256 && hidden_dim % 128 == 0 && hidden_dim <= 32768,
+               "moe_route_f16: hidden_dim=%d must be a multiple of 128 in [256, 32768]", hidden_dim);
+  ATOM_REQUIRE(num_experts >= 1 && num_experts <= atom::MOE_MAX_EXPERTS && top_k >= 1 && top_k <= std::min(num_experts, atom::MOE_MAX_TOPK),
+               "moe_route_f16: num_experts=%d must be in [1, 64], top_k=%d in [1, min(num_experts, 8)]", num_experts, top_k);
+  ATOM_REQUIRE(aligned16(hidden) && aligned16(norm_weight) && aligned16(router_weight) && (!normed || aligned16(normed)),
+               "moe_route_f16: hidden, norm_weight, router_weight and normed must be 16-byte aligned");
+  const size_t smem = (size_t)hidden_dim * 6 + (128 + atom::MOE_MAX_EXPERTS) * 4;
+  int rc = ensure_dynamic_smem(atom::moe_route_kernel, 32768 * 6 + (128 + atom::MOE_MAX_EXPERTS) * 4, "moe_route_f16");
+  if (rc) return rc;
+  return launch_k("moe_route_f16", atom::moe_route_kernel, dim3(seq_len), dim3(atom::ROUTE_THREADS), smem, (cudaStream_t)stream,
+                  (const __half*)hidden, (const __half*)norm_weight, (const int16_t*)reorder_index, eps, (const __half*)router_weight,
+                  hidden_dim, num_experts, top_k, (int32_t*)topk_ids, (__half*)topk_weights, (float*)router_logits, (__half*)normed);
+}
+
+int atom_moe_plan(const void* topk_ids, int seq_len, int num_experts, int top_k, int token_tile, int tiles_max, void* dest_row,
+                  void* tiles, void* stream) {
+  ATOM_REQUIRE(topk_ids && dest_row && tiles, "moe_plan: null pointer argument");
+  ATOM_REQUIRE(seq_len > 0 && num_experts >= 1 && num_experts <= atom::MOE_MAX_EXPERTS && top_k >= 1 &&
+               top_k <= std::min(num_experts, atom::MOE_MAX_TOPK),
+               "moe_plan: seq_len=%d must be positive, num_experts=%d in [1, 64], top_k=%d in [1, min(num_experts, 8)]", seq_len,
+               num_experts, top_k);
+  ATOM_REQUIRE(token_tile == 16 || token_tile == 32 || token_tile == 64, "moe_plan: token_tile=%d must be 16, 32 or 64", token_tile);
+  const int64_t slots = (int64_t)seq_len * top_k;
+  ATOM_REQUIRE(slots < (1ll << 30) && tiles_max >= moe_tiles_max(slots, num_experts, token_tile),
+               "moe_plan: tiles_max=%d is below min(T*k, (T*k + E*(BN-1)) / BN) = %lld", tiles_max,
+               (long long)moe_tiles_max(slots, num_experts, token_tile));
+  ATOM_REQUIRE(aligned16(tiles), "moe_plan: tiles must be 16-byte aligned");
+  return launch_k("moe_plan", atom::moe_plan_kernel, dim3(1), dim3(atom::PLAN_THREADS), 0, (cudaStream_t)stream,
+                  (const int32_t*)topk_ids, (int)slots, num_experts, token_tile, tiles_max, (int32_t*)dest_row, (int4*)tiles);
+}
+
+int atom_moe_gather_i4(const void* o_outliers, const void* o_norms, const void* outlier_scales, const void* norm_scales, int seq_len,
+                       int hidden_dim, int top_k, const void* dest_row, int rows_cap, void* p_outliers, void* p_norms,
+                       void* p_outlier_scales, void* p_norm_scales, void* stream) {
+  int rc = quant_check("moe_gather_i4", seq_len, hidden_dim, p_outliers, p_norms, p_outlier_scales, p_norm_scales);
+  if (rc) return rc;
+  ATOM_REQUIRE(o_outliers && o_norms && outlier_scales && norm_scales && dest_row, "moe_gather_i4: null input pointer");
+  ATOM_REQUIRE(top_k >= 1 && top_k <= atom::MOE_MAX_TOPK && rows_cap > 0, "moe_gather_i4: top_k=%d must be in [1, 8], rows_cap=%d positive",
+               top_k, rows_cap);
+  ATOM_REQUIRE(aligned16(o_outliers) && aligned16(o_norms) && aligned16(p_outliers) && aligned16(p_norms),
+               "moe_gather_i4: INT4 / INT8 rows must be 16-byte aligned");
+  return launch_k("moe_gather_i4", atom::moe_gather_kernel, dim3((unsigned)(seq_len * top_k)), dim3(atom::GATHER_THREADS), 0,
+                  (cudaStream_t)stream, (const int8_t*)o_outliers, (const uint8_t*)o_norms, (const __half*)outlier_scales,
+                  (const __half*)norm_scales, hidden_dim, top_k, atom::scale_size(seq_len), (const int32_t*)dest_row, (int8_t*)p_outliers,
+                  (uint8_t*)p_norms, (__half*)p_outlier_scales, (__half*)p_norm_scales, atom::scale_size(rows_cap));
+}
+
+int atom_gemm_i4_gateup_act_grouped(const void* a, const void* b_gu, const void* a_scale, const void* b_scale_gu, const void* a_keeper,
+                                    const void* b_keeper_gu, const void* a_keeper_scale, const void* b_keeper_scale_gu, void* o_outliers,
+                                    void* o_norms, void* outlier_scales, void* norm_scales, const void* tiles, int num_tiles,
+                                    int token_tile, int64_t rows_cap, int64_t num_experts, int64_t I, int64_t K, void* stream) {
+  int rc = gemm_grouped_check("gemm_i4_gateup_act_grouped", a, b_gu, a_scale, b_scale_gu, a_keeper, b_keeper_gu, a_keeper_scale,
+                              b_keeper_scale_gu, tiles, num_tiles, token_tile, rows_cap, num_experts, 2 * I, K);
+  if (rc) return rc;
+  ATOM_REQUIRE(o_outliers && o_norms && outlier_scales && norm_scales, "gemm_i4_gateup_act_grouped: null output pointer");
+  ATOM_REQUIRE(I >= 256 && I % 128 == 0, "gemm_i4_gateup_act_grouped: I=%lld must be a multiple of 128 >= 256", (long long)I);
+  GemmOperands op{a, b_gu, a_keeper, b_keeper_gu, rows_cap, num_experts * 2 * I, K};
+  atom::GemmArgs args{};
+  args.a_scale = (const __half*)a_scale; args.a_keeper_scale = (const __half*)a_keeper_scale;
+  args.b_scale = (const __half*)b_scale_gu; args.b_keeper_scale = (const __half*)b_keeper_scale_gu;
+  args.M = (int)rows_cap; args.N = (int)(2 * I); args.G = (int)(K / 128 - 1); args.lda_scale = atom::scale_size((int)rows_cap);
+  args.trace = g_trace; args.ldb_scale = (int)(2 * I); args.gu_rows = (int)I;
+  args.q8_out = (int8_t*)o_outliers; args.q4_out = (uint8_t*)o_norms; args.q8_scale = (__half*)outlier_scales; args.q4_scale = (__half*)norm_scales;
+  args.tiles = (const int4*)tiles; args.expert_rows = (int)(2 * I);
+  return gemm_grouped_dispatch<atom::EPI_GATEUP>(op, args, token_tile, num_tiles, I, (cudaStream_t)stream);
+}
+
+int atom_gemm_i4_o16_grouped(const void* a, const void* b, const void* a_scale, const void* b_scale, const void* a_keeper,
+                             const void* b_keeper, const void* a_keeper_scale, const void* b_keeper_scale, void* d, const void* tiles,
+                             int num_tiles, int token_tile, int64_t rows_cap, int64_t num_experts, int64_t N, int64_t K, void* stream) {
+  int rc = gemm_grouped_check("gemm_i4_o16_grouped", a, b, a_scale, b_scale, a_keeper, b_keeper, a_keeper_scale, b_keeper_scale, tiles,
+                              num_tiles, token_tile, rows_cap, num_experts, N, K);
+  if (rc) return rc;
+  ATOM_REQUIRE(d && aligned16(d), "gemm_i4_o16_grouped: d must be a 16-byte aligned pointer");
+  ATOM_REQUIRE(N > 0 && N % 8 == 0, "gemm_i4_o16_grouped: N=%lld must be a positive multiple of 8", (long long)N);
+  GemmOperands op{a, b, a_keeper, b_keeper, rows_cap, num_experts * N, K};
+  atom::GemmArgs args{};
+  args.a_scale = (const __half*)a_scale; args.b_scale = (const __half*)b_scale;
+  args.a_keeper_scale = (const __half*)a_keeper_scale; args.b_keeper_scale = (const __half*)b_keeper_scale;
+  args.d = (__half*)d; args.M = (int)rows_cap; args.N = (int)N; args.G = (int)(K / 128 - 1);
+  args.lda_scale = atom::scale_size((int)rows_cap); args.trace = g_trace; args.ldb_scale = (int)N;
+  args.tiles = (const int4*)tiles; args.expert_rows = (int)N;
+  return gemm_grouped_dispatch<atom::EPI_O16>(op, args, token_tile, num_tiles, N, (cudaStream_t)stream);
+}
+
+int atom_moe_combine_f16(const void* y, const void* topk_ids, const void* topk_weights, const void* dest_row, int seq_len, int hidden_dim,
+                         int top_k, void* out, void* stream) {
+  ATOM_REQUIRE(y && topk_ids && topk_weights && dest_row && out, "moe_combine_f16: null pointer argument");
+  ATOM_REQUIRE(seq_len > 0 && hidden_dim > 0 && hidden_dim % 8 == 0 && top_k >= 1 && top_k <= atom::MOE_MAX_TOPK,
+               "moe_combine_f16: seq_len=%d must be positive, hidden_dim=%d a multiple of 8, top_k=%d in [1, 8]", seq_len, hidden_dim, top_k);
+  ATOM_REQUIRE(aligned16(y) && aligned16(out), "moe_combine_f16: y and out must be 16-byte aligned");
+  return launch_k("moe_combine_f16", atom::moe_combine_kernel, dim3(seq_len), dim3(atom::COMBINE_THREADS), 0, (cudaStream_t)stream,
+                  (const __half*)y, (const int32_t*)topk_ids, (const __half*)topk_weights, (const int32_t*)dest_row, top_k, hidden_dim,
+                  (__half*)out);
 }
 
 }  // extern "C"

@@ -48,6 +48,10 @@ struct GemmArgs {
   unsigned long long* trace;     // optional device buffer [ctas][128] of clock64 stamps (atom_gemm_set_trace), else null
   ArArgs ar;                     // EPI_PUSH: D goes to slot [call % 3][rank] of every rank's receive buffer (comm_kernels.cuh);
                                  // the consumer is rmsnorm_quant_kernel's reducing variant
+  // grouped expert GEMM (EPI_GROUPED): blockIdx.y indexes `tiles`, one (expert, first row, valid rows, 0) per token tile
+  // (valid rows 0 = empty); the weights of all experts are stacked, `expert_rows` rows per expert (2I gate/up, H down)
+  const int4* tiles;
+  int expert_rows;
 };
 
 // timeline stamps for pipeline debugging: per CTA  0 start | 1 setup done | 2 main loop done | 3 reduction done | 4 end
@@ -64,11 +68,15 @@ __host__ __device__ __forceinline__ int scale_size(int m) { return m / 16 * 64 +
 
 // EPI_QKV: o16 for the q tiles, o4 for the k and v tiles.  EPI_GATEUP: 256 weight rows per CTA (gate tile + up tile).
 // EPI_PUSH: EPI_O16 whose result goes to every rank's all-reduce receive buffer.
-enum { EPI_O16 = 0, EPI_O4 = 1, EPI_QKV = 2, EPI_GATEUP = 3, EPI_PUSH = 4 };
+// EPI_GROUPED: a mode bit or-ed into EPI_O16 / EPI_GATEUP -- the grouped expert GEMM of the MoE block (moe_kernels.cuh).  A
+// tile of the token-tile table selects the expert (weight rows and scales) and the rows of the permuted activations; rows
+// past the tile's valid count are not stored.  A bit of the epilogue parameter rather than a parameter of its own, so that
+// every other instantiation keeps its symbol and its code.
+enum { EPI_O16 = 0, EPI_O4 = 1, EPI_QKV = 2, EPI_GATEUP = 3, EPI_PUSH = 4, EPI_GROUPED = 8 };
 
 template <int BN, int kSplit, int kEpi>
 struct GemmCfg {
-  static constexpr int ROWS = kEpi == EPI_GATEUP ? 256 : 128;    // weight rows per CTA
+  static constexpr int ROWS = (kEpi & ~EPI_GROUPED) == EPI_GATEUP ? 256 : 128;    // weight rows per CTA
   static constexpr int MT = ROWS / 128;                          // 64-row wgmma tiles per consumer warpgroup
   static constexpr int THREADS = 384;                            // producer warpgroup + two consumer warpgroups
   static constexpr int PACK = BN <= 32 ? 8 : 4;                  // packed ring depth (groups): decode shapes are a weight stream
@@ -91,6 +99,7 @@ struct GemmCfg {
   static_assert(BN * TILE_PITCH * 4 <= OFF_SCALE, "the output tile is staged over the idle operand rings");
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
   static_assert(kSplit == 1 || kEpi == EPI_O16 || kEpi == EPI_PUSH, "the quantising epilogues work on un-split FP32 sums");
+  static_assert(!(kEpi & EPI_GROUPED) || (kSplit == 1 && BN <= 64), "grouped mode: token tiles of 16 / 32 / 64, no K split");
 };
 
 template <int BN, int kSplit, int kEpi>
@@ -101,6 +110,8 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
                const __grid_constant__ CUtensorMap tm_a8,   // INT8 keeper tokens    (box 128 B x BN rows, SW128)
                const GemmArgs args) {
   using C = GemmCfg<BN, kSplit, kEpi>;
+  constexpr bool kGrouped = (kEpi & EPI_GROUPED) != 0;
+  constexpr int kE = kEpi & ~EPI_GROUPED;                    // the epilogue
   constexpr int NR = BN / 2;                                // accumulator registers per 64-row tile
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024-B alignment (SWIZZLE_128B atoms) by offsetting the shared array, NOT by integer-casting the pointer:
@@ -117,8 +128,18 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
   // the warp index through a shuffle: the compiler then knows the role branches below are warp-uniform
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
   // blockIdx.x = output-channel tile: CTAs launched together share the token tile (L2) and stream disjoint weights
-  const int n0 = blockIdx.x * 128, m0 = blockIdx.y * BN;
-  const int n_limit = kEpi == EPI_GATEUP ? args.gu_rows : args.N;   // channels of one weight segment
+  // grouped mode: gtile = the tile's (expert, first row, valid rows, 0).  The table is written by the preceding kernels: nothing of
+  // it, of the activations or of the expert's weights is read before griddepcontrol.wait (no weight prefetch ahead of the
+  // wait in this mode).  Every grouped-only term below sits in a `kGrouped ?` branch, so the other instantiations compile
+  // to the code they had before the mode existed.
+  int4 gtile = make_int4(0, 0, 0, 0);
+  if constexpr (kGrouped) {
+    griddep_wait();
+    gtile = args.tiles[blockIdx.y];
+    if (gtile.z <= 0) return;                                 // empty tile: the whole CTA leaves before any barrier
+  }
+  const int n0 = blockIdx.x * 128, m0 = kGrouped ? gtile.y : blockIdx.y * BN;
+  const int n_limit = kE == EPI_GATEUP ? args.gu_rows : args.N;   // channels of one weight segment
 
   // K split over the cluster: groups [g_begin, g_end) of the G+1 groups (index G = INT8 keeper)
   const int total_groups = args.G + 1;
@@ -156,9 +177,11 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
       const int ps = s % C::PACK, g = g_begin + s;
       if (part != 2) {
         mbar_arrive_expect_tx(&pack_full[ps], C::PACK_W + C::PACK_Q);
-        tma_load_2d(smem + C::OFF_PACK_W + ps * C::PACK_W, &tm_w4, &pack_full[ps], g * 64, n0);
-        if constexpr (kEpi == EPI_GATEUP)
-          tma_load_2d(smem + C::OFF_PACK_W + ps * C::PACK_W + 128 * 64, &tm_w4, &pack_full[ps], g * 64, args.gu_rows + n0);
+        tma_load_2d(smem + C::OFF_PACK_W + ps * C::PACK_W, &tm_w4, &pack_full[ps], g * 64,
+                    kGrouped ? gtile.x * args.expert_rows + n0 : n0);
+        if constexpr (kE == EPI_GATEUP)
+          tma_load_2d(smem + C::OFF_PACK_W + ps * C::PACK_W + 128 * 64, &tm_w4, &pack_full[ps], g * 64,
+                      kGrouped ? gtile.x * args.expert_rows + args.gu_rows + n0 : args.gu_rows + n0);
       }
       if (part != 1) tma_load_2d(smem + C::OFF_PACK_Q + ps * C::PACK_Q, &tm_a4, &pack_full[ps], g * 64, m0);
     };
@@ -170,7 +193,7 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
         const int seg = t / 16, c = t % 16;                         // gate/up: segment 1 = the up rows
         if (n0 + 8 * c < n_limit) sbv = ld_cg_v4(bs_row + (size_t)seg * args.gu_rows + n0 + 8 * c);
       }
-      if (t < BN && m0 + t < args.M) sav = __ushort_as_half(ld_cg_u16(as_row + scale_index(m0 + t)));
+      if (t < BN && m0 + t < (kGrouped ? gtile.y + gtile.z : args.M)) sav = __ushort_as_half(ld_cg_u16(as_row + scale_index(m0 + t)));
     };
     auto store_scales = [&](int slot_idx, const uint4& sbv, __half sav) {
       uint8_t* slot = smem + C::OFF_SCALE + slot_idx * C::SCALE_BYTES;
@@ -183,8 +206,10 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
       for (int s = 0; s < first; ++s) issue_stage(s, 1);
       if (has_keeper) {
         mbar_arrive_expect_tx(keep_full, C::KEEP_TX);
-        tma_load_2d(smem + C::OFF_KEEP_W, &tm_w8, keep_full, 0, n0);
-        if constexpr (kEpi == EPI_GATEUP) tma_load_2d(smem + C::OFF_KEEP_W + 128 * 128, &tm_w8, keep_full, 0, args.gu_rows + n0);
+        tma_load_2d(smem + C::OFF_KEEP_W, &tm_w8, keep_full, 0, kGrouped ? gtile.x * args.expert_rows + n0 : n0);
+        if constexpr (kE == EPI_GATEUP)
+          tma_load_2d(smem + C::OFF_KEEP_W + 128 * 128, &tm_w8, keep_full, 0,
+                      kGrouped ? gtile.x * args.expert_rows + args.gu_rows + n0 : args.gu_rows + n0);
       }
       griddep_wait();                       // from here on the preceding kernel's output (the activations) may be read
       for (int s = 0; s < first; ++s) issue_stage(s, 2);
@@ -195,14 +220,14 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
     uint4 sbv;
     __half sav;
     if (has_keeper) {
-      load_scales(args.b_keeper_scale, args.a_keeper_scale, sbv, sav);
+      load_scales(kGrouped ? args.b_keeper_scale + (size_t)gtile.x * args.expert_rows : args.b_keeper_scale, args.a_keeper_scale, sbv, sav);
       store_scales(C::EXP, sbv, sav);
       __syncwarp();
       if (lane == 0) mbar_arrive(keep_full);
     }
     for (int s = 0; s < n4; ++s) {
       const int ps = s % C::PACK, es = s % C::EXP, g = g_begin + s;
-      load_scales(args.b_scale + (size_t)g * args.ldb_scale, args.a_scale + (size_t)g * args.lda_scale, sbv, sav);
+      load_scales((kGrouped ? args.b_scale + (size_t)gtile.x * args.G * args.ldb_scale : args.b_scale) + (size_t)g * args.ldb_scale, args.a_scale + (size_t)g * args.lda_scale, sbv, sav);
       if (t == 0 && s >= 1 && s + C::PACK - 1 < n4) {               // refill the slot the previous group has left
         const int nx = s + C::PACK - 1;
         mbar_wait(&pack_empty[nx % C::PACK], ((nx / C::PACK) - 1) & 1);
@@ -349,14 +374,14 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
     constexpr float kInv = 1.0f / 256.0f;   // exact: removes the 16 * 16 operand factor
     // q/k/v: tiles [0, seg_tiles) are q, the next kv_tiles k, the last kv_tiles v (kv_tiles == seg_tiles: three equal parts)
     const int bx = (int)blockIdx.x;
-    const int seg = kEpi == EPI_QKV ? (bx < args.seg_tiles ? 0 : (bx < args.seg_tiles + args.kv_tiles ? 1 : 2)) : 0;
-    const int otile = kEpi == EPI_QKV ? (seg == 0 ? bx : bx - args.seg_tiles - (seg - 1) * args.kv_tiles) : bx;
-    const int n_out_dim = kEpi == EPI_QKV ? (seg == 0 ? args.seg_tiles : args.kv_tiles) * 128 : args.N;   // row length of the output this tile writes
+    const int seg = kE == EPI_QKV ? (bx < args.seg_tiles ? 0 : (bx < args.seg_tiles + args.kv_tiles ? 1 : 2)) : 0;
+    const int otile = kE == EPI_QKV ? (seg == 0 ? bx : bx - args.seg_tiles - (seg - 1) * args.kv_tiles) : bx;
+    const int n_out_dim = kE == EPI_QKV ? (seg == 0 ? args.seg_tiles : args.kv_tiles) * 128 : args.N;   // row length of the output this tile writes
     const int n_out = otile * 128 + lane * 4;
-    const bool o16 = kEpi == EPI_O16 || kEpi == EPI_PUSH || (kEpi == EPI_QKV && seg == 0);
+    const bool o16 = kE == EPI_O16 || kE == EPI_PUSH || (kE == EPI_QKV && seg == 0);
     for (int tk = cw; tk < BN; tk += 8) {
       const int m = m0 + tk;
-      if (m >= args.M) break;
+      if (m >= (kGrouped ? gtile.y + gtile.z : args.M)) break;
       if (kSplit > 1 && (tk % kSplit) != (int)krank) continue;  // split-K: rank r reduces + stores the token rows r mod kSplit
       float v[4];
       {
@@ -376,7 +401,7 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
           v[e] = sum;
         }
       }
-      if constexpr (kEpi == EPI_GATEUP) {
+      if constexpr (kE == EPI_GATEUP) {
         // SiLU(gate) * up, then the dynamic quantisation of activate_fp16_i4 (Activate.cuh:102-166) for this 128-channel
         // group of the token.  Both projections are rounded to FP16 first, as they are when the reference stores them
         // between the kernels.
@@ -417,7 +442,7 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
         }
       } else if (o16) {
         __half2 h0 = __floats2half2_rn(v[0] * kInv, v[1] * kInv), h1 = __floats2half2_rn(v[2] * kInv, v[3] * kInv);
-        if constexpr (kEpi == EPI_PUSH) {
+        if constexpr (kE == EPI_PUSH) {
           // fused all-reduce, push half: the row goes to slot [call % 3][rank] of EVERY rank's receive buffer (-0.0, the
           // buffers' "not yet arrived" pattern, travels as +0.0) as 16-byte stores of 8 consecutive channels: 2-byte stores
           // over NVLink cost an order of magnitude more per byte.  The following add+RMSNorm kernel polls and sums the slots.
@@ -439,8 +464,8 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
         }
       } else {
         // o4 (DenseLayerGEMM_i4_o4.cu:705-787): per (token, 128-channel head) asymmetric INT4 with the reference's |v| min/max
-        uint8_t* d4 = (kEpi == EPI_QKV && seg == 2) ? args.d4_v : args.d4;
-        __half2* d_scale = (kEpi == EPI_QKV && seg == 2) ? args.d_scale_v : args.d_scale;
+        uint8_t* d4 = (kE == EPI_QKV && seg == 2) ? args.d4_v : args.d4;
+        __half2* d_scale = (kE == EPI_QKV && seg == 2) ? args.d_scale_v : args.d_scale;
         uint32_t umx = 0u, umn = 0x7f800000u;
 #pragma unroll
         for (int e = 0; e < 4; ++e) {

@@ -402,3 +402,141 @@ def append_kv_i4(kv, k, v, k_param, v_param, layer_idx):
                                                 kv.indicies.data_ptr(), kv.last_page_offset.data_ptr(), k.data_ptr(),
                                                 v.data_ptr(), k_param.data_ptr(), v_param.data_ptr(), L, layer_idx, H,
                                                 P, B, _stream(k)), "append_kv_i4")
+
+
+# ------------------------------------------------------------------------------------------------ sparse MoE block (Mixtral)
+def moe_token_tile(seq_len, num_experts, top_k):
+    """Token tile of the grouped expert GEMM: the smallest of 16 / 32 / 64 that holds the mean rows per expert."""
+    mean = -(-int(seq_len) * int(top_k) // int(num_experts))
+    return 16 if mean <= 16 else (32 if mean <= 32 else 64)
+
+
+def moe_tiles(seq_len, num_experts, top_k):
+    """(BN, tiles_max, rows_cap) of one MoE block: the token tile, the length of the tile table (every expert's segment padded to
+    BN rows: at most min(T*k, (T*k + E*(BN-1)) // BN) tiles) and the rows of the permuted workspace.  Host-known sizes only, so
+    the block can be captured in a CUDA graph whatever the routing."""
+    bn = moe_token_tile(seq_len, num_experts, top_k)
+    slots = int(seq_len) * int(top_k)
+    tiles_max = min(slots, (slots + int(num_experts) * (bn - 1)) // bn)
+    return bn, tiles_max, tiles_max * bn
+
+
+def moe_route_f16(hidden_sum, norm_weight, reorder_index, eps, router_weight, top_k, router_logits=False, normed=False):
+    """EXTENSION: the FP router of the MoE block on the FP16 normalised row (formed exactly as rmsnorm_fp16_i4 forms it, in the
+    reordered channel order of `router_weight` f16 [E, H]).  Returns (topk_ids i32 [T,k], topk_weights f16 [T,k]) plus, on request,
+    the FP32 logits [T,E] and the normalised row f16 [T,H]."""
+    if isinstance(norm_weight, torch.Tensor) and norm_weight.dtype != torch.float16:
+        norm_weight = norm_weight.to(torch.float16)
+    _req_width("moe_route_f16", f16_hidden_sum_2=hidden_sum, f16_norm_weight_2=norm_weight, reorder_index_2=reorder_index,
+               f16_router_weight_2=router_weight)
+    _req_cuda(hidden_sum, norm_weight, reorder_index, router_weight)
+    t, h = hidden_sum.shape
+    e = router_weight.size(0)
+    if router_weight.shape != (e, h) or norm_weight.numel() != h or reorder_index.numel() != h:
+        raise RuntimeError("moe_route_f16: router_weight must be [E, H], norm_weight and reorder_index [H]")
+    dev = hidden_sum.device
+    ids = torch.empty((t, top_k), dtype=torch.int32, device=dev)
+    w = torch.empty((t, top_k), dtype=torch.float16, device=dev)
+    lg = torch.empty((t, e), dtype=torch.float32, device=dev) if router_logits else None
+    yn = torch.empty((t, h), dtype=torch.float16, device=dev) if normed else None
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().atom_moe_route_f16(hidden_sum.data_ptr(), norm_weight.data_ptr(), float(eps), reorder_index.data_ptr(),
+                                                 router_weight.data_ptr(), t, h, e, int(top_k), ids.data_ptr(), w.data_ptr(),
+                                                 lg.data_ptr() if lg is not None else None, yn.data_ptr() if yn is not None else None,
+                                                 _stream(hidden_sum)), "moe_route_f16")
+    return (ids, w) + ((lg,) if router_logits else ()) + ((yn,) if normed else ())
+
+
+def moe_plan(topk_ids, num_experts, token_tile=None, tiles_max=None):
+    """EXTENSION: (dest_row i32 [T,k], tiles i32 [tiles_max,4]) of the routing -- see include/atom_b200.h.  token_tile / tiles_max
+    default to moe_tiles()."""
+    _req_width("moe_plan", topk_ids_4=topk_ids)
+    _req_cuda(topk_ids)
+    t, k = topk_ids.shape
+    bn, tmax, _ = moe_tiles(t, num_experts, k)
+    bn = bn if token_tile is None else int(token_tile)
+    tmax = tmax if tiles_max is None else int(tiles_max)
+    dest = torch.empty((t, k), dtype=torch.int32, device=topk_ids.device)
+    tiles = torch.empty((tmax, 4), dtype=torch.int32, device=topk_ids.device)
+    with torch.cuda.device(topk_ids.device):
+        _lib.check(_lib.lib().atom_moe_plan(topk_ids.data_ptr(), t, int(num_experts), k, bn, tmax, dest.data_ptr(), tiles.data_ptr(),
+                                            _stream(topk_ids)), "moe_plan")
+    return dest, tiles
+
+
+def moe_gather_i4(x, dest_row, rows_cap, out=None):
+    """EXTENSION: the activation 4-tuple `x` of T tokens permuted into the experts' segments: a 4-tuple of rows_cap rows (scales in
+    the layout of S(rows_cap)).  `out`: an existing 4-tuple to fill (pad rows keep what they held)."""
+    o8, o4, s8, s4 = x
+    _req_width("moe_gather_i4", o_outliers_1=o8, o_norms_1=o4, f16_outlier_scales_2=s8, f16_norm_scales_2=s4, dest_row_4=dest_row)
+    _req_cuda(o8, o4, s8, s4, dest_row)
+    t, k = dest_row.shape
+    h = o4.size(1) * 2 + 128
+    if o8.shape != (t, 128) or o4.size(0) != t:
+        raise RuntimeError("moe_gather_i4: the tuple must hold one row per token of dest_row")
+    out = out if out is not None else _quant_outputs(int(rows_cap), h, o8.device)
+    with torch.cuda.device(o8.device):
+        _lib.check(_lib.lib().atom_moe_gather_i4(o8.data_ptr(), o4.data_ptr(), s8.data_ptr(), s4.data_ptr(), t, h, k, dest_row.data_ptr(),
+                                                 int(rows_cap), out[0].data_ptr(), out[1].data_ptr(), out[2].data_ptr(), out[3].data_ptr(),
+                                                 _stream(o8)), "moe_gather_i4")
+    return out
+
+
+def _grouped_args(what, x, w4, s4, w8, s8, tiles, token_tile):
+    o8, o4, xs8, xs4 = x
+    _req_width(what, a_1=o4, b_1=w4, f16_a_scale_2=xs4, f16_b_scale_2=s4, a_keeper_1=o8, b_keeper_1=w8, f16_a_keeper_scale_2=xs8,
+               f16_b_keeper_scale_2=s8, tiles_4=tiles)
+    _req_cuda(o4, w4, xs4, s4, o8, w8, xs8, s8, tiles)
+    rows_cap, k = o8.size(0), o4.size(1) * 2 + 128
+    if w4.dim() != 3 or w8.dim() != 3 or w4.shape[:2] != w8.shape[:2] or w4.size(2) * 2 + 128 != k or \
+            s4.shape != (w4.size(0), k // 128 - 1, w4.size(1)) or s8.shape != w4.shape[:2]:
+        raise RuntimeError(f"{what}: weights must be stacked [E, N, ...] with scales [E, K/128-1, N] and [E, N]")
+    if rows_cap != tiles.size(0) * int(token_tile):
+        raise RuntimeError(f"{what}: the permuted activations must have tiles x token_tile rows")
+    return rows_cap, k
+
+
+def dense_layer_gemm_i4_gateup_act_grouped(x, w13_int4, w13_scale, w13_int8, w13_keeper_scale, tiles, token_tile):
+    """EXTENSION: the gate/up projections + SiLU(gate) * up + quantisation of every expert in one launch over the permuted
+    activation tuple `x` (moe_gather_i4) and the tile table (moe_plan).  w13_* are stacked [E, 2I, ...] (gate rows, then up rows,
+    per expert).  Returns the activation tuple of the down projection (rows_cap rows; pad rows unwritten)."""
+    rows_cap, k = _grouped_args("dense_layer_gemm_i4_gateup_act_grouped", x, w13_int4, w13_scale, w13_int8, w13_keeper_scale, tiles,
+                                token_tile)
+    e, n2 = w13_int4.shape[:2]
+    out = _quant_outputs(rows_cap, n2 // 2, x[0].device)
+    with torch.cuda.device(x[0].device):
+        _lib.check(_lib.lib().atom_gemm_i4_gateup_act_grouped(x[1].data_ptr(), w13_int4.data_ptr(), x[3].data_ptr(), w13_scale.data_ptr(),
+                                                              x[0].data_ptr(), w13_int8.data_ptr(), x[2].data_ptr(),
+                                                              w13_keeper_scale.data_ptr(), out[0].data_ptr(), out[1].data_ptr(),
+                                                              out[2].data_ptr(), out[3].data_ptr(), tiles.data_ptr(), tiles.size(0),
+                                                              int(token_tile), rows_cap, e, n2 // 2, k, _stream(x[0])),
+                   "dense_layer_gemm_i4_gateup_act_grouped")
+    return out
+
+
+def dense_layer_gemm_i4_fp16_grouped(x, w2_int4, w2_scale, w2_int8, w2_keeper_scale, tiles, token_tile):
+    """EXTENSION: the down projection of every expert in one launch; w2_* stacked [E, H, ...].  Returns f16 [rows_cap, H]."""
+    rows_cap, k = _grouped_args("dense_layer_gemm_i4_fp16_grouped", x, w2_int4, w2_scale, w2_int8, w2_keeper_scale, tiles, token_tile)
+    e, n = w2_int4.shape[:2]
+    d = torch.empty((rows_cap, n), dtype=torch.float16, device=x[0].device)
+    with torch.cuda.device(x[0].device):
+        _lib.check(_lib.lib().atom_gemm_i4_o16_grouped(x[1].data_ptr(), w2_int4.data_ptr(), x[3].data_ptr(), w2_scale.data_ptr(),
+                                                       x[0].data_ptr(), w2_int8.data_ptr(), x[2].data_ptr(), w2_keeper_scale.data_ptr(),
+                                                       d.data_ptr(), tiles.data_ptr(), tiles.size(0), int(token_tile), rows_cap, e, n, k,
+                                                       _stream(x[0])), "dense_layer_gemm_i4_fp16_grouped")
+    return d
+
+
+def moe_combine_f16(y, topk_ids, topk_weights, dest_row):
+    """EXTENSION: out f16 [T,H] = the experts' outputs weighted and summed per token in ascending expert order (FP16 products
+    and adds from +0.0), bit for bit the index_add_ loop of the simulator."""
+    _req_width("moe_combine_f16", f16_y_2=y, topk_ids_4=topk_ids, f16_topk_weights_2=topk_weights, dest_row_4=dest_row)
+    _req_cuda(y, topk_ids, topk_weights, dest_row)
+    t, k = topk_ids.shape
+    if topk_weights.shape != (t, k) or dest_row.shape != (t, k):
+        raise RuntimeError("moe_combine_f16: topk_ids, topk_weights and dest_row must all be [T, k]")
+    out = torch.empty((t, y.size(1)), dtype=torch.float16, device=y.device)
+    with torch.cuda.device(y.device):
+        _lib.check(_lib.lib().atom_moe_combine_f16(y.data_ptr(), topk_ids.data_ptr(), topk_weights.data_ptr(), dest_row.data_ptr(), t,
+                                                   y.size(1), k, out.data_ptr(), _stream(y)), "moe_combine_f16")
+    return out

@@ -155,6 +155,13 @@ class QMixtralDecoderLayer(nn.Module):
             outputs += (router_logits,)
         return outputs
 
+    @torch.no_grad()
+    def to_int4(self, device="cuda"):
+        """Real-INT4 serving layer (atom_b200.mixtral.MixtralDecoderLayer) from this simulated one; every QLinearLayer must still
+        hold (or have saved, via quant()) its reordered FP weight.  See export.int4_mixtral_decoder_layer."""
+        from .export import int4_mixtral_decoder_layer
+        return int4_mixtral_decoder_layer(self, device)
+
 
 # ------------------------------------------------------------------------------------------------ test stand-ins
 class _ToyExpert(nn.Module):

@@ -205,6 +205,57 @@ ATOM_API int atom_reduce_add_rmsnorm_fp16_i4(const void* peer_buffers, void* sta
                                     int seq_len, int hidden_dim, void* o_outliers, void* o_norms, void* outlier_scales,
                                     void* norm_scales, void* stream);
 
+/* EXTENSION (Mixtral sparse MoE block, csrc/moe_kernels.cuh).  E = num_experts <= 64 experts, k = top_k <= min(E, 8) per token.
+ * One block: atom_add_rmsnorm_fp16_i4 (the activation tuple every expert reads: all experts share expert 0's channel orders),
+ * route, plan, gather, grouped gate/up+act, grouped down, combine -- seven launches whose sizes depend only on (T, E, k), so the
+ * block is graph-capturable with data-dependent routing.  BN = token tile = 16 / 32 / 64 for ceil(T*k/E) <= 16 / 32 / more;
+ * tiles_max = min(T*k, (T*k + E*(BN-1)) / BN); rows_cap = tiles_max * BN rows of permuted workspace.
+ *
+ * atom_moe_route_f16: the FP router on the FP16 normalised row.  hidden f16 [T,H] (the residual sum the add+RMSNorm returned),
+ *   norm_weight f16 [H], reorder_index i16 [H], router_weight f16 [E,H] in the reordered channel order.  y = half(float(x) *
+ *   float(w) * rstd) exactly as atom_rmsnorm_fp16_i4 forms it; logits FP32; softmax FP32; top-k on the logits, an exact tie goes
+ *   to the lower expert index.  topk_ids i32 [T,k], topk_weights f16 [T,k] = fp16(p_i / sum of the selected p); optional
+ *   (NULL = not written): router_logits f32 [T,E], normed f16 [T,H] (y). */
+ATOM_API int atom_moe_route_f16(const void* hidden, const void* norm_weight, float eps, const void* reorder_index, const void* router_weight,
+                       int seq_len, int hidden_dim, int num_experts, int top_k, void* topk_ids, void* topk_weights,
+                       void* router_logits, void* normed, void* stream);
+
+/* atom_moe_plan: one CTA.  dest_row i32 [T,k]: the permuted row of every (token, slot); expert e's segment starts at
+ * sum_{e'<e} ceil(count_e'/BN)*BN, tokens ascending inside it.  tiles i32 [tiles_max,4] = (expert, first row, valid rows, 0), the
+ * non-empty tiles in expert order, then (0,0,0,0).  Ids outside [0,E) are not routed (dest_row -1). */
+ATOM_API int atom_moe_plan(const void* topk_ids, int seq_len, int num_experts, int top_k, int token_tile, int tiles_max, void* dest_row,
+                  void* tiles, void* stream);
+
+/* atom_moe_gather_i4: copy each routed token's rows of the activation tuple (o_outliers i8 [T,128], o_norms u8 [T,(H-128)/2],
+ * scales in the layout of S(T)) to row dest_row of the permuted tuple (p_* with rows_cap rows, scales in the layout of
+ * S(rows_cap)).  Pad rows are not written. */
+ATOM_API int atom_moe_gather_i4(const void* o_outliers, const void* o_norms, const void* outlier_scales, const void* norm_scales, int seq_len,
+                       int hidden_dim, int top_k, const void* dest_row, int rows_cap, void* p_outliers, void* p_norms,
+                       void* p_outlier_scales, void* p_norm_scales, void* stream);
+
+/* Grouped expert GEMMs over the permuted activations (rows_cap = num_tiles * token_tile rows) and weights stacked over the experts:
+ *   gate/up: b_gu u8 [E, 2I, (K-128)/2], b_scale_gu f16 [E, K/128-1, 2I], b_keeper_gu i8 [E, 2I, 128], b_keeper_scale_gu f16 [E, 2I]
+ *            (per expert rows [0,I) = gate (w1), [I,2I) = up (w3)); outputs the activation tuple of rows_cap rows for the down
+ *            projection, as atom_gemm_i4_gateup_act;
+ *   down:    b u8 [E, N, (K-128)/2], b_scale f16 [E, K/128-1, N], b_keeper i8 [E, N, 128], b_keeper_scale f16 [E, N]; d f16 [rows_cap, N].
+ * Tile j of the plan's table computes its rows against its expert's weights; rows past its valid count are not stored, empty
+ * tiles return at once.  No K split: every stored row is bit-identical to the per-expert atom_gemm_i4_gateup_act / atom_gemm_i4_o16
+ * call with ATOM_GEMM_NO_SPLITK on that expert's rows.  Everything (the tile table included) is read after the preceding kernel
+ * has completed. */
+ATOM_API int atom_gemm_i4_gateup_act_grouped(const void* a, const void* b_gu, const void* a_scale, const void* b_scale_gu, const void* a_keeper,
+                                    const void* b_keeper_gu, const void* a_keeper_scale, const void* b_keeper_scale_gu, void* o_outliers,
+                                    void* o_norms, void* outlier_scales, void* norm_scales, const void* tiles, int num_tiles,
+                                    int token_tile, int64_t rows_cap, int64_t num_experts, int64_t I, int64_t K, void* stream);
+ATOM_API int atom_gemm_i4_o16_grouped(const void* a, const void* b, const void* a_scale, const void* b_scale, const void* a_keeper,
+                             const void* b_keeper, const void* a_keeper_scale, const void* b_keeper_scale, void* d, const void* tiles,
+                             int num_tiles, int token_tile, int64_t rows_cap, int64_t num_experts, int64_t N, int64_t K, void* stream);
+
+/* atom_moe_combine_f16: out f16 [T,H] = sum over t's slots in ascending expert order of fp16(y[dest_row] * w), one FP16 rounding per
+ * product and per add, from +0.0 -- bit for bit `out = zeros; out.index_add_(0, tok_e, (y_e * w_e).half())` expert by expert.
+ * y f16 [rows_cap,H] (the down projection).  The result is the MoE delta of the residual stream. */
+ATOM_API int atom_moe_combine_f16(const void* y, const void* topk_ids, const void* topk_weights, const void* dest_row, int seq_len, int hidden_dim,
+                         int top_k, void* out, void* stream);
+
 /* replaces append_kv_i4 (punica_ops.cc:166-209 -> FlashInferAppendKvKernel_i4<128>, flashinfer_impl.cuh:73-96)
  *   k,v u8 [B,H,64]  k_param,v_param f16 [B,H,2] */
 ATOM_API int atom_append_kv_i4(void* kv_data, void* kv_param, const void* kv_indptr, const void* kv_indices,
