@@ -536,73 +536,67 @@ static int kv_check(const char* what, const void* data, const void* param, const
   return ATOM_OK;
 }
 
+}  // extern "C"
+
+// one launch of batch_decode_kernel<G, kMaxTpl, kP>
+template <int G, int kMaxTpl, int kP>
+static int launch_decode(const char* what, void* o, const void* q, const atom::KvArgs& kv, float log2_theta, cudaStream_t stream) {
+  int rc = ensure_dynamic_smem(atom::batch_decode_kernel<G, kMaxTpl, kP>, 100 * 1024, what);
+  if (rc) return rc;
+  return launch_k(what, atom::batch_decode_kernel<G, kMaxTpl, kP>, dim3(kv.B, kv.H), dim3(atom::dec_threads(G)),
+                  atom::batch_decode_smem_bytes(G, kv.P), stream, (__half*)o, (const __half*)q, kv, log2_theta);
+}
+
+// the page sizes 16 / 32 of the reference benchmarks get their strides as immediates; for G = 1 a page of at most 32 tokens
+// has at most four tokens per lane
+template <int G>
+static int dispatch_decode(const char* what, void* o, const void* q, const atom::KvArgs& kv, float log2_theta, cudaStream_t stream) {
+  if (kv.P == 16) return launch_decode<G, 2, 16>(what, o, q, kv, log2_theta, stream);
+  if (kv.P == 32) return launch_decode<G, 4, 32>(what, o, q, kv, log2_theta, stream);
+  if (G == 1 && kv.P <= 32) return launch_decode<1, 4, 0>(what, o, q, kv, log2_theta, stream);
+  return launch_decode<G, 8, 0>(what, o, q, kv, log2_theta, stream);
+}
+
+static int batch_decode(const char* what, void* o, const void* q, const void* kv_data, const void* kv_param, const void* kv_indptr,
+                        const void* kv_indices, const void* last_page_offset, int num_layers, int layer_idx, int num_q_heads,
+                        int num_kv_heads, int page_size, int batch_size, float rope_theta, void* stream) {
+  int rc = kv_check(what, kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx, num_kv_heads, page_size,
+                    batch_size);
+  if (rc) return rc;
+  ATOM_REQUIRE(o && q, "%s: null q/o", what);
+  ATOM_REQUIRE(num_q_heads > 0 && num_q_heads % num_kv_heads == 0,
+               "%s: num_q_heads=%d must be a positive multiple of num_kv_heads=%d", what, num_q_heads, num_kv_heads);
+  ATOM_REQUIRE(rope_theta > 1.f && rope_theta < 1e30f, "%s: rope_theta=%g must be a finite base above 1", what, (double)rope_theta);
+  const int group = num_q_heads / num_kv_heads;
+  if (group != 1 && group != 2 && group != 4 && group != 8)
+    return fail(ATOM_E_UNSUPPORTED, "%s: %d query heads per KV head (num_q_heads=%d, num_kv_heads=%d); supported group sizes are 1, 2, "
+                                    "4 and 8", what, group, num_q_heads, num_kv_heads);
+  ATOM_REQUIRE(page_size % 8 == 0 && page_size <= 64, "%s: page_size=%d must be a multiple of 8, at most 64", what, page_size);
+  ATOM_REQUIRE(aligned16(kv_data) && aligned16(kv_param), "%s: KV pool must be 16-byte aligned", what);
+  const atom::KvArgs kv{(uint8_t*)kv_data, (__half2*)kv_param, (const int32_t*)kv_indptr, (const int32_t*)kv_indices,
+                        (const int32_t*)last_page_offset, num_layers, layer_idx, num_kv_heads, page_size, batch_size};
+  const float log2_theta = log2f(rope_theta);
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (group == 1) return dispatch_decode<1>(what, o, q, kv, log2_theta, st);
+  if (group == 2) return dispatch_decode<2>(what, o, q, kv, log2_theta, st);
+  if (group == 4) return dispatch_decode<4>(what, o, q, kv, log2_theta, st);
+  return dispatch_decode<8>(what, o, q, kv, log2_theta, st);
+}
+
+extern "C" {
+
 int atom_batch_decode_i4(void* o, const void* q, const void* kv_data, const void* kv_param, const void* kv_indptr,
                          const void* kv_indices, const void* last_page_offset, int num_layers, int layer_idx,
                          int num_heads, int page_size, int batch_size, void* stream) {
-  int rc = kv_check("batch_decode_i4", kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx,
-                    num_heads, page_size, batch_size);
-  if (rc) return rc;
-  ATOM_REQUIRE(o && q, "batch_decode_i4: null q/o");
-  ATOM_REQUIRE(page_size % 8 == 0 && page_size <= 64, "batch_decode_i4: page_size=%d must be a multiple of 8, at most 64", page_size);
-  ATOM_REQUIRE(aligned16(kv_data) && aligned16(kv_param), "batch_decode_i4: KV pool must be 16-byte aligned");
-  atom::KvArgs kv{(uint8_t*)kv_data, (__half2*)kv_param, (const int32_t*)kv_indptr, (const int32_t*)kv_indices,
-                  (const int32_t*)last_page_offset, num_layers, layer_idx, num_heads, page_size, batch_size};
-  const size_t smem = atom::batch_decode_smem_bytes(page_size);
-#define ATOM_DECODE(TPL, PG)                                                                                              \
-  do {                                                                                                                    \
-    if ((rc = ensure_dynamic_smem(atom::batch_decode_kernel<TPL, PG>, 100 * 1024, "batch_decode_i4"))) return rc;         \
-    return launch_k("batch_decode_i4", atom::batch_decode_kernel<TPL, PG>, dim3(batch_size, num_heads),                   \
-                    dim3(atom::DEC_THREADS), smem, (cudaStream_t)stream, (__half*)o, (const __half*)q, kv);               \
-  } while (0)
-  if (page_size == 16) ATOM_DECODE(2, 16);      // the two page sizes of the harness / the reference benchmarks: strides as immediates
-  if (page_size == 32) ATOM_DECODE(4, 32);
-  if (page_size <= 32) ATOM_DECODE(4, 0);
-  ATOM_DECODE(8, 0);
-#undef ATOM_DECODE
+  return batch_decode("batch_decode_i4", o, q, kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx,
+                      num_heads, num_heads, page_size, batch_size, 1e4f, stream);
 }
 
 int atom_batch_decode_gqa_i4(void* o, const void* q, const void* kv_data, const void* kv_param, const void* kv_indptr,
                              const void* kv_indices, const void* last_page_offset, int num_layers, int layer_idx,
                              int num_q_heads, int num_kv_heads, int page_size, int batch_size, float rope_theta, void* stream) {
-  int rc = kv_check("batch_decode_gqa_i4", kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx,
-                    num_kv_heads, page_size, batch_size);
-  if (rc) return rc;
-  ATOM_REQUIRE(o && q, "batch_decode_gqa_i4: null q/o");
-  ATOM_REQUIRE(num_q_heads > 0 && num_q_heads % num_kv_heads == 0,
-               "batch_decode_gqa_i4: num_q_heads=%d must be a positive multiple of num_kv_heads=%d", num_q_heads, num_kv_heads);
-  ATOM_REQUIRE(rope_theta > 1.f && rope_theta < 1e30f, "batch_decode_gqa_i4: rope_theta=%g must be a finite base above 1", (double)rope_theta);
-  const int group = num_q_heads / num_kv_heads;
-  // multi-head attention with the reference's RoPE base: the kernel every existing caller runs, untouched
-  if (group == 1 && rope_theta == 10000.f)
-    return atom_batch_decode_i4(o, q, kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx, num_kv_heads,
-                                page_size, batch_size, stream);
-  if (group != 1 && group != 2 && group != 4 && group != 8)
-    return fail(ATOM_E_UNSUPPORTED, "batch_decode_gqa_i4: %d query heads per KV head (num_q_heads=%d, num_kv_heads=%d); supported group "
-                                    "sizes are 1, 2, 4 and 8", group, num_q_heads, num_kv_heads);
-  ATOM_REQUIRE(page_size % 8 == 0 && page_size <= 64, "batch_decode_gqa_i4: page_size=%d must be a multiple of 8, at most 64", page_size);
-  ATOM_REQUIRE(aligned16(kv_data) && aligned16(kv_param), "batch_decode_gqa_i4: KV pool must be 16-byte aligned");
-  atom::KvArgs kv{(uint8_t*)kv_data, (__half2*)kv_param, (const int32_t*)kv_indptr, (const int32_t*)kv_indices,
-                  (const int32_t*)last_page_offset, num_layers, layer_idx, num_kv_heads, page_size, batch_size};
-  const size_t smem = atom::batch_decode_gqa_smem_bytes(page_size);
-  const float log2_theta = log2f(rope_theta);
-#define ATOM_DECODE_GQA(G_, TPL, PG)                                                                                         \
-  do {                                                                                                                       \
-    if ((rc = ensure_dynamic_smem(atom::batch_decode_gqa_kernel<G_, TPL, PG>, 100 * 1024, "batch_decode_gqa_i4"))) return rc; \
-    return launch_k("batch_decode_gqa_i4", atom::batch_decode_gqa_kernel<G_, TPL, PG>, dim3(batch_size, num_kv_heads),       \
-                    dim3(atom::GQA_THREADS), smem, (cudaStream_t)stream, (__half*)o, (const __half*)q, kv, log2_theta);      \
-  } while (0)
-#define ATOM_DECODE_GQA_P(G_)                    \
-  do {                                           \
-    if (page_size == 16) ATOM_DECODE_GQA(G_, 2, 16); \
-    if (page_size == 32) ATOM_DECODE_GQA(G_, 4, 32); \
-    ATOM_DECODE_GQA(G_, 8, 0);                   \
-  } while (0)
-  if (group == 1) ATOM_DECODE_GQA(1, 8, 0);       // multi-head attention with another RoPE base: eight page stripes, any page size
-  if (group == 2) ATOM_DECODE_GQA_P(2);
-  if (group == 4) ATOM_DECODE_GQA_P(4);
-  ATOM_DECODE_GQA_P(8);
-#undef ATOM_DECODE_GQA_P
-#undef ATOM_DECODE_GQA
+  return batch_decode("batch_decode_gqa_i4", o, q, kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx,
+                      num_q_heads, num_kv_heads, page_size, batch_size, rope_theta, stream);
 }
 
 int atom_append_kv_i4(void* kv_data, void* kv_param, const void* kv_indptr, const void* kv_indices,

@@ -213,9 +213,8 @@ class LlamaAttention(nn.Module):
         if self._qkv is not None:
             outlier, norms, outlier_scales, norm_scales = hidden_states
             w4, s4, w8, s8 = self._qkv
-            kv_rows = None if self.num_kv_heads == self.num_heads else self.num_kv_heads * self.head_dim
             q_proj, k_proj, v_proj = ops.dense_layer_gemm_i4_qkv(norms, w4, norm_scales, s4, outlier, w8, outlier_scales, s8,
-                                                                 kv_rows=kv_rows)
+                                                                 kv_rows=self.num_kv_heads * self.head_dim)
         else:
             q_proj, k_proj, v_proj = run_concurrently([self.q_proj, self.k_proj, self.v_proj], hidden_states)
         nvtx.range_pop()

@@ -226,26 +226,7 @@ def dense_layer_gemm_i4_qkv(a, b_qkv, a_scale, b_scale_qkv, a_keeper, b_keeper_q
     _req_cuda(a, b_qkv, a_scale, b_scale_qkv, a_keeper, b_keeper_qkv, a_keeper_scale, b_keeper_scale_qkv)
     m, n3 = a.size(0), b_qkv.size(0)
     k = a.size(1) * 2 + a_keeper.size(1)
-    if kv_rows is not None:
-        return _gemm_i4_qkv_gqa(a, b_qkv, a_scale, b_scale_qkv, a_keeper, b_keeper_qkv, a_keeper_scale, b_keeper_scale_qkv, flags,
-                                int(kv_rows), m, n3, k)
-    if n3 % 384 != 0 or b_scale_qkv.numel() < (k // 128 - 1) * n3 or b_keeper_qkv.size(0) != n3:
-        raise RuntimeError("dense_layer_gemm_i4_qkv: weights must be the row concatenation [q; k; v] with H % 128 == 0")
-    h = n3 // 3
-    q = torch.empty((m, h), dtype=torch.float16, device=a.device)
-    kk = torch.empty((m, h // 2), dtype=torch.uint8, device=a.device)
-    vv = torch.empty((m, h // 2), dtype=torch.uint8, device=a.device)
-    ks = torch.empty((m, h // 128 * 2), dtype=torch.float16, device=a.device)
-    vs = torch.empty((m, h // 128 * 2), dtype=torch.float16, device=a.device)
-    with torch.cuda.device(a.device):
-        _lib.check(_lib.lib().atom_gemm_i4_qkv(a.data_ptr(), b_qkv.data_ptr(), a_scale.data_ptr(), b_scale_qkv.data_ptr(),
-                                               a_keeper.data_ptr(), b_keeper_qkv.data_ptr(), a_keeper_scale.data_ptr(),
-                                               b_keeper_scale_qkv.data_ptr(), q.data_ptr(), kk.data_ptr(), ks.data_ptr(), vv.data_ptr(),
-                                               vs.data_ptr(), m, h, k, flags, _stream(a)), "dense_layer_gemm_i4_qkv")
-    return q, (kk, ks), (vv, vs)
-
-
-def _gemm_i4_qkv_gqa(a, b_qkv, a_scale, b_scale_qkv, a_keeper, b_keeper_qkv, a_keeper_scale, b_keeper_scale_qkv, flags, kv_rows, m, n3, k):
+    kv_rows = n3 // 3 if kv_rows is None else int(kv_rows)
     hq = n3 - 2 * kv_rows
     if kv_rows <= 0 or hq <= 0 or kv_rows % 128 or hq % 128 or b_scale_qkv.numel() < (k // 128 - 1) * n3 or b_keeper_qkv.size(0) != n3:
         raise RuntimeError("dense_layer_gemm_i4_qkv: weights must be the row concatenation [q; k; v] with kv_rows rows of k and of v, "
@@ -259,7 +240,7 @@ def _gemm_i4_qkv_gqa(a, b_qkv, a_scale, b_scale_qkv, a_keeper, b_keeper_qkv, a_k
         _lib.check(_lib.lib().atom_gemm_i4_qkv_gqa(a.data_ptr(), b_qkv.data_ptr(), a_scale.data_ptr(), b_scale_qkv.data_ptr(),
                                                    a_keeper.data_ptr(), b_keeper_qkv.data_ptr(), a_keeper_scale.data_ptr(),
                                                    b_keeper_scale_qkv.data_ptr(), q.data_ptr(), kk.data_ptr(), ks.data_ptr(), vv.data_ptr(),
-                                                   vs.data_ptr(), m, hq, kv_rows, k, flags, _stream(a)), "dense_layer_gemm_i4_qkv (gqa)")
+                                                   vs.data_ptr(), m, hq, kv_rows, k, flags, _stream(a)), "dense_layer_gemm_i4_qkv")
     return q, (kk, ks), (vv, vs)
 
 
@@ -303,18 +284,11 @@ def batch_decode_i4(q, kv, layer_idx, rope_theta=10000.0):
     if q.dim() != 3 or q.size(2) != 128 or kv.indptr.size(0) != q.size(0) + 1 or kv.last_page_offset.size(0) != q.size(0):
         raise RuntimeError("batch_decode_i4: shape mismatch")
     o = torch.empty(q.shape, dtype=q.dtype, device=q.device)
-    if q.size(1) != H or float(rope_theta) != 10000.0:
-        with torch.cuda.device(q.device):
-            _lib.check(_lib.lib().atom_batch_decode_gqa_i4(o.data_ptr(), q.data_ptr(), kv.data.data_ptr(), kv.param.data_ptr(),
-                                                           kv.indptr.data_ptr(), kv.indicies.data_ptr(),
-                                                           kv.last_page_offset.data_ptr(), L, layer_idx, q.size(1), H, P, q.size(0),
-                                                           float(rope_theta), _stream(q)), "batch_decode_i4 (gqa)")
-        return o
     with torch.cuda.device(q.device):
-        _lib.check(_lib.lib().atom_batch_decode_i4(o.data_ptr(), q.data_ptr(), kv.data.data_ptr(), kv.param.data_ptr(),
-                                                   kv.indptr.data_ptr(), kv.indicies.data_ptr(),
-                                                   kv.last_page_offset.data_ptr(), L, layer_idx, H, P, q.size(0),
-                                                   _stream(q)), "batch_decode_i4")
+        _lib.check(_lib.lib().atom_batch_decode_gqa_i4(o.data_ptr(), q.data_ptr(), kv.data.data_ptr(), kv.param.data_ptr(),
+                                                       kv.indptr.data_ptr(), kv.indicies.data_ptr(),
+                                                       kv.last_page_offset.data_ptr(), L, layer_idx, q.size(1), H, P, q.size(0),
+                                                       float(rope_theta), _stream(q)), "batch_decode_i4")
     return o
 
 
@@ -357,21 +331,13 @@ def prefill_attention_i4(q, k, k_param, v, v_param, seqlen_indptr, seqlens=None,
         raise RuntimeError("prefill_attention_i4: seqlen_indptr does not cover the tokens")
     pos = torch.cat([torch.arange(n, dtype=torch.int32) for n in seqlens]).to(q.device, non_blocking=True)
     table = rope_table(max_len, q.device, rope_theta)
-    if hkv != h:
-        kf = torch.empty((t, hkv * 128), dtype=q.dtype, device=q.device)
-        vf, out = torch.empty_like(kf), torch.empty_like(q)
-        with torch.cuda.device(q.device):
-            _lib.check(_lib.lib().atom_prefill_attention_gqa_i4(q.data_ptr(), k.data_ptr(), k_param.data_ptr(), v.data_ptr(),
-                                                                v_param.data_ptr(), seqlen_indptr.data_ptr(), pos.data_ptr(),
-                                                                table.data_ptr(), kf.data_ptr(), vf.data_ptr(), out.data_ptr(), t, b,
-                                                                max_len, h, hkv, _stream(q)), "prefill_attention_i4 (gqa)")
-        return out
-    kf, vf, out = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
+    kf = torch.empty((t, hkv * 128), dtype=q.dtype, device=q.device)
+    vf, out = torch.empty_like(kf), torch.empty_like(q)
     with torch.cuda.device(q.device):
-        _lib.check(_lib.lib().atom_prefill_attention_i4(q.data_ptr(), k.data_ptr(), k_param.data_ptr(), v.data_ptr(), v_param.data_ptr(),
-                                                        seqlen_indptr.data_ptr(), pos.data_ptr(), table.data_ptr(), kf.data_ptr(),
-                                                        vf.data_ptr(), out.data_ptr(), t, b, max_len, h, _stream(q)),
-                   "prefill_attention_i4")
+        _lib.check(_lib.lib().atom_prefill_attention_gqa_i4(q.data_ptr(), k.data_ptr(), k_param.data_ptr(), v.data_ptr(),
+                                                            v_param.data_ptr(), seqlen_indptr.data_ptr(), pos.data_ptr(),
+                                                            table.data_ptr(), kf.data_ptr(), vf.data_ptr(), out.data_ptr(), t, b,
+                                                            max_len, h, hkv, _stream(q)), "prefill_attention_i4")
     return out
 
 

@@ -160,8 +160,7 @@ class TPLlamaDecoderLayer(nn.Module):
         fused = getattr(self, "_qkv", None) is not None and b <= 64
         if fused:
             w4, s4, w8, s8 = self._qkv
-            kv_rows = None if self.local_kv_heads == self.local_heads else self.local_kv_heads * 128
-            q, (k, ks), (v, vs) = ops.dense_layer_gemm_i4_qkv(x[1], w4, x[3], s4, x[0], w8, x[2], s8, kv_rows=kv_rows)
+            q, (k, ks), (v, vs) = ops.dense_layer_gemm_i4_qkv(x[1], w4, x[3], s4, x[0], w8, x[2], s8, kv_rows=self.local_kv_heads * 128)
             q = q.view(b, self.local_heads, 128)
         else:
             q = self.q_proj(x).view(b, self.local_heads, 128)

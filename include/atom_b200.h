@@ -154,8 +154,8 @@ ATOM_API int atom_batch_decode_i4(void* o, const void* q, const void* kv_data, c
  * num_kv_heads heads -- the same layout with H = num_kv_heads; query head h attends KV head h / G.
  *   o,q f16 [B,num_q_heads,128]  kv_data u8 [pages,L,2,num_kv_heads,P,64]  kv_param f16 [pages,L,2,num_kv_heads,P,2]
  * One CTA per (sequence, KV head) reads every page of that head once and serves its G query heads.  rope_theta is the RoPE base
- * (1e4 for Llama-1/2, 5e5 for Llama-3, 1e6 for Mixtral).  G in {2, 4, 8}; G = 1 with rope_theta = 1e4 IS atom_batch_decode_i4
- * (same kernel, same bits), G = 1 with another base is supported; any other ratio returns ATOM_E_UNSUPPORTED. */
+ * (1e4 for Llama-1/2, 5e5 for Llama-3, 1e6 for Mixtral).  G in {1, 2, 4, 8}; G = 1 with rope_theta = 1e4 IS
+ * atom_batch_decode_i4 (same kernel, same bits); any other ratio returns ATOM_E_UNSUPPORTED. */
 ATOM_API int atom_batch_decode_gqa_i4(void* o, const void* q, const void* kv_data, const void* kv_param, const void* kv_indptr,
                              const void* kv_indices, const void* last_page_offset, int num_layers, int layer_idx,
                              int num_q_heads, int num_kv_heads, int page_size, int batch_size, float rope_theta, void* stream);

@@ -105,8 +105,8 @@ def _weight_term(w, dl, D, v, o):
 
 
 def decode_bound(q, data, param, indptr, indices, last, layer, hq, theta):
-    """(float64 reference [B, Hq, 128], per-element bound of |kernel - reference| [B, Hq, 128]) for batch_decode_kernel and
-    batch_decode_gqa_kernel.
+    """(float64 reference [B, Hq, 128], per-element bound of |kernel - reference| [B, Hq, 128]) for batch_decode_kernel at
+    every group size.
 
     Score of token t (natural log units), s_t = sum_i Re(zq_i conj(zk_ti) e^{j(len-1-t)theta_i}) / sqrt(128).  Kernel error:
       * K path, packed FP16, per component of the rotated pair (re = kre c - kim s): the dequantising HFMA2 of kre and kim

@@ -128,6 +128,16 @@ def test_prefill_attention_matches_the_eager_dequant_rope_sdpa_path(lens, heads)
     vp = torch.stack((torch.rand(t, heads, generator=g) * 0.2 + 0.05, torch.rand(t, heads, generator=g) * 1.5), -1).half().to(dev).view(t, heads * 2)
     indptr = torch.tensor([0] + list(np.cumsum(lens)), dtype=torch.int32, device=dev)
     got = ops.prefill_attention_i4(q, k4, kp, v4, vp, indptr, seqlens=lens)
+    # the multi-head C entry point, called directly, gives the operator's bits
+    from atom_b200 import _lib
+    pos = torch.cat([torch.arange(n, dtype=torch.int32) for n in lens]).to(dev)
+    table = ops.rope_table(max(lens), dev)
+    kf, vf, direct = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
+    _lib.check(_lib.lib().atom_prefill_attention_i4(q.data_ptr(), k4.data_ptr(), kp.data_ptr(), v4.data_ptr(), vp.data_ptr(),
+                                                    indptr.data_ptr(), pos.data_ptr(), table.data_ptr(), kf.data_ptr(), vf.data_ptr(),
+                                                    direct.data_ptr(), t, len(lens), max(lens), heads,
+                                                    torch.cuda.current_stream().cuda_stream), "prefill_attention_i4")
+    assert torch.equal(direct, got)
     kd, vd = _dequant_o4(k4, kp, heads), _dequant_o4(v4, vp, heads)
     ref, off = [], 0
     for n in lens:

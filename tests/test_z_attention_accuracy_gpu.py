@@ -1,4 +1,4 @@
-"""GPU accuracy suite (-m gpu) of the attention kernels: batch_decode_kernel, batch_decode_gqa_kernel and the prefill kernels
+"""GPU accuracy suite (-m gpu) of the attention kernels: batch_decode_kernel at every group size and the prefill kernels
 against the float64 reference of tests/attn_ref64.py, element by element inside the bound derived there from the kernels'
 arithmetic (|kernel - ref64| <= bound; the assert message gives the worst error-to-bound ratio, and every passing case prints it).
 
@@ -19,8 +19,8 @@ DEV = "cuda:0"
 LN2 = np.log(2.0)
 # kernel variant -> (query heads, KV heads, RoPE base or None = varies with the case, page stripes S)
 VARIANTS = {
-    "mha": (2, 2, 1e4, 4),       # batch_decode_kernel (one query head per KV head at base 1e4)
-    "g1": (2, 2, 5e5, 8),        # batch_decode_gqa_kernel<1, ...>: multi-head at another base
+    "mha": (2, 2, 1e4, 4),       # batch_decode_kernel<1, ...>: one query head per KV head at base 1e4
+    "g1": (2, 2, 5e5, 4),        # batch_decode_kernel<1, ...>: multi-head at another base
     "g2": (4, 2, None, 4),
     "g4": (8, 2, None, 2),
     "g8": (8, 1, None, 1),

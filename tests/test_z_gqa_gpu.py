@@ -89,14 +89,14 @@ def test_gqa_entry_with_one_head_per_group_is_the_mha_kernel_bit_for_bit():
     data, param, indptr, indices, last = _kv_fixture(rng, H, P, 2, lens)
     kv = _KV(data, param, indptr, indices, last)
     q = T(rng.standard_normal((len(lens), H, 128)).astype(np.float16))
-    ref = ops.batch_decode_i4(q, kv, 1)
+    ref = ops.batch_decode_i4(q, kv, 1)                     # through atom_batch_decode_gqa_i4 with G = 1 and base 1e4
     o = torch.zeros_like(q)
     st = torch.cuda.current_stream().cuda_stream
-    _lib.check(_lib.lib().atom_batch_decode_gqa_i4(o.data_ptr(), q.data_ptr(), kv.data.data_ptr(), kv.param.data_ptr(), kv.indptr.data_ptr(),
-                                                   kv.indicies.data_ptr(), kv.last_page_offset.data_ptr(), 2, 1, H, H, P, len(lens), 10000.0,
-                                                   st), "batch_decode_gqa_i4")
+    _lib.check(_lib.lib().atom_batch_decode_i4(o.data_ptr(), q.data_ptr(), kv.data.data_ptr(), kv.param.data_ptr(), kv.indptr.data_ptr(),
+                                               kv.indicies.data_ptr(), kv.last_page_offset.data_ptr(), 2, 1, H, P, len(lens), st),
+               "batch_decode_i4")
     assert torch.equal(o, ref)
-    # one head per group with another base runs the eight-stripe instantiation: inside the oracle bound
+    # one head per group with another base runs the same four-stripe instantiation: inside the oracle bound
     o5 = ops.batch_decode_i4(q, kv, 1, rope_theta=5e5).cpu().numpy()
     assert _excess(o5, GO.batch_decode_gqa_i4(q.cpu().numpy(), data, param, indptr, indices, last, 1, theta=5e5)) <= 5e-4
 
@@ -133,11 +133,19 @@ def test_fused_gqa_qkv_equals_three_projections(m, hq, hkv, k):
 
 @pytest.mark.parametrize("m,h,k", [(16, 256, 512), (100, 512, 1024)])
 def test_fused_mha_qkv_unchanged_and_equal_through_both_entries(m, h, k):
-    from atom_b200 import ops
+    from atom_b200 import _lib, ops
     act, ws, (b, bs, bk, bks) = _qkv_operands(m, h, h, k)
     q_ref, k_ref, v_ref = _three_calls(act, ws)
-    for kv_rows in (None, h):                  # atom_gemm_i4_qkv, then atom_gemm_i4_qkv_gqa with equal parts
-        q, (kk, ks), (vv, vs) = ops.dense_layer_gemm_i4_qkv(act[0], b, act[1], bs, act[2], bk, act[3], bks, kv_rows=kv_rows)
+    # the operator with three equal parts implied and given (atom_gemm_i4_qkv_gqa), then atom_gemm_i4_qkv called directly
+    outs = [ops.dense_layer_gemm_i4_qkv(act[0], b, act[1], bs, act[2], bk, act[3], bks, kv_rows=kv_rows) for kv_rows in (None, h)]
+    q = torch.empty(m, h, dtype=torch.float16, device=DEV)
+    kk, vv = (torch.empty(m, h // 2, dtype=torch.uint8, device=DEV) for _ in range(2))
+    ks, vs = (torch.empty(m, h // 128 * 2, dtype=torch.float16, device=DEV) for _ in range(2))
+    _lib.check(_lib.lib().atom_gemm_i4_qkv(act[0].data_ptr(), b.data_ptr(), act[1].data_ptr(), bs.data_ptr(), act[2].data_ptr(),
+                                           bk.data_ptr(), act[3].data_ptr(), bks.data_ptr(), q.data_ptr(), kk.data_ptr(), ks.data_ptr(),
+                                           vv.data_ptr(), vs.data_ptr(), m, h, k, 0, torch.cuda.current_stream().cuda_stream), "gemm_i4_qkv")
+    outs.append((q, (kk, ks), (vv, vs)))
+    for q, (kk, ks), (vv, vs) in outs:
         assert torch.equal(q, q_ref) and torch.equal(kk, k_ref[0]) and torch.equal(ks, k_ref[1])
         assert torch.equal(vv, v_ref[0]) and torch.equal(vs, v_ref[1])
 

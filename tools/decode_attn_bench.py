@@ -2,7 +2,7 @@
 """Decode attention over the INT4 paged KV cache: the grouped-query kernel against the multi-head kernel on a head-repeated
 pool (what serving a GQA model without a GQA kernel would cost).  Needs a GPU; there is no CPU path.
 
-    python tools/decode_attn_bench.py [--batch 32] [--kv 1024 4096] [--heads 64:8 32:8 8:1] [--page 32] [--out result.json]
+    python tools/decode_attn_bench.py [--batch 32] [--kv 1024 4096] [--heads 64:8 32:8 8:1] [--page 32] [--theta 1e4] [--out result.json]
 
 Method: for every shape both variants are captured into one CUDA graph each, holding one launch per page-table set; the sets
 live in distinct regions of a pool and together exceed the L2 cache several times, so every launch streams its pages from HBM.
@@ -60,17 +60,17 @@ def build_sets(batch, kv_len, hkv, page, nsets, dev, gen):
     return data, param, tables
 
 
-def capture(q, kvs, cycles):
+def capture(q, kvs, cycles, theta):
     def run():
         out = None
         for _ in range(cycles):
             for kv in kvs:
-                out = ops.batch_decode_i4(q, kv, 0)
+                out = ops.batch_decode_i4(q, kv, 0, rope_theta=theta)
         return out
     st = torch.cuda.Stream()
     st.wait_stream(torch.cuda.current_stream())
     with torch.cuda.stream(st):
-        first = ops.batch_decode_i4(q, kvs[0], 0).clone()          # warm-up of this shape: module load, smem attribute
+        first = ops.batch_decode_i4(q, kvs[0], 0, rope_theta=theta).clone()   # warm-up of this shape: module load, smem attribute
         run()
         st.synchronize()
         g = torch.cuda.CUDAGraph()
@@ -96,6 +96,7 @@ def main():
     ap.add_argument("--kv", type=int, nargs="+", default=[1024, 4096])
     ap.add_argument("--heads", nargs="+", default=["64:8", "32:8", "8:1"], help="query heads : KV heads")
     ap.add_argument("--page", type=int, default=32)
+    ap.add_argument("--theta", type=float, default=1e4, help="RoPE base passed to every call")
     ap.add_argument("--reps", type=int, default=15, help="alternating timed replays per variant")
     ap.add_argument("--out", default=None, help="also write the records to this JSON file")
     args = ap.parse_args()
@@ -111,7 +112,8 @@ def main():
         for kv_len in args.kv:
             B, P, G = args.batch, args.page, hq // hkv
             q = torch.randn((B, hq, 128), device=dev, dtype=torch.float16, generator=gen)
-            rec = {"batch": B, "kv_len": kv_len, "q_heads": hq, "kv_heads": hkv, "page": P, "card": name, "power_limit": limit}
+            rec = {"batch": B, "kv_len": kv_len, "q_heads": hq, "kv_heads": hkv, "page": P, "rope_theta": args.theta, "card": name,
+                   "power_limit": limit}
             # the two variants sweep the same number of bytes, so the repeated pool needs fewer sets
             n_gqa = min(64, max(2, math.ceil(L2_SWEEP_BYTES / (136 * B * kv_len * hkv))))
             n_mha = min(64, max(2, math.ceil(L2_SWEEP_BYTES / (136 * B * kv_len * hq))))
@@ -124,12 +126,12 @@ def main():
             rperm = torch.randperm(used, device=dev, generator=gen).to(torch.int32)
             mha_kvs = [_KV(rdata, rparam, tables[0][0], rperm[s * B * pps:(s + 1) * B * pps].contiguous(), tables[0][2]) for s in range(n_mha)]
             cyc_g, cyc_m = max(1, 64 // n_gqa), max(1, 64 // n_mha)
-            g_gqa, o_gqa = capture(q, gqa_kvs, cyc_g)
-            g_mha, o_mha = capture(q, mha_kvs, cyc_m)
+            g_gqa, o_gqa = capture(q, gqa_kvs, cyc_g, args.theta)
+            g_mha, o_mha = capture(q, mha_kvs, cyc_m, args.theta)
             # same cache content for the two variants' first launches only if the page tables match: check on a shared table
             same = _KV(rdata, rparam, tables[0][0], tables[0][1] % used, tables[0][2])
-            ref = ops.batch_decode_i4(q, same, 0)
-            got = ops.batch_decode_i4(q, _KV(data, param, tables[0][0], tables[0][1] % used, tables[0][2]), 0)
+            ref = ops.batch_decode_i4(q, same, 0, rope_theta=args.theta)
+            got = ops.batch_decode_i4(q, _KV(data, param, tables[0][0], tables[0][1] % used, tables[0][2]), 0, rope_theta=args.theta)
             rec["max_abs_diff_gqa_vs_mha"] = float((got.float() - ref.float()).abs().max())
             t_g, t_m = [], []
             for _ in range(args.reps):
