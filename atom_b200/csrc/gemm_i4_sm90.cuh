@@ -54,11 +54,31 @@ struct GemmArgs {
   int expert_rows;
 };
 
-// timeline stamps for pipeline debugging: per CTA  0 start | 1 setup done | 2 main loop done | 3 reduction done | 4 end
+// timeline stamps for pipeline debugging (tools/gemm_phase_trace.py), 128 clock64 slots per CTA:
+//   0 start | 1 setup done | 2 keeper done (end of the consumers' main loop) | 3 every rank's tile staged | 4 end (thread 0)
+//   5 producer past griddepcontrol.wait | 6 split-K reduction + output stores done | 7 consumers leave
+// Stamps 2, 3, 6 and 7 come from consumer warp 0, the others from thread 0 (the same SM clock).
+// Built with -DATOM_GEMM_TRACE_GROUPS, INT4 group s < TRACE_GROUPS also stamps slot 8 + kind * TRACE_GROUPS + s:
+//   producer thread 0:  0 pack_full passed | 1 scale slot free (exp_empty) | 2 scales stored (their loads returned) | 3 exp_full
+//   consumer warp 0:    4 pack_full passed | 5 exp_full passed | 6 group dequantised
+// A compile-time switch: even untaken, a runtime branch in the per-group loops costs the 16-token split-K launch about
+// 0.6 us (H100 80GB HBM3, 700 W).
+#ifdef ATOM_GEMM_TRACE_GROUPS
+constexpr bool kTraceGroups = true;
+#else
+constexpr bool kTraceGroups = false;
+#endif
+constexpr int TRACE_GROUPS = 16;
 __device__ __forceinline__ void trace_stamp(const GemmArgs& a, int slot) {
   if (a.trace != nullptr) {
     const int cta = (blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
     a.trace[(size_t)cta * 128 + slot] = (unsigned long long)clock64();
+  }
+}
+
+__device__ __forceinline__ void trace_group(const GemmArgs& a, int kind, int s) {
+  if constexpr (kTraceGroups) {
+    if (s < TRACE_GROUPS) trace_stamp(a, 8 + kind * TRACE_GROUPS + s);
   }
 }
 
@@ -212,6 +232,7 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
                       kGrouped ? gtile.x * args.expert_rows + args.gu_rows + n0 : args.gu_rows + n0);
       }
       griddep_wait();                       // from here on the preceding kernel's output (the activations) may be read
+      trace_stamp(args, 5);
       for (int s = 0; s < first; ++s) issue_stage(s, 2);
       if (has_keeper) tma_load_2d(smem + C::OFF_KEEP_Q, &tm_a8, keep_full, 0, m0);
     } else {
@@ -234,7 +255,9 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
         issue_stage(nx, 0);
       }
       mbar_wait(&pack_full[ps], (s / C::PACK) & 1);
+      if (t == 0) trace_group(args, 0, s);
       if (s >= C::EXP) mbar_wait(&exp_empty[es], ((s / C::EXP) - 1) & 1);
+      if (t == 0) trace_group(args, 1, s);
       const uint8_t* packed = smem + C::OFF_PACK_Q + ps * C::PACK_Q;
       uint8_t* expanded = smem + C::OFF_EXP + es * C::EXP_Q;
 #pragma unroll
@@ -250,9 +273,11 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
         }
       }
       store_scales(es, sbv, sav);
+      if (t == 0) trace_group(args, 2, s);
       fence_proxy_async_smem();             // generic-proxy stores -> visible to the wgmma operand fetch
       __syncwarp();
       if (lane == 0) { mbar_arrive(&pack_empty[ps]); mbar_arrive(&exp_full[es]); }
+      if (t == 0) trace_group(args, 3, s);
     }
     if constexpr (kSplit > 1) { cluster_wait(); cluster_arrive(); cluster_wait(); cluster_arrive(); cluster_wait(); }
   } else {
@@ -288,6 +313,7 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
     for (int s = 0; s < n4; ++s) {
       const int ps = s % C::PACK, es = s % C::EXP;
       mbar_wait(&pack_full[ps], (s / C::PACK) & 1);
+      if (cw == 0 && lane == 0) trace_group(args, 4, s);
       uint4 wa[C::MT], wb[C::MT];
 #pragma unroll
       for (int t = 0; t < C::MT; ++t) {
@@ -298,6 +324,7 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
       __syncwarp();
       if (lane == 0) mbar_arrive(&pack_empty[ps]);
       mbar_wait(&exp_full[es], (s / C::EXP) & 1);
+      if (cw == 0 && lane == 0) trace_group(args, 5, s);
       const uint64_t db = wgmma_desc_k_sw128(smem_u32(smem + C::OFF_EXP + es * C::EXP_Q));
       const __half* sb = reinterpret_cast<const __half*>(smem + C::OFF_SCALE + es * C::SCALE_BYTES);
       const __half* sa = sb + C::ROWS;
@@ -319,6 +346,7 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(&exp_empty[es]);
+      if (cw == 0 && lane == 0) trace_group(args, 6, s);
     }
     if (has_keeper) {
       mbar_wait(keep_full, 0);
@@ -389,17 +417,15 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
         v[0] = f.x; v[1] = f.y; v[2] = f.z; v[3] = f.w;
       }
       if constexpr (kSplit > 1) {
+        // every remote rank's 4 channels in one 16-B load, all in flight together (one at a time, the remote-load latency
+        // stacked up 4 (kSplit - 1) deep per token row), then the rank-order sums
         const uint32_t local = smem_u32(tile + tk * C::TILE_PITCH + lane * 4);
+        float4 p[kSplit];
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          float sum = 0.f;
+        for (int rk = 0; rk < kSplit; ++rk) p[rk] = rk == (int)krank ? make_float4(v[0], v[1], v[2], v[3]) : ld_dsmem_v4(mapa_shared(local, rk));
+        v[0] = p[0].x; v[1] = p[0].y; v[2] = p[0].z; v[3] = p[0].w;
 #pragma unroll
-          for (int rk = 0; rk < kSplit; ++rk) {
-            const float p = rk == (int)krank ? v[e] : ld_dsmem_f32(mapa_shared(local + 4 * e, rk));
-            sum = rk == 0 ? p : sum + p;
-          }
-          v[e] = sum;
-        }
+        for (int rk = 1; rk < kSplit; ++rk) { v[0] += p[rk].x; v[1] += p[rk].y; v[2] += p[rk].z; v[3] += p[rk].w; }
       }
       if constexpr (kE == EPI_GATEUP) {
         // SiLU(gate) * up, then the dynamic quantisation of activate_fp16_i4 (Activate.cuh:102-166) for this 128-channel
@@ -482,8 +508,10 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
         if (lane == 0) d_scale[(size_t)m * (n_out_dim / 128) + otile] = __floats2half2_rn(scale, zero);
       }
     }
+    if (cw == 0 && lane == 0) trace_stamp(args, 6);
     // split-K: no CTA of the cluster leaves while its tile may still be read
     if constexpr (kSplit > 1) { cluster_arrive(); cluster_wait(); }
+    if (cw == 0 && lane == 0) trace_stamp(args, 7);
   }
   if (threadIdx.x == 0) trace_stamp(args, 4);
 }

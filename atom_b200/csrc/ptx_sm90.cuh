@@ -145,8 +145,10 @@ __device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.w
 __device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
   uint32_t r; asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank)); return r;
 }
-__device__ __forceinline__ float ld_dsmem_f32(uint32_t addr) {
-  float v; asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory"); return v;
+__device__ __forceinline__ float4 ld_dsmem_v4(uint32_t addr) {
+  float4 v;
+  asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
+  return v;
 }
 
 // ------------------------------------------------------------------ programmatic dependent launch (PDL)
