@@ -29,6 +29,8 @@ _SIGNATURES = {
     "atom_set_pdl": (_I, [_I]),
     "atom_batch_decode_i4": (_I, [_P] * 7 + [_I] * 5 + [_P]),
     "atom_batch_decode_gqa_i4": (_I, [_P] * 7 + [_I] * 6 + [_F, _P]),
+    "atom_batch_decode_split_gqa_i4": (_I, [_P] * 7 + [_I] * 6 + [_F, _I, _P]),
+    "atom_decode_kv_split": (_I, [_I] * 4),
     "atom_prefill_attention_i4": (_I, [_P] * 11 + [_I] * 4 + [_P]),
     "atom_prefill_attention_gqa_i4": (_I, [_P] * 11 + [_I] * 5 + [_P]),
     "atom_allreduce_push_f16": (_I, [_P] * 4 + [_I64, _I64, _I, _I, _P]),

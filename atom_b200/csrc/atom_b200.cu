@@ -11,9 +11,11 @@
 #include <cstdlib>
 #include <cstdio>
 #include <cstring>
+#include <map>
 #include <mutex>
 #include <set>
 #include <string>
+#include <tuple>
 #include <unordered_map>
 #include <utility>
 
@@ -538,28 +540,98 @@ static int kv_check(const char* what, const void* data, const void* param, const
 
 }  // extern "C"
 
-// one launch of batch_decode_kernel<G, kMaxTpl, kP>
+// multiprocessors of the current device, read once per device (no synchronisation: safe while a graph is being captured)
+static int device_sm_count(int* sms) {
+  static std::mutex mu;
+  static std::unordered_map<int, int> counts;
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return fail(ATOM_E_CUDA, "batch_decode: no current CUDA device");
+  std::lock_guard<std::mutex> lk(mu);
+  auto it = counts.find(dev);
+  if (it == counts.end()) {
+    int n = 0;
+    cudaError_t e = cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    if (e != cudaSuccess) return fail(ATOM_E_CUDA, "batch_decode: multiprocessor count: %s", cudaGetErrorString(e));
+    it = counts.emplace(dev, n).first;
+  }
+  *sms = it->second;
+  return ATOM_OK;
+}
+
+// one launch of batch_decode_kernel<G, kMaxTpl, kP, kSplit>; split: grid (B, Hkv, C), one cluster of C CTAs per (sequence, KV
+// head).  Before the first split launch of each (instantiation, C, device) the cluster is checked to fit (cudaOccupancyMax-
+// ActiveClusters); a C that does not is replaced by the largest smaller one that does (C = 1: the unsplit kernel).
 template <int G, int kMaxTpl, int kP>
-static int launch_decode(const char* what, void* o, const void* q, const atom::KvArgs& kv, float log2_theta, cudaStream_t stream) {
-  int rc = ensure_dynamic_smem(atom::batch_decode_kernel<G, kMaxTpl, kP>, 100 * 1024, what);
+static int launch_decode(const char* what, void* o, const void* q, const atom::KvArgs& kv, float log2_theta, int split,
+                         cudaStream_t stream) {
+  if (split > 1) {
+    auto kern = atom::batch_decode_kernel<G, kMaxTpl, kP, true>;
+    int rc = ensure_dynamic_smem(kern, 100 * 1024, what);
+    if (rc) return rc;
+    const size_t smem = atom::batch_decode_smem_bytes(G, kv.P);
+    cudaLaunchConfig_t cfg{};
+    cfg.blockDim = dim3(atom::dec_threads(G)); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+    cudaLaunchAttribute attr[2];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    cfg.attrs = attr;
+    {
+      static std::mutex mu;
+      static std::map<std::tuple<const void*, int, int, size_t>, int> fits;      // (kernel, C, device, smem) -> usable C
+      int dev = 0;
+      if (cudaGetDevice(&dev) != cudaSuccess) return fail(ATOM_E_CUDA, "%s: no current CUDA device", what);
+      const auto key = std::make_tuple(reinterpret_cast<const void*>(kern), split, dev, smem);
+      std::lock_guard<std::mutex> lk(mu);
+      auto it = fits.find(key);
+      if (it == fits.end()) {
+        int c = split;
+        for (; c > 1; c /= 2) {
+          cfg.gridDim = dim3(kv.B, kv.H, c);
+          attr[0].val.clusterDim.x = 1; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = c;
+          cfg.numAttrs = 1;
+          int n = 0;
+          cudaError_t e = cudaOccupancyMaxActiveClusters(&n, kern, &cfg);
+          if (e != cudaSuccess) return fail(ATOM_E_CUDA, "%s: cudaOccupancyMaxActiveClusters(C=%d): %s", what, c, cudaGetErrorString(e));
+          if (n > 0) break;
+        }
+        it = fits.emplace(key, c).first;
+      }
+      split = it->second;
+    }
+    if (split > 1) {
+      cfg.gridDim = dim3(kv.B, kv.H, split);
+      attr[0].val.clusterDim.x = 1; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = split;
+      cfg.numAttrs = 1;
+      const int pdl = pdl_enabled() ? 1 : 0;
+      if (pdl) {
+        attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr[1].val.programmaticStreamSerializationAllowed = 1;
+        cfg.numAttrs = 2;
+      }
+      cudaError_t e = cudaLaunchKernelEx(&cfg, kern, (__half*)o, (const __half*)q, kv, log2_theta, pdl);
+      if (e != cudaSuccess) return fail(ATOM_E_CUDA, "%s launch (kv split %d): %s", what, split, cudaGetErrorString(e));
+      return check_launch(what);
+    }
+  }
+  int rc = ensure_dynamic_smem(atom::batch_decode_kernel<G, kMaxTpl, kP, false>, 100 * 1024, what);
   if (rc) return rc;
-  return launch_k(what, atom::batch_decode_kernel<G, kMaxTpl, kP>, dim3(kv.B, kv.H), dim3(atom::dec_threads(G)),
+  return launch_k(what, atom::batch_decode_kernel<G, kMaxTpl, kP, false>, dim3(kv.B, kv.H), dim3(atom::dec_threads(G)),
                   atom::batch_decode_smem_bytes(G, kv.P), stream, (__half*)o, (const __half*)q, kv, log2_theta);
 }
 
 // the page sizes 16 / 32 of the reference benchmarks get their strides as immediates; for G = 1 a page of at most 32 tokens
 // has at most four tokens per lane
 template <int G>
-static int dispatch_decode(const char* what, void* o, const void* q, const atom::KvArgs& kv, float log2_theta, cudaStream_t stream) {
-  if (kv.P == 16) return launch_decode<G, 2, 16>(what, o, q, kv, log2_theta, stream);
-  if (kv.P == 32) return launch_decode<G, 4, 32>(what, o, q, kv, log2_theta, stream);
-  if (G == 1 && kv.P <= 32) return launch_decode<1, 4, 0>(what, o, q, kv, log2_theta, stream);
-  return launch_decode<G, 8, 0>(what, o, q, kv, log2_theta, stream);
+static int dispatch_decode(const char* what, void* o, const void* q, const atom::KvArgs& kv, float log2_theta, int split,
+                           cudaStream_t stream) {
+  if (kv.P == 16) return launch_decode<G, 2, 16>(what, o, q, kv, log2_theta, split, stream);
+  if (kv.P == 32) return launch_decode<G, 4, 32>(what, o, q, kv, log2_theta, split, stream);
+  if (G == 1 && kv.P <= 32) return launch_decode<1, 4, 0>(what, o, q, kv, log2_theta, split, stream);
+  return launch_decode<G, 8, 0>(what, o, q, kv, log2_theta, split, stream);
 }
 
 static int batch_decode(const char* what, void* o, const void* q, const void* kv_data, const void* kv_param, const void* kv_indptr,
                         const void* kv_indices, const void* last_page_offset, int num_layers, int layer_idx, int num_q_heads,
-                        int num_kv_heads, int page_size, int batch_size, float rope_theta, void* stream) {
+                        int num_kv_heads, int page_size, int batch_size, float rope_theta, int kv_split, void* stream) {
   int rc = kv_check(what, kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx, num_kv_heads, page_size,
                     batch_size);
   if (rc) return rc;
@@ -575,28 +647,58 @@ static int batch_decode(const char* what, void* o, const void* q, const void* kv
   ATOM_REQUIRE(aligned16(kv_data) && aligned16(kv_param), "%s: KV pool must be 16-byte aligned", what);
   const atom::KvArgs kv{(uint8_t*)kv_data, (__half2*)kv_param, (const int32_t*)kv_indptr, (const int32_t*)kv_indices,
                         (const int32_t*)last_page_offset, num_layers, layer_idx, num_kv_heads, page_size, batch_size};
+  ATOM_REQUIRE(kv_split == 0 || kv_split == 1 || kv_split == 2 || kv_split == 4 || kv_split == 8,
+               "%s: kv_split=%d must be 0 (automatic), 1 (no split), 2, 4 or 8", what, kv_split);
+  int split = kv_split;
+  if (split == 0) {
+    int sms = 0;
+    if ((rc = device_sm_count(&sms))) return rc;
+    split = atom_decode_kv_split(batch_size, num_kv_heads, group, sms);
+  }
   const float log2_theta = log2f(rope_theta);
   const cudaStream_t st = (cudaStream_t)stream;
-  if (group == 1) return dispatch_decode<1>(what, o, q, kv, log2_theta, st);
-  if (group == 2) return dispatch_decode<2>(what, o, q, kv, log2_theta, st);
-  if (group == 4) return dispatch_decode<4>(what, o, q, kv, log2_theta, st);
-  return dispatch_decode<8>(what, o, q, kv, log2_theta, st);
+  if (group == 1) return dispatch_decode<1>(what, o, q, kv, log2_theta, split, st);
+  if (group == 2) return dispatch_decode<2>(what, o, q, kv, log2_theta, split, st);
+  if (group == 4) return dispatch_decode<4>(what, o, q, kv, log2_theta, split, st);
+  return dispatch_decode<8>(what, o, q, kv, log2_theta, split, st);
 }
 
 extern "C" {
+
+// Split-KV rule: a (sequence, KV head) grid that already gives every SM a CTA is not split; a smaller one is spread over the
+// smallest cluster C in {2, 4, 8} that reaches one CTA per SM, 8 at most (the portable cluster size).  Host-known sizes only:
+// the sequence lengths live on the device, and a captured graph replays the launch with new ones.
+int atom_decode_kv_split(int batch, int num_kv_heads, int group, int sm_count) {
+  ATOM_REQUIRE(batch > 0 && num_kv_heads > 0 && sm_count > 0, "decode_kv_split: batch=%d num_kv_heads=%d sm_count=%d must be positive",
+               batch, num_kv_heads, sm_count);
+  ATOM_REQUIRE(group == 1 || group == 2 || group == 4 || group == 8, "decode_kv_split: group=%d must be 1, 2, 4 or 8", group);
+  const long long ctas = (long long)batch * num_kv_heads;
+  if (ctas >= sm_count) return 1;
+  for (int c = 2; c < 8; c *= 2)
+    if (ctas * c >= sm_count) return c;
+  return 8;
+}
 
 int atom_batch_decode_i4(void* o, const void* q, const void* kv_data, const void* kv_param, const void* kv_indptr,
                          const void* kv_indices, const void* last_page_offset, int num_layers, int layer_idx,
                          int num_heads, int page_size, int batch_size, void* stream) {
   return batch_decode("batch_decode_i4", o, q, kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx,
-                      num_heads, num_heads, page_size, batch_size, 1e4f, stream);
+                      num_heads, num_heads, page_size, batch_size, 1e4f, 0, stream);
 }
 
 int atom_batch_decode_gqa_i4(void* o, const void* q, const void* kv_data, const void* kv_param, const void* kv_indptr,
                              const void* kv_indices, const void* last_page_offset, int num_layers, int layer_idx,
                              int num_q_heads, int num_kv_heads, int page_size, int batch_size, float rope_theta, void* stream) {
   return batch_decode("batch_decode_gqa_i4", o, q, kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx,
-                      num_q_heads, num_kv_heads, page_size, batch_size, rope_theta, stream);
+                      num_q_heads, num_kv_heads, page_size, batch_size, rope_theta, 0, stream);
+}
+
+int atom_batch_decode_split_gqa_i4(void* o, const void* q, const void* kv_data, const void* kv_param, const void* kv_indptr,
+                                   const void* kv_indices, const void* last_page_offset, int num_layers, int layer_idx,
+                                   int num_q_heads, int num_kv_heads, int page_size, int batch_size, float rope_theta, int kv_split,
+                                   void* stream) {
+  return batch_decode("batch_decode_split_gqa_i4", o, q, kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers,
+                      layer_idx, num_q_heads, num_kv_heads, page_size, batch_size, rope_theta, kv_split, stream);
 }
 
 int atom_append_kv_i4(void* kv_data, void* kv_param, const void* kv_indptr, const void* kv_indices,

@@ -77,6 +77,12 @@ append_kv_kernel(KvArgs kv, const uint8_t* __restrict__ k, const uint8_t* __rest
 // FP32 (V is accumulated in half2 only within one page).  An
 // all-FP32 version of this kernel executed 75 M warp instructions per layer, 36 % of them nibble extraction/conversion.
 // Softmax is blocked per page; V dequant is folded: sum_t p_t (n s_t - z_t) = sum_t (p_t s_t) n - sum_t p_t z_t.
+// Split-KV (kSplit): grid (B, Hkv, C) with cluster dims (1, 1, C), C = %cluster_nctarank in {2, 4, 8}.  The page striping extends
+// over the cluster: CTA rank r owns the global stripes r*S + s, and global stripe r*S + s takes pages r*S + s + k*S*C, so its
+// bracket starts at (len-1 - (r*S + s) P) theta and steps by e^{-j S C P theta}.  The CTA's stripe merge is left un-normalised:
+// (m, d, acc[32]) per (head g, quarter c) unit in the (then idle) bracket area; after a cluster barrier every rank combines its
+// share of the G*4 units x 8 float4 chunks over ranks 0..C-1 in rank order (FP32, all DSMEM loads in flight together),
+// normalises and stores; a second cluster barrier keeps every CTA resident while its shared memory is read.
 constexpr int DEC_STAGES = 8;
 
 // consumer warps of batch_decode_kernel<G, ...>: four page stripes for G = 1 (4 CTAs per SM), G heads x 8/G stripes otherwise
@@ -134,12 +140,15 @@ __device__ __forceinline__ void flush_pv(float (&acc)[32], __half2 (&pv)[16]) {
 }
 
 // kMaxTpl: tokens per lane per page = P / 8 <= kMaxTpl.  kP: page size as a compile-time constant (16 / 32: the sizes the harness
-// uses -- all table strides and the token loops become immediates) or 0 = read it from the arguments.
-template <int G, int kMaxTpl, int kP>
+// uses -- all table strides and the token loops become immediates) or 0 = read it from the arguments.  kSplit: the sequence's
+// pages are spread over a cluster of C CTAs (see above); false is the one-CTA-per-(sequence, KV head) kernel.
+template <int G, int kMaxTpl, int kP, bool kSplit>
 __global__ void __launch_bounds__(dec_threads(G), G == 1 ? 4 : 2)
 batch_decode_kernel(__half* __restrict__ o, const __half* __restrict__ q, KvArgs kv, float log2_theta, int pdl) {
   static_assert(G == 1 || G == 2 || G == 4 || G == 8, "the consumer warps are split into G heads x S page stripes");
   constexpr int kConsumers = dec_consumers(G), kThreads = dec_threads(G), S = kConsumers / G;
+  int rank = 0, nranks = 1;                                        // split-KV: this CTA's rank and the cluster size C
+  if constexpr (kSplit) { rank = (int)cluster_ctarank(); nranks = (int)cluster_nctarank(); }
   extern __shared__ __align__(128) uint8_t smem_d[];
   if (pdl) { griddep_launch_dependents(); griddep_wait(); }      // q and the newest KV entry come from the preceding kernels
   const int P = kP ? kP : kv.P;
@@ -180,11 +189,11 @@ batch_decode_kernel(__half* __restrict__ o, const __half* __restrict__ q, KvArgs
   }
   if (tid < 64) {
     const float f = exp2f(-(float)tid * kFreqStep);
-    float sn, cs; sincosf((float)(S * P) * f, &sn, &cs);
+    float sn, cs; sincosf((float)(S * nranks * P) * f, &sn, &cs);
     stepr[tid] = make_float2(cs, -sn);
   }
   if (warp < kConsumers) {
-    // FP32 query bracket of this warp: zq e^{j (len-1 - stripe*P) theta} of query head hkv*G + g.  Lane (ts, c) owns couple
+    // FP32 query bracket of this warp: zq e^{j (len-1 - (rank*S + stripe)*P) theta} of query head hkv*G + g.  Lane (ts, c) owns couple
     // u = ts of quarter c: the pairs ja = 8(u/4) + u%4 and ja + 4; it keeps the FP32 values in smem and publishes their half2
     // packing.
     const __half* qh = q + ((size_t)b * Hq + hkv * G + g) * 128;
@@ -195,7 +204,7 @@ batch_decode_kernel(__half* __restrict__ o, const __half* __restrict__ q, KvArgs
       const int i = 16 * c + ja + 4 * x;
       const float f = exp2f(-(float)i * kFreqStep);
       const float xr = __half2float(qh[i]), xi = __half2float(qh[i + 64]);
-      float sn, cs; sincosf((float)(seq_len - 1 - stripe * P) * f, &sn, &cs);
+      float sn, cs; sincosf((float)(seq_len - 1 - (rank * S + stripe) * P) * f, &sn, &cs);
       v2[x] = make_float2(xr * cs - xi * sn, xi * cs + xr * sn);
       brk[warp * 64 + i] = v2[x];
     }
@@ -207,9 +216,12 @@ batch_decode_kernel(__half* __restrict__ o, const __half* __restrict__ q, KvArgs
   if (warp == kConsumers) {
     // ------------------------------------------------------------ producer: one elected lane streams the pages
     if (lane == 0) {
-      for (int pg = 0; pg < npages; ++pg) {
-        const int s = pg % DEC_STAGES;
-        mbar_wait(&empty[s], ((pg / DEC_STAGES) & 1) ^ 1);
+      // the CTA's lp-th page (its ring slot order) is global page lp, or split (lp / S) * S * C + rank * S + lp % S
+      for (int lp = 0;; ++lp) {
+        const int pg = kSplit ? (lp / S) * S * nranks + rank * S + lp % S : lp;
+        if (pg >= npages) break;
+        const int s = lp % DEC_STAGES;
+        mbar_wait(&empty[s], ((lp / DEC_STAGES) & 1) ^ 1);
         const int page = kv.indices[page_begin + pg];
         const size_t rk = kv_row(kv, page, 0, hkv, 0), rv = kv_row(kv, page, 1, hkv, 0);
         uint8_t* st = ring + s * stage_bytes;
@@ -219,6 +231,11 @@ batch_decode_kernel(__half* __restrict__ o, const __half* __restrict__ q, KvArgs
         bulk_g2s(st + 128 * P, kv.param + rk, 4 * P, &full[s]);
         bulk_g2s(st + 132 * P, kv.param + rv, 4 * P, &full[s]);
       }
+    }
+    if constexpr (kSplit) {        // the cluster barriers are CTA-wide (.aligned): the producer warp joins both
+      __syncwarp();
+      cluster_arrive(); cluster_wait();
+      cluster_arrive(); cluster_wait();
     }
     return;
   }
@@ -231,8 +248,9 @@ batch_decode_kernel(__half* __restrict__ o, const __half* __restrict__ q, KvArgs
   float2* mybrk = brk + warp * 64 + 16 * c;
   uint2* mybrkh = brkh + (warp * 4 + c) * 8;
 
-  for (int pg = stripe; pg < npages; pg += S) {
-    const int s = pg % DEC_STAGES;
+  // global page pg of the stripe is the CTA's lp-th (lp = pg unsplit)
+  for (int pg = rank * S + stripe, lp = stripe; pg < npages; pg += S * nranks, lp += S) {
+    const int s = lp % DEC_STAGES;
     const int valid = (pg == npages - 1) ? last_valid : P;
     // this page's query bracket as half2 couples (j, j+4); then every lane advances its own couple to the stripe's next
     // page (FP32 in smem, constant rotation e^{-j S P theta}) and publishes the new half2 packing
@@ -257,7 +275,7 @@ batch_decode_kernel(__half* __restrict__ o, const __half* __restrict__ q, KvArgs
       mybrkh[ts] = make_uint2(*reinterpret_cast<const uint32_t*>(&re2), *reinterpret_cast<const uint32_t*>(&im2));
     }
     // (the __syncwarp() at the end of the page orders these writes before the next page's reads)
-    mbar_wait(&full[s], (pg / DEC_STAGES) & 1);
+    mbar_wait(&full[s], (lp / DEC_STAGES) & 1);
     const uint8_t* st = ring + s * stage_bytes;
     const uint8_t* kblk = st;
     const uint8_t* vblk = st + 64 * P;
@@ -384,11 +402,58 @@ batch_decode_kernel(__half* __restrict__ o, const __half* __restrict__ q, KvArgs
 #pragma unroll
       for (int i = 0; i < 32; ++i) out[i] = fmaf(src[2 + i], sx, out[i]);
     }
-    const float inv = 1.f / dd;
-    __half* dst = o + ((size_t)b * Hq + hkv * G + warp) * 128 + 32 * c;
+    if constexpr (kSplit) {
+      // un-normalised (m, d, acc) of unit (g, c) for the cluster merge, in the bracket area the page loop no longer uses (16-B
+      // aligned float4 chunks: acc of unit u at u*32, (m, d) at G*128 + 2u; G*544 bytes <= brk + brkh)
+      const int u = warp * 4 + c;
+      float* cmb = reinterpret_cast<float*>(brk);
+      *reinterpret_cast<float2*>(cmb + G * 128 + 2 * u) = make_float2(mm, dd);
 #pragma unroll
-    for (int i = 0; i < 32; i += 2)
-      *reinterpret_cast<__half2*>(dst + i) = __floats2half2_rn(out[i] * inv, out[i + 1] * inv);
+      for (int i = 0; i < 32; i += 4) *reinterpret_cast<float4*>(cmb + u * 32 + i) = make_float4(out[i], out[i + 1], out[i + 2], out[i + 3]);
+    } else {
+      const float inv = 1.f / dd;
+      __half* dst = o + ((size_t)b * Hq + hkv * G + warp) * 128 + 32 * c;
+#pragma unroll
+      for (int i = 0; i < 32; i += 2)
+        *reinterpret_cast<__half2*>(dst + i) = __floats2half2_rn(out[i] * inv, out[i + 1] * inv);
+    }
+  }
+  if constexpr (kSplit) {
+    __syncwarp();
+    cluster_arrive(); cluster_wait();          // every rank's units are staged
+    // rank r combines items r*per .. r*per + per-1 of the G*4 units x 8 float4 chunks: over ranks 0..C-1 in rank order, FP32
+    const int per = G * 32 / nranks;
+    if (tid < per) {
+      const int it = rank * per + tid, u = it >> 3, k = it & 7;
+      const float* cmb = reinterpret_cast<const float*>(brk);
+      const uint32_t a_md = smem_u32(cmb + G * 128 + 2 * u), a_acc = smem_u32(cmb + u * 32 + 4 * k);
+      float2 md[8];
+      float4 a[8];
+#pragma unroll
+      for (int r = 0; r < 8; ++r)
+        if (r < nranks) { md[r] = ld_dsmem_v2(mapa_shared(a_md, r)); a[r] = ld_dsmem_v4(mapa_shared(a_acc, r)); }
+      float mm = -5e4f;
+#pragma unroll
+      for (int r = 0; r < 8; ++r)
+        if (r < nranks) mm = fmaxf(mm, md[r].x);
+      float dd = 0.f;
+      float4 out = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+      for (int r = 0; r < 8; ++r) {
+        if (r < nranks) {
+          const float sx = exp2f(md[r].x - mm);
+          dd = fmaf(md[r].y, sx, dd);
+          out.x = fmaf(a[r].x, sx, out.x); out.y = fmaf(a[r].y, sx, out.y);
+          out.z = fmaf(a[r].z, sx, out.z); out.w = fmaf(a[r].w, sx, out.w);
+        }
+      }
+      const float inv = 1.f / dd;
+      const __half2 lo = __floats2half2_rn(out.x * inv, out.y * inv), hi = __floats2half2_rn(out.z * inv, out.w * inv);
+      __half* dst = o + ((size_t)b * Hq + hkv * G + (u >> 2)) * 128 + 32 * (u & 3) + 4 * k;
+      *reinterpret_cast<uint2*>(dst) = make_uint2(*reinterpret_cast<const uint32_t*>(&lo), *reinterpret_cast<const uint32_t*>(&hi));
+    }
+    __syncwarp();
+    cluster_arrive(); cluster_wait();          // no CTA leaves while its units may still be read
   }
 }
 

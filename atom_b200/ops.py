@@ -275,21 +275,33 @@ def _kv_dims(kv):
     return kv.data.size(1), kv.data.size(3), kv.data.size(4)
 
 
-def batch_decode_i4(q, kv, layer_idx, rope_theta=10000.0):
+def batch_decode_i4(q, kv, layer_idx, rope_theta=10000.0, kv_split=0):
     """ops/__init__.py:21-32.  EXTENSION (grouped-query attention): q may hold G = 2, 4 or 8 query heads per head of the cache
     (query head h attends KV head h // G), and `rope_theta` is the RoPE base; one query head per KV head at the default base
-    is the reference's operator."""
+    is the reference's operator.  EXTENSION (split-KV): `kv_split` spreads each sequence's pages over a cluster of that many
+    CTAs -- 0 = automatic (`decode_kv_split`: only grids of fewer (sequence, KV head) pairs than SMs split), 1 = never,
+    2 / 4 / 8 = forced; other values raise."""
     _req_cuda(q, kv.data, kv.param, kv.indptr, kv.indicies, kv.last_page_offset)
     L, H, P = _kv_dims(kv)
     if q.dim() != 3 or q.size(2) != 128 or kv.indptr.size(0) != q.size(0) + 1 or kv.last_page_offset.size(0) != q.size(0):
         raise RuntimeError("batch_decode_i4: shape mismatch")
     o = torch.empty(q.shape, dtype=q.dtype, device=q.device)
     with torch.cuda.device(q.device):
-        _lib.check(_lib.lib().atom_batch_decode_gqa_i4(o.data_ptr(), q.data_ptr(), kv.data.data_ptr(), kv.param.data_ptr(),
-                                                       kv.indptr.data_ptr(), kv.indicies.data_ptr(),
-                                                       kv.last_page_offset.data_ptr(), L, layer_idx, q.size(1), H, P, q.size(0),
-                                                       float(rope_theta), _stream(q)), "batch_decode_i4")
+        _lib.check(_lib.lib().atom_batch_decode_split_gqa_i4(o.data_ptr(), q.data_ptr(), kv.data.data_ptr(), kv.param.data_ptr(),
+                                                             kv.indptr.data_ptr(), kv.indicies.data_ptr(),
+                                                             kv.last_page_offset.data_ptr(), L, layer_idx, q.size(1), H, P, q.size(0),
+                                                             float(rope_theta), int(kv_split), _stream(q)), "batch_decode_i4")
     return o
+
+
+def decode_kv_split(batch, num_kv_heads, group, device=None):
+    """The cluster size `batch_decode_i4(..., kv_split=0)` uses for `batch` sequences of `num_kv_heads` KV heads with `group`
+    query heads each on `device` (default: the current CUDA device): 1 when the grid already gives every SM a CTA."""
+    dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    c = _lib.lib().atom_decode_kv_split(int(batch), int(num_kv_heads), int(group), int(sms))
+    _lib.check(min(c, 0), "decode_kv_split")
+    return c
 
 
 _rope_tables = {}

@@ -160,6 +160,22 @@ ATOM_API int atom_batch_decode_gqa_i4(void* o, const void* q, const void* kv_dat
                              const void* kv_indices, const void* last_page_offset, int num_layers, int layer_idx,
                              int num_q_heads, int num_kv_heads, int page_size, int batch_size, float rope_theta, void* stream);
 
+/* EXTENSION (split-KV decode): atom_batch_decode_gqa_i4 with the KV length of each (sequence, KV head) spread over a cluster of
+ * kv_split CTAs whose partial softmax states are merged through distributed shared memory in rank order (no workspace, one
+ * launch, deterministic and independent of where the pages sit).  kv_split: 0 = automatic (atom_decode_kv_split on the current
+ * device), 1 = never split (the atom_batch_decode_gqa_i4 kernel, bit for bit), 2 / 4 / 8 = that cluster size (a size that cannot
+ * be scheduled on the device falls back to the largest smaller one that can); anything else returns ATOM_E_INVALID.
+ * atom_batch_decode_i4 and atom_batch_decode_gqa_i4 are this call with kv_split = 0. */
+ATOM_API int atom_batch_decode_split_gqa_i4(void* o, const void* q, const void* kv_data, const void* kv_param, const void* kv_indptr,
+                                            const void* kv_indices, const void* last_page_offset, int num_layers, int layer_idx,
+                                            int num_q_heads, int num_kv_heads, int page_size, int batch_size, float rope_theta,
+                                            int kv_split, void* stream);
+
+/* The cluster size kv_split = 0 picks: 1 when batch * num_kv_heads >= sm_count (every SM already has a CTA), otherwise the
+ * smallest C in {2, 4, 8} with batch * num_kv_heads * C >= sm_count, and 8 at most.  group (query heads per KV head, 1/2/4/8) is
+ * validated.  Returns C, or ATOM_E_INVALID for non-positive sizes or another group. */
+ATOM_API int atom_decode_kv_split(int batch, int num_kv_heads, int group, int sm_count);
+
 /* EXTENSION (SURVEY.md 8 f3): the prefill attention the reference leaves as a placeholder
  * (punica/models/llama.py:171-190, SDPA over torch.randn K/V): causal attention of every prompt over its own just-quantised
  * K/V -- the o4 outputs of the k/v projections, x = nibble * scale - zero (quantization.cuh:76) -- with RoPE(theta 1e4) on q
