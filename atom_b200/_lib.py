@@ -33,6 +33,7 @@ _SIGNATURES = {
     "atom_decode_kv_split": (_I, [_I] * 4),
     "atom_prefill_attention_i4": (_I, [_P] * 11 + [_I] * 4 + [_P]),
     "atom_prefill_attention_gqa_i4": (_I, [_P] * 11 + [_I] * 5 + [_P]),
+    "atom_prefill_attention_ctx_gqa_i4": (_I, [_P] * 11 + [_I] * 5 + [_P] * 5 + [_I] * 3 + [_P]),
     "atom_allreduce_push_f16": (_I, [_P] * 4 + [_I64, _I64, _I, _I, _P]),
     "atom_allreduce_state_words": (_I, []),
     "atom_gemm_i4_o16_push": (_I, [_P] * 10 + [_I64, _I, _I, _I64, _I64, _I64, _U32, _P]),

@@ -476,9 +476,12 @@ int atom_gemm_i4_o4(const void* a, const void* b, const void* a_scale, const voi
                      flags, stream, true);
 }
 
+// ctx == nullptr: every prompt is a whole sequence (prefill_attn_kernel<false>); otherwise prompt b is the tail of sequence b of
+// the cache *ctx (prefill_attn_kernel<true>, grid ordered KV head by KV head)
 static int prefill_attention(const char* what, const void* q, const void* k, const void* k_param, const void* v, const void* v_param,
                              const void* seqlen_indptr, const void* pos_of_token, const void* rope_table, void* k_f16, void* v_f16,
-                             void* out, int total_tokens, int batch_size, int max_len, int num_heads, int num_kv_heads, void* stream) {
+                             void* out, int total_tokens, int batch_size, int max_len, int num_heads, int num_kv_heads, void* stream,
+                             const atom::KvArgs* ctx = nullptr) {
   ATOM_REQUIRE(q && k && k_param && v && v_param && seqlen_indptr && pos_of_token && rope_table && k_f16 && v_f16 && out,
                "%s: null pointer argument", what);
   ATOM_REQUIRE(batch_size > 0 && num_heads > 0 && max_len > 0, "%s: batch_size=%d num_heads=%d max_len=%d must be positive", what,
@@ -494,10 +497,19 @@ static int prefill_attention(const char* what, const void* q, const void* k, con
       (const float2*)rope_table, (__half*)k_f16, (__half*)v_f16, th, num_kv_heads);
   int rc = check_launch("prefill_attention_i4 (dequant + RoPE)");
   if (rc) return rc;
-  const dim3 grid((unsigned)((max_len + atom::PF_BQ - 1) / atom::PF_BQ), (unsigned)batch_size, (unsigned)num_heads);
-  atom::prefill_attn_kernel<<<grid, atom::PF_THREADS, 0, (cudaStream_t)stream>>>(
-      (const __half*)q, (const __half*)k_f16, (const __half*)v_f16, (const int32_t*)seqlen_indptr, (const float2*)rope_table,
-      (__half*)out, num_heads, num_kv_heads, 0.08838834764831845f * 1.4426950408889634f);
+  const unsigned q_tiles = (unsigned)((max_len + atom::PF_BQ - 1) / atom::PF_BQ);
+  const float scale_log2 = 0.08838834764831845f * 1.4426950408889634f;
+  if (ctx == nullptr) {
+    const dim3 grid(q_tiles, (unsigned)batch_size, (unsigned)num_heads);
+    atom::prefill_attn_kernel<false><<<grid, atom::PF_THREADS, 0, (cudaStream_t)stream>>>(
+        (const __half*)q, (const __half*)k_f16, (const __half*)v_f16, (const int32_t*)seqlen_indptr, (const float2*)rope_table,
+        (__half*)out, num_heads, num_kv_heads, scale_log2);
+  } else {
+    const dim3 grid(q_tiles * (unsigned)(num_heads / num_kv_heads), (unsigned)num_kv_heads, (unsigned)batch_size);
+    atom::prefill_attn_kernel<true, atom::KvArgs><<<grid, atom::PF_THREADS, 0, (cudaStream_t)stream>>>(
+        (const __half*)q, (const __half*)k_f16, (const __half*)v_f16, (const int32_t*)seqlen_indptr, (const float2*)rope_table,
+        (__half*)out, num_heads, num_kv_heads, scale_log2, *ctx);
+  }
   return check_launch(what);
 }
 
@@ -536,6 +548,31 @@ static int kv_check(const char* what, const void* data, const void* param, const
   ATOM_REQUIRE(L > 0 && layer >= 0 && layer < L, "%s: layer_idx=%d out of range [0,%d)", what, layer, L);
   ATOM_REQUIRE(H > 0 && P > 0 && B > 0, "%s: num_heads=%d page_size=%d batch_size=%d must be positive", what, H, P, B);
   return ATOM_OK;
+}
+
+int atom_prefill_attention_ctx_gqa_i4(const void* q, const void* k, const void* k_param, const void* v, const void* v_param,
+                                      const void* seqlen_indptr, const void* pos_of_token, const void* rope_table, void* k_f16,
+                                      void* v_f16, void* out, int total_tokens, int batch_size, int max_len, int num_q_heads,
+                                      int num_kv_heads, const void* kv_data, const void* kv_param, const void* kv_indptr,
+                                      const void* kv_indices, const void* last_page_offset, int num_layers, int layer_idx,
+                                      int page_size, void* stream) {
+  const char* what = "prefill_attention_ctx_gqa_i4";
+  int rc = kv_check(what, kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx, num_kv_heads, page_size,
+                    batch_size);
+  if (rc) return rc;
+  ATOM_REQUIRE(num_q_heads > 0 && num_q_heads % num_kv_heads == 0,
+               "%s: num_q_heads=%d must be a positive multiple of num_kv_heads=%d", what, num_q_heads, num_kv_heads);
+  const int group = num_q_heads / num_kv_heads;
+  if (group != 1 && group != 2 && group != 4 && group != 8)
+    return fail(ATOM_E_UNSUPPORTED, "%s: %d query heads per KV head (num_q_heads=%d, num_kv_heads=%d); supported group sizes are 1, 2, "
+                                    "4 and 8", what, group, num_q_heads, num_kv_heads);
+  ATOM_REQUIRE(page_size % 8 == 0 && page_size <= 64, "%s: page_size=%d must be a multiple of 8, at most 64", what, page_size);
+  ATOM_REQUIRE(aligned16(kv_data) && aligned16(kv_param) && aligned16(rope_table), "%s: KV pool and rope table must be 16-byte aligned",
+               what);
+  const atom::KvArgs kv{(uint8_t*)kv_data, (__half2*)kv_param, (const int32_t*)kv_indptr, (const int32_t*)kv_indices,
+                        (const int32_t*)last_page_offset, num_layers, layer_idx, num_kv_heads, page_size, batch_size};
+  return prefill_attention(what, q, k, k_param, v, v_param, seqlen_indptr, pos_of_token, rope_table, k_f16, v_f16, out, total_tokens,
+                           batch_size, max_len, num_q_heads, num_kv_heads, stream, &kv);
 }
 
 }  // extern "C"

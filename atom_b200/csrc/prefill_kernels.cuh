@@ -14,8 +14,12 @@
 // (K row-major [token][dim], V transposed [dim][token] so both B fragments are contiguous 32-bit loads, padded
 // pitches => conflict-free).  The MMA is mma.sync.m16n8k16 (the warp-level tensor path); a wgmma variant is the
 // next step for this kernel.
+// Prefill over a cached prefix (prefill_attn_kernel<true>): prompt b is the tail of its cached sequence, as init_kv_i4 writes it
+// (positions ctx_b .. ctx_b + L_b - 1).  Its queries also attend, without a causal mask, to the ctx_b tokens before it, which the
+// kernel reads straight from the INT4 pages (no FP16 scratch grows with the context) -- see the kernel's comment.
 #pragma once
 #include "ptx_sm90.cuh"
+#include "kv_kernels.cuh"
 
 namespace atom {
 
@@ -59,15 +63,105 @@ kv_dequant_rope_kernel(const uint8_t* __restrict__ k4, const __half2* __restrict
   vo[i + 64] = __float2half_rn((float)((vb[32 + (i >> 1)] >> sh) & 0xF) * vp.x - vp.y);
 }
 
+// tokens of sequence b cached before its prompt of L tokens (the page table holds seq_len_b = ctx_b + L)
+__device__ __forceinline__ int prefill_ctx_len(const KvArgs& kv, int b, int L) {
+  return max((kv.indptr[b + 1] - kv.indptr[b] - 1) * kv.P + kv.last_page_offset[b] - L, 0);   // < 0 only on a bad page table
+}
+
+// Context tile of prefill_attn_kernel<true>: 64 tokens of sequence b's cached prefix (KV head hk) into Ks / Vt, as
+// kv_dequant_rope_kernel would have turned them into kf / vf: x = fp16(n * s - z), K rotated in FP32 at its absolute position
+// from the (cos, sin) table and rounded to FP16 (the same fused multiply-adds, pinned with intrinsics).  Token slots outside
+// [0, ctx) are zeros (masked by the caller).  Thread = (token tid / 2, pair half tid % 2): the RoPE pairs i = 32 hf .. 32 hf + 31
+// of one token, i.e. bytes 16 hf .. 16 hf + 15 and 32 + 16 hf .. 32 + 16 hf + 15 of its K and V rows (one 16-byte load each).
+// rope: the table shifted to the prompt's first position (row p = absolute position ctx + p); k0: key position of the tile's first
+// slot (-ctx .. -1 are the context tokens)
+__device__ __forceinline__ void prefill_ctx_tile(const KvArgs& kv, int b, int L, int hk, int k0, const float2* __restrict__ rope,
+                                                 __half* Ks, __half* Vt, int tid) {
+  const int ctx = prefill_ctx_len(kv, b, L);
+  const int tok = tid >> 1, hf = tid & 1, kpos = k0 + tok, c = ctx + kpos;
+  const bool live = c >= 0 && c < ctx;
+  size_t rk = 0;
+  if (live) rk = kv_row(kv, kv.indices[kv.indptr[b] + c / kv.P], 0, hk, c % kv.P);
+  const size_t rv = rk + (size_t)kv.H * kv.P;                  // the V row of the same (page, layer, head, entry)
+  {                                                             // K: dequantise, rotate, round, store row-major
+    uint4 lo = make_uint4(0, 0, 0, 0), hi = lo;
+    float2 p = make_float2(0.f, 0.f);
+    if (live) {
+      lo = *reinterpret_cast<const uint4*>(kv.data + rk * 64 + 16 * hf);
+      hi = *reinterpret_cast<const uint4*>(kv.data + rk * 64 + 32 + 16 * hf);
+      p = __half22float2(kv.param[rk]);
+    }
+    const float2* rp = rope + (ptrdiff_t)kpos * 64 + 32 * hf;
+    const uint32_t wl[4] = {lo.x, lo.y, lo.z, lo.w}, wh[4] = {hi.x, hi.y, hi.z, hi.w};
+#pragma unroll
+    for (int w = 0; w < 4; ++w) {                     // pairs i = 32 hf + 8 w + e, e < 8: nibble e of word w (low and high half)
+      uint32_t re[4], im[4];
+#pragma unroll
+      for (int e = 0; e < 8; e += 2) {
+        float4 cs = make_float4(1.f, 0.f, 1.f, 0.f);
+        if (live) cs = *reinterpret_cast<const float4*>(rp + 8 * w + e);
+        const float a1 = __half2float(__float2half_rn(__fmaf_rn((float)((wl[w] >> (4 * e)) & 0xF), p.x, -p.y)));
+        const float a2 = __half2float(__float2half_rn(__fmaf_rn((float)((wh[w] >> (4 * e)) & 0xF), p.x, -p.y)));
+        const float b1 = __half2float(__float2half_rn(__fmaf_rn((float)((wl[w] >> (4 * e + 4)) & 0xF), p.x, -p.y)));
+        const float b2 = __half2float(__float2half_rn(__fmaf_rn((float)((wh[w] >> (4 * e + 4)) & 0xF), p.x, -p.y)));
+        re[e >> 1] = pack_h2(__fmaf_rn(a1, cs.x, -__fmul_rn(a2, cs.y)), __fmaf_rn(b1, cs.z, -__fmul_rn(b2, cs.w)));
+        im[e >> 1] = pack_h2(__fmaf_rn(a1, cs.y, __fmul_rn(a2, cs.x)), __fmaf_rn(b1, cs.w, __fmul_rn(b2, cs.z)));
+      }
+      *reinterpret_cast<uint4*>(&Ks[tok * PF_KPITCH + 32 * hf + 8 * w]) = make_uint4(re[0], re[1], re[2], re[3]);
+      *reinterpret_cast<uint4*>(&Ks[tok * PF_KPITCH + 64 + 32 * hf + 8 * w]) = make_uint4(im[0], im[1], im[2], im[3]);
+    }
+  }
+  {                                                             // V: dequantise, round, store transposed
+    uint4 lo = make_uint4(0, 0, 0, 0), hi = lo;
+    float2 p = make_float2(0.f, 0.f);
+    if (live) {
+      lo = *reinterpret_cast<const uint4*>(kv.data + rv * 64 + 16 * hf);
+      hi = *reinterpret_cast<const uint4*>(kv.data + rv * 64 + 32 + 16 * hf);
+      p = __half22float2(kv.param[rv]);
+    }
+    const uint32_t wl[4] = {lo.x, lo.y, lo.z, lo.w}, wh[4] = {hi.x, hi.y, hi.z, hi.w};
+#pragma unroll
+    for (int w = 0; w < 4; ++w) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const int d = 32 * hf + 8 * w + e;
+        Vt[d * PF_VPITCH + tok] = __float2half_rn(__fmaf_rn((float)((wl[w] >> (4 * e)) & 0xF), p.x, -p.y));
+        Vt[(d + 64) * PF_VPITCH + tok] = __float2half_rn(__fmaf_rn((float)((wh[w] >> (4 * e)) & 0xF), p.x, -p.y));
+      }
+    }
+  }
+}
+
+__device__ __forceinline__ int prefill_ctx_len(int, int) { return 0; }                             // <false>: no cache
+__device__ __forceinline__ void prefill_ctx_tile(int, int, int, int, const float2*, __half*, __half*, int) {}
+
 // q f16 [T, H*128] (pre-RoPE, the q projection's output); kf, vf f16 [T, Hkv*128] from kv_dequant_rope_kernel (H % Hkv == 0);
 // indptr i32 [B+1]: prompt b owns tokens [indptr[b], indptr[b+1]); out f16 [T, H*128]
-__global__ void __launch_bounds__(PF_THREADS)
+// kCtx = false: grid (q tiles, B, H); every prompt is a whole sequence (positions 0 .. L - 1).
+// kCtx = true: `cache` is one KvArgs (page table, layer); grid (q tiles * G, Hkv, B), G = H / Hkv -- the q tiles and the G query
+// heads of one KV head are adjacent in launch order, so the CTAs that stream the same context pages run together and share them
+// through L2.  Prompt b is the tail of the cached sequence b: ctx_b = seq_len_b - L_b, derived as append_kv_kernel derives its
+// write position.  The context sits at key positions -ctx_b .. -1, in 64-token tiles that end at -1, before the prompt's own
+// causal tiles: every context key precedes every query, so these tiles need no causal mask, only the first (partial) one a length
+// mask, and the online-softmax state carries on into the prompt's tiles unchanged.  q is rotated at ctx_b + r.
+// Every term of the context path sits behind `if constexpr` or a condition on the constant kCtx, and the cache is a trailing
+// parameter pack (empty for <false>): prefill_attn_kernel<false> compiles to the SASS of the kernel before the context path.
+// <true> asks for two CTAs per SM: at the three CTAs ptxas otherwise aims for (168 registers) its context producer spills.
+template <bool kCtx, typename... Cache>
+__global__ void __launch_bounds__(PF_THREADS, kCtx ? 2 : 0)
 prefill_attn_kernel(const __half* __restrict__ q, const __half* __restrict__ kf, const __half* __restrict__ vf,
                     const int32_t* __restrict__ indptr, const float2* __restrict__ rope, __half* __restrict__ out, int H,
-                    int Hkv, float scale_log2) {
+                    int Hkv, float scale_log2, Cache... cache) {
+  static_assert(sizeof...(Cache) == (kCtx ? 1 : 0), "prefill_attn_kernel<true> takes the cache (one KvArgs), <false> nothing");
   __shared__ __align__(16) __half Ks[PF_BK * PF_KPITCH];
   __shared__ __align__(16) __half Vt[128 * PF_VPITCH];
-  const int b = blockIdx.y, h = blockIdx.z, qt = blockIdx.x;
+  int b, h, qt;
+  if constexpr (kCtx) {
+    const int G = H / Hkv;
+    b = blockIdx.z; h = blockIdx.y * G + (int)blockIdx.x % G; qt = (int)blockIdx.x / G;
+  } else {
+    b = blockIdx.y; h = blockIdx.z; qt = blockIdx.x;
+  }
   const int t0 = indptr[b], L = indptr[b + 1] - t0;
   const int q0 = qt * PF_BQ;
   if (q0 >= L) return;
@@ -76,6 +170,7 @@ prefill_attn_kernel(const __half* __restrict__ q, const __half* __restrict__ kf,
   const size_t kv_pitch = (size_t)Hkv * 128;          // grouped-query attention: query head h reads KV head h / (H / Hkv)
   const int hk = h / (H / Hkv);
 
+  if constexpr (kCtx) rope += (size_t)prefill_ctx_len(cache..., b, L) * 64;     // row p of the table = position ctx + p
   // ---- Q fragments of this warp's 16 rows, rotated (FP32 math, rounded to FP16 like `rotary_pos_emb(...).to(q.dtype)`)
   uint32_t qa[8][4];
   {
@@ -109,9 +204,13 @@ prefill_attn_kernel(const __half* __restrict__ q, const __half* __restrict__ kf,
   float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
   const int qrow0 = q0 + warp * 16 + g, qrow1 = qrow0 + 8;
 
-  for (int kt = 0; kt <= qt; ++kt) {
+  for (int kt = kCtx ? -((prefill_ctx_len(cache..., b, L) + PF_BK - 1) / PF_BK) : 0; kt <= qt; ++kt) {
     const int k0 = kt * PF_BK;
     __syncthreads();                                  // the previous tile has been consumed
+    if (kCtx && kt < 0) {
+      // ---- producer, context: 64 cached tokens (key positions k0 .. k0 + 63) dequantised and rotated from the pages
+      prefill_ctx_tile(cache..., b, L, hk, k0, rope, Ks, Vt, tid);
+    } else {
     // ---- producer: 64 tokens of K (row-major) and V (transposed) into shared memory, 16-byte chunks
 #pragma unroll
     for (int it = 0; it < 8; ++it) {
@@ -127,6 +226,7 @@ prefill_attn_kernel(const __half* __restrict__ q, const __half* __restrict__ kf,
 #pragma unroll
       for (int e = 0; e < 8; ++e) Vt[(ch * 8 + e) * PF_VPITCH + tok] = vh[e];
     }
+    }
     __syncthreads();
 
     // ---- S = Q K^T (16 x 64 per warp), FP32
@@ -139,6 +239,17 @@ prefill_attn_kernel(const __half* __restrict__ q, const __half* __restrict__ kf,
         const uint32_t b0 = *reinterpret_cast<const uint32_t*>(&Ks[(8 * j + g) * PF_KPITCH + 16 * kk + 2 * t]);
         const uint32_t b1 = *reinterpret_cast<const uint32_t*>(&Ks[(8 * j + g) * PF_KPITCH + 16 * kk + 8 + 2 * t]);
         mma_16816(s[j], qa[kk], b0, b1);
+      }
+    }
+    if constexpr (kCtx) {                             // the first context tile's slots before the context: no key
+      const int lim = -prefill_ctx_len(cache..., b, L);
+      if (k0 < lim) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+#pragma unroll
+          for (int u = 0; u < 2; ++u)
+            if (k0 + 8 * j + 2 * t + u < lim) s[j][u] = s[j][2 + u] = -INFINITY;
+        }
       }
     }
     // ---- scale, causal / length mask, online softmax (rows qrow0 and qrow1 of this thread)

@@ -110,6 +110,12 @@ class KvCacheInt4:
         """Make room for one more token; a page is added when the last one is full."""
         self._grow_to(self._seqlen + 1)
 
+    def acquire(self, n: int) -> None:
+        """Make room for n more tokens (a prompt chunk, a continuation); pages are added as the last one fills."""
+        if n < 0:
+            raise ValueError("acquire: n must be non-negative")
+        self._grow_to(self._seqlen + int(n))
+
     def release(self) -> None:
         """Give every page back to the pool."""
         while self._pages:
@@ -148,6 +154,9 @@ class BatchedKvCacheInt4:
         self.indptr = dev[:b + 1]
         self.last_page_offset = dev[b + 1:2 * b + 1]
         self.indicies = dev[2 * b + 1:]
+        # host copy of every sequence's length at construction: the prefill over a cached prefix needs each prompt's position
+        # in its sequence (seqlens[b] - prompt length) for the RoPE positions and the table size without reading the device
+        self.seqlens: List[int] = [c.seqlen for c in kv]
 
     @property
     def page_size(self) -> int:

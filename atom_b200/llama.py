@@ -6,7 +6,8 @@ forward(hidden_states, blen, prefill_kv, decode_kv) contract, so the reference's
 Differences (documented in DESIGN.md):
   * hidden / intermediate sizes are free multiples of 128 (reference kernels: 4096 / 11008 only);
   * prefill attention uses the K/V that were just quantised into the cache (dequantised, causal SDPA with RoPE); the
-    reference feeds torch.randn K/V there ("HACK", llama.py:171-174);
+    reference feeds torch.randn K/V there ("HACK", llama.py:171-174).  A prompt whose sequence already holds cached tokens (a
+    chunk of a long prompt, a continuation) attends to them too, at its absolute positions;
   * no HuggingFace dependency: any object with hidden_size / intermediate_size / num_attention_heads /
     num_hidden_layers / rms_norm_eps / vocab_size works as `config` (LlamaConfig does).
 """
@@ -228,9 +229,13 @@ class LlamaAttention(nn.Module):
                            blen.indptr, self.layer_idx)
             nvtx.range_pop()
             nvtx.range_push("prefill_attention")
+            # a prompt that is the tail of a longer cached sequence (a chunk of a long prompt, a continuation) attends to the
+            # whole cached prefix; whole-sequence prompts keep the plain call
+            cached = getattr(prefill_kv, "seqlens", None)
+            ctx = {} if cached is None or list(cached) == list(blen.prefills) else {"kv": prefill_kv, "layer_idx": self.layer_idx}
             stack.append(ops.prefill_attention_i4(q_proj[:blen.doff], k_proj[0][:blen.doff], k_proj[1][:blen.doff],
                                                   v_proj[0][:blen.doff], v_proj[1][:blen.doff], blen.indptr, seqlens=list(blen.prefills),
-                                                  rope_theta=self.rope_theta))
+                                                  rope_theta=self.rope_theta, **ctx))
             nvtx.range_pop()
         if blen.decode > 0:
             q = q_proj[blen.doff:].view(blen.decode, nq, hd)

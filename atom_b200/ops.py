@@ -322,11 +322,15 @@ def rope_table(max_len, device, theta=10000.0):
     return t
 
 
-def prefill_attention_i4(q, k, k_param, v, v_param, seqlen_indptr, seqlens=None, rope_theta=10000.0):
+def prefill_attention_i4(q, k, k_param, v, v_param, seqlen_indptr, seqlens=None, rope_theta=10000.0, *, kv=None, layer_idx=None):
     """EXTENSION: causal prefill attention of every prompt over its own quantised K/V (the o4 projection outputs) with RoPE,
     one launch for all prompts and heads.  q f16 [T, H*128]; k, v u8 [T, Hkv*64]; k_param, v_param f16 [T, Hkv*2] (Hkv = H, or
     a divisor of it for grouped-query attention: taken from k's shape); seqlen_indptr i32 [B+1] (device); seqlens: the prompt
-    lengths as host ints (avoids a device read); rope_theta: the RoPE base.  Returns f16 [T, H*128]."""
+    lengths as host ints (avoids a device read); rope_theta: the RoPE base.  Returns f16 [T, H*128].
+    EXTENSION (chunked prefill, prompt continuation): with `kv` (a BatchedKvCacheInt4 of the B sequences) and `layer_idx`, prompt b
+    is the tail of sequence b of the cache -- what init_kv_i4 just wrote there -- at positions ctx_b .. ctx_b + n_b - 1, ctx_b =
+    kv.seqlens[b] - n_b.  It attends to the whole cached prefix and, causally, to its own tokens; query head counts per KV head
+    of 1, 2, 4 or 8.  When every ctx_b is 0 this is the call without `kv`, bit for bit."""
     _req_width("prefill_attention_i4", f16_q_2=q, k_1=k, f16_k_param_2=k_param, v_1=v, f16_v_param_2=v_param)
     _req_cuda(q, k, k_param, v, v_param, seqlen_indptr)
     t, hd = q.shape
@@ -341,16 +345,50 @@ def prefill_attention_i4(q, k, k_param, v, v_param, seqlen_indptr, seqlens=None,
     b, max_len = len(seqlens), max(seqlens)
     if sum(seqlens) != t or seqlen_indptr.numel() != b + 1:
         raise RuntimeError("prefill_attention_i4: seqlen_indptr does not cover the tokens")
-    pos = torch.cat([torch.arange(n, dtype=torch.int32) for n in seqlens]).to(q.device, non_blocking=True)
-    table = rope_table(max_len, q.device, rope_theta)
+    ctx = _prefill_contexts(kv, layer_idx, seqlens)
+    if not any(ctx):
+        pos = torch.cat([torch.arange(n, dtype=torch.int32) for n in seqlens]).to(q.device, non_blocking=True)
+        table = rope_table(max_len, q.device, rope_theta)
+    else:
+        _req_cuda(kv.data, kv.param, kv.indptr, kv.indicies, kv.last_page_offset)
+        L, H, P = _kv_dims(kv)
+        if H != hkv:
+            raise RuntimeError(f"prefill_attention_i4: the cache has {H} KV heads, k has {hkv}")
+        pos = torch.cat([torch.arange(c, c + n, dtype=torch.int32) for c, n in zip(ctx, seqlens)]).to(q.device, non_blocking=True)
+        table = rope_table(max(c + n for c, n in zip(ctx, seqlens)), q.device, rope_theta)
     kf = torch.empty((t, hkv * 128), dtype=q.dtype, device=q.device)
     vf, out = torch.empty_like(kf), torch.empty_like(q)
     with torch.cuda.device(q.device):
-        _lib.check(_lib.lib().atom_prefill_attention_gqa_i4(q.data_ptr(), k.data_ptr(), k_param.data_ptr(), v.data_ptr(),
-                                                            v_param.data_ptr(), seqlen_indptr.data_ptr(), pos.data_ptr(),
-                                                            table.data_ptr(), kf.data_ptr(), vf.data_ptr(), out.data_ptr(), t, b,
-                                                            max_len, h, hkv, _stream(q)), "prefill_attention_i4")
+        if not any(ctx):
+            _lib.check(_lib.lib().atom_prefill_attention_gqa_i4(q.data_ptr(), k.data_ptr(), k_param.data_ptr(), v.data_ptr(),
+                                                                v_param.data_ptr(), seqlen_indptr.data_ptr(), pos.data_ptr(),
+                                                                table.data_ptr(), kf.data_ptr(), vf.data_ptr(), out.data_ptr(), t, b,
+                                                                max_len, h, hkv, _stream(q)), "prefill_attention_i4")
+        else:
+            _lib.check(_lib.lib().atom_prefill_attention_ctx_gqa_i4(
+                q.data_ptr(), k.data_ptr(), k_param.data_ptr(), v.data_ptr(), v_param.data_ptr(), seqlen_indptr.data_ptr(),
+                pos.data_ptr(), table.data_ptr(), kf.data_ptr(), vf.data_ptr(), out.data_ptr(), t, b, max_len, h, hkv,
+                kv.data.data_ptr(), kv.param.data_ptr(), kv.indptr.data_ptr(), kv.indicies.data_ptr(), kv.last_page_offset.data_ptr(),
+                L, int(layer_idx), P, _stream(q)), "prefill_attention_i4")
     return out
+
+
+def _prefill_contexts(kv, layer_idx, seqlens):
+    """Cached tokens before each prompt (all zeros without a cache), from the host lengths the batch recorded."""
+    if kv is None:
+        return [0] * len(seqlens)
+    lens = getattr(kv, "seqlens", None)
+    if lens is None:
+        raise RuntimeError("prefill_attention_i4: `kv` carries no host sequence lengths (`seqlens`): build it as a BatchedKvCacheInt4")
+    if layer_idx is None:
+        raise RuntimeError("prefill_attention_i4: `kv` needs `layer_idx`")
+    if len(lens) != len(seqlens):
+        raise RuntimeError(f"prefill_attention_i4: `kv` holds {len(lens)} sequences for {len(seqlens)} prompts")
+    ctx = [int(s) - int(n) for s, n in zip(lens, seqlens)]
+    if min(ctx) < 0:
+        b = min(range(len(ctx)), key=ctx.__getitem__)
+        raise RuntimeError(f"prefill_attention_i4: sequence {b} holds {lens[b]} tokens, fewer than its prompt of {seqlens[b]}")
+    return ctx
 
 
 def init_kv_i4(kv, k, v, k_param, v_param, seqlen_indptr, layer_idx):

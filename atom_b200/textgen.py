@@ -79,6 +79,7 @@ MODEL_CFGS = {
 @dataclasses.dataclass
 class TextGenConfig:
     batch_size: int
+    prefill_chunk: Optional[int] = None     # at most this many prompt tokens per step (chunked prefill); None = whole prompts
 
 
 @dataclasses.dataclass
@@ -101,6 +102,16 @@ class RequestContext:
     decode_latency: float = 0.0
 
 
+@dataclasses.dataclass(eq=False)
+class _Prefill:
+    """A request whose prompt is not yet wholly in the cache."""
+    req_idx: int
+    prompt: List[int]
+    kvcache: KvCacheInt4
+    done: int = 0                           # prompt tokens already in the cache
+    start_at: Optional[float] = None        # start of the step that carried its first chunk
+
+
 @dataclasses.dataclass
 class StepBatch:
     input_ids: List[int]
@@ -111,15 +122,26 @@ class StepBatch:
 
 
 class TextGenScheduler:
-    """FCFS continuous batching over a KvPoolInt4 (bench_textgen.py:111-191 as a state machine)."""
+    """FCFS continuous batching over a KvPoolInt4 (bench_textgen.py:111-191 as a state machine).
 
-    def __init__(self, rs: RequestSet, batch_size: int, pool: KvPoolInt4, device, vocab_size: int = 32000):
+    prefill_chunk=None: a step carries the whole prompt of every request it admits (the reference's schedule).  prefill_chunk=N
+    (chunked prefill): a step carries at most N prompt tokens in all -- first the next chunks of the requests that are partly
+    prefilled, FCFS, then the first chunks of newly admitted ones -- so that a long prompt no longer stalls every running
+    sequence's decode for one long step.  A chunk is the tail of its sequence's cached tokens; the model's prefill attention then
+    also reads the chunks before it from the cache.  A request gets its first token from the step that completes its prompt."""
+
+    def __init__(self, rs: RequestSet, batch_size: int, pool: KvPoolInt4, device, vocab_size: int = 32000,
+                 prefill_chunk: Optional[int] = None):
+        if prefill_chunk is not None and int(prefill_chunk) < 1:
+            raise ValueError("prefill_chunk must be a positive number of tokens (or None)")
         self.rs, self.batch_size, self.pool, self.device = rs, batch_size, pool, device
         self.vocab_size = vocab_size
+        self.prefill_chunk = None if prefill_chunk is None else int(prefill_chunk)
         self.next_req_idx = 0
         self.workset: List[RequestContext] = []
         self.done: List[RequestContext] = []
-        self._new: list = []
+        self._prefilling: List[_Prefill] = []     # admitted, prompt not yet wholly cached (FCFS)
+        self._new: list = []                      # this step's prompt chunks: (_Prefill, first token, tokens)
         self._admitted = False
         self._blen = None
         self._rng = np.random.Generator(np.random.PCG64(seed=SEED))
@@ -128,59 +150,99 @@ class TextGenScheduler:
     def finished(self) -> bool:
         return len(self.done) == len(self.rs)
 
+    @property
+    def prompt_tokens(self) -> int:
+        """Prompt tokens the admitted step carries (0: a decode-only step)."""
+        return sum(n for _, _, n in self._new)
+
     def _pages_needed(self, prompt_len: int) -> int:
         # the prompt's pages plus one spare: the first generated token may open a new page
         return (prompt_len + self.pool.block_len - 1) // self.pool.block_len + 1
 
+    def _outstanding(self, p: _Prefill) -> int:
+        # pages a request being prefilled will still take: the rest of its prompt and the spare
+        return self._pages_needed(len(p.prompt)) - len(p.kvcache.indicies)
+
     def admit(self) -> int:
-        """Admit waiting requests (FCFS) while the batch has room and the pool has pages; returns how many are new this step."""
+        """Continue the partly prefilled requests, then admit waiting ones (FCFS) while the batch has room, the step has prompt
+        tokens to spare and the pool has pages; returns how many prompts (whole or chunks) the step carries."""
         assert not self.finished and not self._admitted, "commit() the previous step first"
-        # running requests may each need a fresh page this step; keep those in reserve before admitting anyone
-        reserve = len(self.workset)
-        while len(self.workset) + len(self._new) < self.batch_size and self.next_req_idx < len(self.rs):
+        budget = self.prefill_chunk
+        # running requests may each need a fresh page this step, and the requests being prefilled the pages of the rest of
+        # their prompt: keep those in reserve before admitting anyone, so that no admitted request ever waits for a page
+        reserve = len(self.workset) + sum(self._outstanding(p) for p in self._prefilling)
+        for p in self._prefilling:
+            if budget is not None and budget == 0:
+                break
+            n = len(p.prompt) - p.done if budget is None else min(len(p.prompt) - p.done, budget)
+            before = len(p.kvcache.indicies)
+            p.kvcache.acquire(n)                            # from the reserve
+            reserve -= len(p.kvcache.indicies) - before
+            self._new.append((p, p.done, n))
+            budget = None if budget is None else budget - n
+        while len(self.workset) + len(self._prefilling) < self.batch_size and self.next_req_idx < len(self.rs) and \
+                (budget is None or budget > 0):
             plen = int(self.rs.prompt_lens[self.next_req_idx])
             if self.pool.num_free_blocks - reserve < self._pages_needed(plen):
-                if not self.workset and not self._new:
+                if not self.workset and not self._prefilling:
                     raise RuntimeError(f"KV pool too small for request {self.next_req_idx} (prompt {plen} tokens)")
                 break
             idx = self.next_req_idx
             self.next_req_idx += 1
             prompt = self._rng.integers(0, self.vocab_size, plen).tolist()
-            self._new.append((idx, prompt, KvCacheInt4(self.pool, plen)))
-            reserve += 1
+            n = plen if budget is None else min(plen, budget)
+            p = _Prefill(idx, prompt, KvCacheInt4(self.pool, n))
+            self._prefilling.append(p)
+            self._new.append((p, 0, n))
+            reserve += self._outstanding(p)
+            budget = None if budget is None else budget - n
         self._admitted = True
         return len(self._new)
 
     def next_batch(self) -> StepBatch:
-        """The step's model inputs: prompts of the new requests, then the last token of every running request."""
+        """The step's model inputs: the prompt chunks (whole prompts without chunking), then the last token of every running
+        request."""
         if not self._admitted:
             self.admit()
         input_ids: List[int] = []
-        for _, prompt, _ in self._new:
-            input_ids.extend(prompt)
+        for p, s, n in self._new:
+            input_ids.extend(p.prompt[s:s + n])
         input_ids.extend(int(r.output[-1]) for r in self.workset)
-        self._blen = BatchLenInfo([len(p) for _, p, _ in self._new], len(self.workset), self.device)
-        prefill_kv = BatchedKvCacheInt4([kv for _, _, kv in self._new]) if self._new else None
+        self._blen = BatchLenInfo([n for _, _, n in self._new], len(self.workset), self.device)
+        prefill_kv = BatchedKvCacheInt4([p.kvcache for p, _, _ in self._new]) if self._new else None
         decode_kv = BatchedKvCacheInt4([r.kvcache for r in self.workset]) if self.workset else None
         return StepBatch(input_ids, self._blen, prefill_kv, decode_kv, len(self._new))
 
     def last_token_rows(self) -> List[int]:
-        """Rows of the step's hidden states whose logits are needed: the last token of every prompt, then all decode rows."""
+        """Rows of the step's hidden states whose logits are needed: the last token of every prompt this step completes, then
+        all decode rows.  A chunk in the middle of its prompt has none."""
         blen = self._blen
         rows = [] if blen.indptr is None else (blen.indptr[1:] - 1).tolist()
+        chunks = getattr(self, "_new", None)        # None: a bare step description, whole prompts only
+        if chunks is not None:
+            rows = [r for r, (p, s, n) in zip(rows, chunks) if s + n == len(p.prompt)]
         return rows + list(range(blen.doff, blen.doff + blen.decode))
 
     def commit(self, next_tokens, t1: float, t2: float) -> int:
         """next_tokens: one id per row of last_token_rows().  Returns the number of tokens this step processed."""
-        n_new = len(self._new)
-        assert len(next_tokens) == n_new + len(self.workset)
-        processed = sum(len(p) for _, p, _ in self._new) + len(self.workset)
+        completes = [s + n == len(p.prompt) for p, s, n in self._new]
+        n_first = sum(completes)
+        assert len(next_tokens) == n_first + len(self.workset)
+        processed = sum(n for _, _, n in self._new) + len(self.workset)
         new_workset: List[RequestContext] = []
-        for b, (req_idx, _, kv) in enumerate(self._new):
-            req = RequestContext(req_idx, kv, [int(next_tokens[b])], encode_latency=t2 - t1, decode_start_at=t1)
+        b = 0
+        for (p, _, n), c in zip(self._new, completes):
+            p.done += n
+            if p.start_at is None:
+                p.start_at = t1
+            if not c:
+                continue
+            self._prefilling.remove(p)
+            req = RequestContext(p.req_idx, p.kvcache, [int(next_tokens[b])], encode_latency=t2 - p.start_at, decode_start_at=p.start_at)
+            b += 1
             self._finish_or_continue(req, t2, new_workset)
-        for b, req in enumerate(self.workset):
-            req.output.append(int(next_tokens[n_new + b]))
+        for i, req in enumerate(self.workset):
+            req.output.append(int(next_tokens[n_first + i]))
             self._finish_or_continue(req, t2, new_workset)
         self.workset, self._new, self._admitted = new_workset, [], False
         return processed
@@ -305,14 +367,15 @@ def run_textgen(model: Callable, rs: RequestSet, cfg: TextGenConfig, pool: KvPoo
                 keep_tokens: bool = False, progress: Callable = None, decode_runner: DecodeGraphRunner = None) -> TextGenBenchResult:
     """Drive `model(input_ids, blen, prefill_kv, decode_kv) -> (logits, hidden)` through the whole request set.
     Latencies are wall-clock around the step *including* the device->host read of the next tokens (which synchronises),
-    as in the reference.  With a `decode_runner`, steps that admit no new request are replayed from its CUDA graphs."""
-    sched = TextGenScheduler(rs, cfg.batch_size, pool, device, vocab_size=_vocab_size(model))
+    as in the reference.  With a `decode_runner`, steps that carry no prompt tokens are replayed from its CUDA graphs.
+    cfg.prefill_chunk: see TextGenScheduler."""
+    sched = TextGenScheduler(rs, cfg.batch_size, pool, device, vocab_size=_vocab_size(model), prefill_chunk=cfg.prefill_chunk)
     steps = graphed = 0
     t_start = time.perf_counter()
     while not sched.finished:
-        n_new = sched.admit()
+        sched.admit()
         t1 = time.perf_counter()
-        if decode_runner is not None and n_new == 0:
+        if decode_runner is not None and sched.prompt_tokens == 0:
             next_tokens = decode_runner.run([int(r.output[-1]) for r in sched.workset], [r.kvcache for r in sched.workset])
             graphed += 1
         else:

@@ -195,6 +195,21 @@ ATOM_API int atom_prefill_attention_gqa_i4(const void* q, const void* k, const v
                                   void* out, int total_tokens, int batch_size, int max_len, int num_q_heads, int num_kv_heads,
                                   void* stream);
 
+/* EXTENSION (chunked prefill, prompt continuation): atom_prefill_attention_gqa_i4 over a cached prefix.  Prompt b is the tail of
+ * sequence b of the paged INT4 cache (the tokens atom_init_kv_i4 just wrote with the same seqlen_indptr): with seq_len_b from the
+ * page table (kv_indptr, last_page_offset) and L_b its prompt length, its ctx_b = seq_len_b - L_b cached tokens come first.  Its
+ * queries attend to all of them and, causally, to the prompt's own tokens; q and k are rotated at their absolute positions.
+ *   pos_of_token i32 [T]: ctx_b + i for token i of prompt b; rope_table: rows up to max_b(ctx_b + L_b) - 1; k_f16 / v_f16 hold
+ *   the prompt's tokens only (no scratch grows with the context); kv_*: the cache as for atom_batch_decode_gqa_i4 (num_kv_heads
+ *   heads, layer layer_idx of num_layers, page_size a multiple of 8 up to 64).  num_q_heads / num_kv_heads must be 1, 2, 4 or 8
+ *   (ATOM_E_UNSUPPORTED otherwise).  Everything else as atom_prefill_attention_gqa_i4; with every ctx_b = 0 the result equals it. */
+ATOM_API int atom_prefill_attention_ctx_gqa_i4(const void* q, const void* k, const void* k_param, const void* v, const void* v_param,
+                                      const void* seqlen_indptr, const void* pos_of_token, const void* rope_table, void* k_f16,
+                                      void* v_f16, void* out, int total_tokens, int batch_size, int max_len, int num_q_heads,
+                                      int num_kv_heads, const void* kv_data, const void* kv_param, const void* kv_indptr,
+                                      const void* kv_indices, const void* last_page_offset, int num_layers, int layer_idx,
+                                      int page_size, void* stream);
+
 /* EXTENSION (SURVEY.md 8e; the reference has no multi-GPU code): one-shot all-reduce (sum) of an FP16 vector over NVLink peer
  * memory for the tensor-parallel row-parallel projections.  peer_buffers: DEVICE array of `world` pointers to every rank's
  * receive buffer, f16 [3][world][slot_elems], every half initialised to 0x8000 (FP16 -0.0: the "not yet arrived" pattern;

@@ -47,6 +47,8 @@ def main():
     ap.add_argument("--layers", type=int, default=0, help="override the number of decoder layers (0 = the model's)")
     ap.add_argument("--block-len", type=int, default=32)
     ap.add_argument("--no-cuda-graphs", action="store_true", help="run decode-only steps eagerly too (the reference's way)")
+    ap.add_argument("--prefill-chunk", type=int, default=None,
+                    help="chunked prefill: at most this many prompt tokens per step (default: whole prompts)")
     ap.add_argument("--warmup-batches", type=int, default=1,
                     help="untimed request batches served first (first-use costs: lazy kernel loading, attribute calls, graph "
                          "capture); 0 = time the cold process like the reference's script")
@@ -60,7 +62,7 @@ def main():
     torch.manual_seed(tg.SEED)
     model = build_model(mc, layers)
     rs = tg.generate_request_set(args.batch_size * args.num_batches, args.maxlen)
-    cfg = tg.TextGenConfig(args.batch_size)
+    cfg = tg.TextGenConfig(args.batch_size, prefill_chunk=args.prefill_chunk)
     pool = KvPoolInt4(layers, mc.kv_heads, mc.hidden_size // mc.num_heads,     # the cache holds KV heads (grouped-query: fewer)
                       tg.pool_capacity(args.batch_size, args.maxlen, args.block_len), args.block_len, device)
     runner = None if args.no_cuda_graphs else tg.DecodeGraphRunner(
