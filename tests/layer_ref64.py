@@ -37,6 +37,8 @@ GEMM_AUTO = 0
 
 GEMM_ARGS = {      # the operand names of each GEMM entry point: a, b, a_scale, b_scale, a_keeper, b_keeper, a_keeper_scale, b_keeper_scale
     "dense_layer_gemm_i4_fp16": ("a", "b", "a_scale", "b_scale", "a_keeper", "b_keeper", "a_keeper_scale", "b_keeper_scale"),
+    "dense_layer_gemm_i4_o4": ("a", "b", "a_scale", "b_scale", "a_keeper", "b_keeper", "a_keeper_scale", "b_keeper_scale"),
+    "dense_layer_gemm_i4_fp16_push": ("a", "b", "a_scale", "b_scale", "a_keeper", "b_keeper", "a_keeper_scale", "b_keeper_scale"),
     "dense_layer_gemm_i4_qkv": ("a", "b_qkv", "a_scale", "b_scale_qkv", "a_keeper", "b_keeper_qkv", "a_keeper_scale", "b_keeper_scale_qkv"),
     "dense_layer_gemm_i4_gateup_act": ("a", "b_gu", "a_scale", "b_scale_gu", "a_keeper", "b_keeper_gu", "a_keeper_scale",
                                        "b_keeper_scale_gu"),
@@ -82,12 +84,12 @@ class Call:
 
 class Recorder:
     """Replaces the recorded `atom_b200.ops` functions (install(monkeypatch)) by wrappers that append a Call per invocation to
-    `calls`.  `impl` maps a name to the function that does the work (default: the real operator)."""
+    `calls`.  `impl` maps a name to the function that does the work (default: the real operator); `names`: the recorded ops."""
 
-    def __init__(self, impl=None):
+    def __init__(self, impl=None, names=RECORDED_OPS):
         from atom_b200 import ops
         self.ops, self.calls = ops, []
-        self.impl = {n: (impl or {}).get(n, getattr(ops, n)) for n in RECORDED_OPS}
+        self.impl = {n: (impl or {}).get(n, getattr(ops, n)) for n in names}
 
     def install(self, monkeypatch):
         for name, fn in self.impl.items():
@@ -101,9 +103,12 @@ class Recorder:
             b = sig.bind(*args, **kwargs)
             b.apply_defaults()
             out = fn(*args, **kwargs)
-            self.calls.append(Call(name, {k: host(v) for k, v in b.arguments.items()}, host(out)))
+            self._log(Call(name, {k: host(v) for k, v in b.arguments.items()}, host(out)))
             return out
         return rec
+
+    def _log(self, call):
+        self.calls.append(call)
 
 
 # ------------------------------------------------------------------------------------------------------------------ parameters
@@ -145,6 +150,11 @@ class MoeParams:
         self.w2 = tuple(host(t) for t in (moe.w2_int4, moe.w2_scale, moe.w2_int8, moe.w2_keeper_scale))
 
 
+def norm_params(norm):
+    """(weight, reorder_index, eps) of a LlamaRMSNormInt4, as stored."""
+    return host(norm.weight), host(norm.reorder_index), norm.variance_epsilon
+
+
 class LayerParams:
     """What the reference knows of one LlamaDecoderLayer or MixtralDecoderLayer: its parameters, as stored.  The operands of the
     fused q/k/v and gate/up launches are the reference's own concatenation of q_proj / k_proj / v_proj and gate_proj / up_proj."""
@@ -153,9 +163,7 @@ class LayerParams:
         a = layer.self_attn
         self.index, self.hidden = index, a.hidden_size
         self.hq, self.hkv, self.theta = a.num_heads, a.num_kv_heads, a.rope_theta
-        self.ln1 = (host(layer.input_layernorm.weight), host(layer.input_layernorm.reorder_index), layer.input_layernorm.variance_epsilon)
-        self.ln2 = (host(layer.post_attention_layernorm.weight), host(layer.post_attention_layernorm.reorder_index),
-                    layer.post_attention_layernorm.variance_epsilon)
+        self.ln1, self.ln2 = norm_params(layer.input_layernorm), norm_params(layer.post_attention_layernorm)
         self.attn_index = host(a.reorder_index)
         self.qkv = Lin.cat([Lin.of(a.q_proj), Lin.of(a.k_proj), Lin.of(a.v_proj)])
         self.o = Lin.of(a.o_proj)
@@ -217,8 +225,12 @@ class ModelRef:
         self.hist = {}                      # (key, layer) -> [k u8 [n, Hkv, 64], k (s, z) [n, Hkv, 2], v, v (s, z)]
 
     # ---------------------------------------------------------------------------------------------------------- checks
+    def _where(self, st):
+        """The stage as errors name it."""
+        return st
+
     def _fail(self, st, msg):
-        raise WiringError(f"{st}: {msg}")
+        raise WiringError(f"{self._where(st)}: {msg}")
 
     def _eq(self, st, what, got, want):
         if not same(got, want):
@@ -279,7 +291,10 @@ class ModelRef:
             bad = np.argwhere(got.view(np.uint16) != ref.view(np.uint16))
             self._fail(st, f"FP16 GEMM differs from the oracle at K split {ksplit} ({len(bad)} values, first at {bad[:1].tolist()})")
         S, T = G.ref64(*t, rows=rows)
-        G.check_o16(got, S, T, lin.k // 128 - 1, ksplit, what=st)
+        try:
+            G.check_o16(got, S, T, lin.k // 128 - 1, ksplit, what=self._where(st))
+        except AssertionError as e:
+            raise WiringError(str(e)) from None
 
     def _o4(self, st, act, lin, out, rows):
         t = (act[1], lin.b, act[3], lin.bs, act[0], lin.bk, act[2], lin.bks)
@@ -289,7 +304,7 @@ class ModelRef:
             self._fail(st, "INT4 GEMM output (codes or (scale, zero)) differs from the oracle")
         S, T = G.ref64(*t, rows=rows)
         try:
-            G.check_o4(gd, gds, S, T, lin.k // 128 - 1, what=st)
+            G.check_o4(gd, gds, S, T, lin.k // 128 - 1, what=self._where(st))
         except AssertionError as e:                                  # names the stage, (row, head) and element
             raise WiringError(str(e)) from None
 
@@ -369,23 +384,9 @@ class ModelRef:
                 residual = s
                 ref = O.rmsnorm_fp16_i4(s, w, idx, eps)
             st = f"{L} input_layernorm"
-            self._eq(st, "weight", c.args["weight"], w)
-            self._eq(st, "reorder_index", c.args["reorder_index"], idx)
-            if c.args["eps"] != eps:
-                self._fail(st, f"eps {c.args['eps']} != {eps}")
+            self._norm_args(st, c, p.ln1)
             self._quant(st, x, ref, m, exact=False)
-            # ---- q/k/v
-            st = f"{L} qkv_proj"
-            c = self._next(st, ["dense_layer_gemm_i4_qkv"])
-            self._gemm_call(st, c, x, p.qkv)
-            nq, nkv = p.hq * 128, p.hkv * 128
-            if c.args["kv_rows"] != nkv:
-                self._fail(st, f"kv_rows {c.args['kv_rows']} != {nkv}")
-            q, (k4, ks), (v4, vs) = c.out
-            self._o16(st + " (q)", x, p.qkv.rows(0, nq), q, 1)
-            rows = self._rows(m, 2 * nkv, p.hidden)
-            self._o4(st + " (k)", x, p.qkv.rows(nq, nq + nkv), (k4, ks), rows)
-            self._o4(st + " (v)", x, p.qkv.rows(nq + nkv, nq + 2 * nkv), (v4, vs), rows)
+            q, k4, ks, v4, vs = self._qkv(L, p, x, m)
             stack = []
             # ---- prompts: cache write and causal attention over their own K/V
             if pf:
@@ -418,41 +419,10 @@ class ModelRef:
                 stack.append(c.out)
             # ---- running sequences: one appended position, decode attention over the whole history
             if nd:
-                st = f"{L} append_kv"
-                c = self._next(st, ["append_kv_i4"])
-                for name, t in (("k", k4), ("v", v4), ("k_param", ks), ("v_param", vs)):
-                    self._eq(st, name, c.args[name], t[doff:])
-                self._table(st, c.args["kv"], step.dtab)
-                if c.args["layer_idx"] != l:
-                    self._fail(st, f"layer_idx {c.args['layer_idx']}, the layer is {l}")
-                seqs = []
-                for j, key in enumerate(dkeys):
-                    h = self.hist.get((key, l))
-                    if h is None or len(h[0]) != self.seqs[key][1] - 1:
-                        self._fail(st, f"decode row {j}: the reference holds no history of {self.seqs[key][1] - 1} positions")
-                    r = doff + j
-                    new = (k4[r].reshape(1, p.hkv, 64), ks[r].reshape(1, p.hkv, 2), v4[r].reshape(1, p.hkv, 64), vs[r].reshape(1, p.hkv, 2))
-                    h = self.hist[(key, l)] = [np.concatenate([a, b]) for a, b in zip(h, new)]
-                    un = lambda b: A.unpack(b.transpose(1, 0, 2))                               # noqa: E731  [Hkv, n, 128]
-                    seqs.append((un(h[0]), h[1].transpose(1, 0, 2), un(h[2]), h[3].transpose(1, 0, 2)))
-                st = f"{L} batch_decode"
-                c = self._next(st, ["batch_decode_i4"])
-                self._eq(st, "q", c.args["q"], q[doff:])
-                self._table(st, c.args["kv"], step.dtab)
-                if c.args["layer_idx"] != l or c.args["rope_theta"] != p.theta:
-                    self._fail(st, f"layer_idx {c.args['layer_idx']} / rope_theta {c.args['rope_theta']}, expected {l} / {p.theta}")
-                data, param, ip, ind, last = A.make_pool(seqs, self.P, p.hkv)                     # private: from the history alone
-                ref, bnd = A.decode_bound(q[doff:].reshape(nd, p.hq, 128), data, param, ip, ind, last, 0, p.hq, p.theta)
-                self._attn_bound(st, c.out, ref, bnd)
-                stack.append(c.out.reshape(nd, p.hidden))
+                stack.append(self._decode(L, l, p, q, k4, ks, v4, vs, doff, nd, dkeys, step.dtab))
             attn = np.concatenate(stack) if len(stack) > 1 else stack[0]
             # ---- o_proj
-            st = f"{L} o_proj reorder"
-            c = self._next(st, ["reorder_fp16_i4"])
-            self._eq(st, "hidden_states ([prefill attention; decode attention])", c.args["hidden_states"], attn)
-            self._eq(st, "reorder_index", c.args["reorder_index"], p.attn_index)
-            self._quant(st, c.out, O.reorder_fp16_i4(attn.reshape(m, p.hidden), p.attn_index), m)
-            xo = c.out
+            xo = self._reorder(L, p, attn, m)
             st = f"{L} o_proj"
             c = self._next(st, ["dense_layer_gemm_i4_fp16"])
             self._gemm_call(st, c, xo, p.o, GEMM_AUTO)
@@ -464,8 +434,7 @@ class ModelRef:
             self._eq(st, "hidden_states", c.args["hidden_states"], o)
             self._eq(st, "residual", c.args["residual"], residual)
             w, idx, eps = p.ln2
-            self._eq(st, "weight", c.args["weight"], w)
-            self._eq(st, "reorder_index", c.args["reorder_index"], idx)
+            self._norm_args(st, c, p.ln2)
             s, x = c.out
             if not same(s, fp16_sum(residual, o)):
                 self._fail(st, "residual + attention is not the exact FP16 sum")
@@ -484,8 +453,93 @@ class ModelRef:
             self._audit(pool_before, pool_after, pkeys + dkeys)
         return step.info
 
+    # ---------------------------------------------------------------------------------------------------------- stages
+    def _norm_args(self, st, c, ln):
+        w, idx, eps = ln
+        self._eq(st, "weight", c.args["weight"], w)
+        self._eq(st, "reorder_index", c.args["reorder_index"], idx)
+        if c.args["eps"] != eps:
+            self._fail(st, f"eps {c.args['eps']} != {eps}")
+
+    def _qkv(self, L, p, x, m, fused=True):
+        """The q/k/v projections of the quantised input x: one fused launch, or (fused=False) q_proj, k_proj and v_proj as three
+        GEMMs on the projections' own operands (p.q, p.k, p.v).  Returns (q, k codes, k (scale, zero), v codes, v (scale, zero))."""
+        st = f"{L} qkv_proj"
+        nq, nkv = p.hq * 128, p.hkv * 128
+        rows = self._rows(m, 2 * nkv, p.hidden)
+        if fused:
+            c = self._next(st, ["dense_layer_gemm_i4_qkv"])
+            self._gemm_call(st, c, x, p.qkv)
+            if c.args["kv_rows"] != nkv:
+                self._fail(st, f"kv_rows {c.args['kv_rows']} != {nkv}")
+            q, (k4, ks), (v4, vs) = c.out
+            self._o16(st + " (q)", x, p.qkv.rows(0, nq), q, 1)
+        else:
+            c = self._next(f"{L} q_proj", ["dense_layer_gemm_i4_fp16"])
+            self._gemm_call(f"{L} q_proj", c, x, p.q, GEMM_AUTO)
+            q = c.out
+            self._o16(f"{L} q_proj", x, p.q, q, G.dispatch(m, nq, p.hidden, GEMM_AUTO)[1])
+            kv = []
+            for name, lin in (("k_proj", p.k), ("v_proj", p.v)):
+                c = self._next(f"{L} {name}", ["dense_layer_gemm_i4_o4"])
+                self._gemm_call(f"{L} {name}", c, x, lin, GEMM_AUTO)
+                kv.append(c.out)
+            (k4, ks), (v4, vs) = kv
+            st = f"{L} k_proj / v_proj"
+        self._o4(st + " (k)", x, p.qkv.rows(nq, nq + nkv), (k4, ks), rows)
+        self._o4(st + " (v)", x, p.qkv.rows(nq + nkv, nq + 2 * nkv), (v4, vs), rows)
+        return q, k4, ks, v4, vs
+
+    def _decode(self, L, l, p, q, k4, ks, v4, vs, doff, nd, dkeys, dtab):
+        """append_kv of the rows [doff, doff + nd) and decode attention over each running sequence's history; returns the
+        attention output [nd, heads * 128]."""
+        st = f"{L} append_kv"
+        c = self._next(st, ["append_kv_i4"])
+        for name, t in (("k", k4), ("v", v4), ("k_param", ks), ("v_param", vs)):
+            self._eq(st, name, c.args[name], t[doff:])
+        self._table(st, c.args["kv"], dtab)
+        if c.args["layer_idx"] != l:
+            self._fail(st, f"layer_idx {c.args['layer_idx']}, the layer is {l}")
+        seqs = []
+        for j, key in enumerate(dkeys):
+            h = self.hist.get((key, l))
+            if h is None or len(h[0]) != self.seqs[key][1] - 1:
+                self._fail(st, f"decode row {j}: the reference holds no history of {self.seqs[key][1] - 1} positions")
+            r = doff + j
+            new = (k4[r].reshape(1, p.hkv, 64), ks[r].reshape(1, p.hkv, 2), v4[r].reshape(1, p.hkv, 64), vs[r].reshape(1, p.hkv, 2))
+            h = self.hist[(key, l)] = [np.concatenate([a, b]) for a, b in zip(h, new)]
+            un = lambda b: A.unpack(b.transpose(1, 0, 2))                               # noqa: E731  [Hkv, n, 128]
+            seqs.append((un(h[0]), h[1].transpose(1, 0, 2), un(h[2]), h[3].transpose(1, 0, 2)))
+        st = f"{L} batch_decode"
+        c = self._next(st, ["batch_decode_i4"])
+        self._eq(st, "q", c.args["q"], q[doff:])
+        self._table(st, c.args["kv"], dtab)
+        if c.args["layer_idx"] != l or c.args["rope_theta"] != p.theta:
+            self._fail(st, f"layer_idx {c.args['layer_idx']} / rope_theta {c.args['rope_theta']}, expected {l} / {p.theta}")
+        data, param, ip, ind, last = A.make_pool(seqs, self.P, p.hkv)                     # private: from the history alone
+        ref, bnd = A.decode_bound(q[doff:].reshape(nd, p.hq, 128), data, param, ip, ind, last, 0, p.hq, p.theta)
+        self._attn_bound(st, c.out, ref, bnd)
+        return c.out.reshape(nd, p.hq * 128)
+
+    def _reorder(self, L, p, attn, m):
+        st = f"{L} o_proj reorder"
+        c = self._next(st, ["reorder_fp16_i4"])
+        self._eq(st, "hidden_states ([prefill attention; decode attention])", c.args["hidden_states"], attn)
+        self._eq(st, "reorder_index", c.args["reorder_index"], p.attn_index)
+        self._quant(st, c.out, O.reorder_fp16_i4(attn.reshape(m, p.hq * 128), p.attn_index), m)
+        return c.out
+
     def _mlp(self, L, p, x, m):
-        """gate/up (one fused launch for M <= 64, else two GEMMs and activate), then down; returns the FP16 delta."""
+        """gate/up and activate, then down; returns the FP16 delta."""
+        xa = self._gateup(L, p, x, m)
+        st = f"{L} down_proj"
+        c = self._next(st, ["dense_layer_gemm_i4_fp16"])
+        self._gemm_call(st, c, xa, p.down, GEMM_AUTO)
+        self._o16(st, xa, p.down, c.out, G.dispatch(m, p.hidden, p.inter, GEMM_AUTO)[1])
+        return c.out
+
+    def _gateup(self, L, p, x, m):
+        """gate/up (one fused launch for M <= 64, else two GEMMs and activate); returns the quantised activation."""
         if m <= 64:
             st = f"{L} gate/up (fused)"
             c = self._next(st, ["dense_layer_gemm_i4_gateup_act"])
@@ -507,11 +561,6 @@ class ModelRef:
             self._eq(st, "a (gate)", c.args["a"], outs[0])
             self._eq(st, "b (up)", c.args["b"], outs[1])
             self._quant(st, c.out, O.activate_fp16_i4(outs[0], outs[1]), m, exact=False)
-        st = f"{L} down_proj"
-        xa = c.out
-        c = self._next(st, ["dense_layer_gemm_i4_fp16"])
-        self._gemm_call(st, c, xa, p.down, GEMM_AUTO)
-        self._o16(st, xa, p.down, c.out, G.dispatch(m, p.hidden, p.inter, GEMM_AUTO)[1])
         return c.out
 
     def _moe(self, L, p, s, x, m):
@@ -660,7 +709,7 @@ class ModelRef:
         bad_p = np.argwhere(param.view(np.uint16) != after[1].view(np.uint16))
         if len(bad_d) or len(bad_p):
             where = (bad_d if len(bad_d) else bad_p)[0].tolist()
-            self._fail("pool audit", f"{len(bad_d)} data bytes and {len(bad_p)} parameters differ from the reference's history "
+            self._fail(f"layer {where[1]} pool audit", f"{len(bad_d)} data bytes and {len(bad_p)} parameters differ from the reference's history "
                                      f"(owned slots) or from the pool before the step (all others); first at "
                                      f"[page, layer, k|v, head, entry] = {where[:5]}")
 
