@@ -7,8 +7,8 @@
 // a mask, no sign extension) on their way to the tensor cores:
 //
 //   TMA: packed INT4 tiles (64 B rows) of the weights (128 channels) and of the tokens (BN rows) -> smem "packed ring"
-//   producer warpgroup: one thread issues the TMA loads; all four warps widen the TOKEN tile into the K-major SWIZZLE_128B
-//       INT8 operand ("expanded ring") and stage the group's scales next to it
+//   producer warpgroup: one thread issues the TMA loads; three warps widen the TOKEN tile into the K-major SWIZZLE_128B
+//       INT8 operand ("expanded ring"), the fourth loads the groups' scales a few groups ahead and stages them next to it
 //   two consumer warpgroups, 64 channels each: the WEIGHTS are the wgmma A operand and are widened in REGISTERS (one LDS.128
 //       per row and group, no shared-memory round trip); wgmma m64nBNk32 s8 x 4 per 128-wide quantisation group, INT32
 //       accumulators in registers; acc = fmaf(float(c), float(hmul(sA, sB)), acc)
@@ -59,7 +59,8 @@ struct GemmArgs {
 //   5 producer past griddepcontrol.wait | 6 split-K reduction + output stores done | 7 consumers leave
 // Stamps 2, 3, 6 and 7 come from consumer warp 0, the others from thread 0 (the same SM clock).
 // Built with -DATOM_GEMM_TRACE_GROUPS, INT4 group s < TRACE_GROUPS also stamps slot 8 + kind * TRACE_GROUPS + s:
-//   producer thread 0:  0 pack_full passed | 1 scale slot free (exp_empty) | 2 scales stored (their loads returned) | 3 exp_full
+//   producer thread 0:  0 pack_full passed | 3 exp_full (token tile widened)
+//   scale warp, lane 0: 1 scale slot free (exp_empty) | 2 scales stored (their loads returned)
 //   consumer warp 0:    4 pack_full passed | 5 exp_full passed | 6 group dequantised
 // A compile-time switch: even untaken, a runtime branch in the per-group loops costs the 16-token split-K launch about
 // 0.6 us (H100 80GB HBM3, 700 W).
@@ -101,6 +102,14 @@ struct GemmCfg {
   static constexpr int THREADS = 384;                            // producer warpgroup + two consumer warpgroups
   static constexpr int PACK = BN <= 32 ? 8 : 4;                  // packed ring depth (groups): decode shapes are a weight stream
   static constexpr int EXP = BN <= 64 ? 4 : 3;                   // expanded token tiles / scale slots
+  // Decode tiles (BN <= 32) load the scales in a producer warp of their own (SCALE_WARP), SCALE_AHEAD groups ahead, and
+  // widen the token tile with the other three; larger tiles need all four warps to widen and load the scales in line.
+  static constexpr bool SCALE_WARP_ON = BN <= 32;
+  static constexpr int SCALE_WARP = 3;
+  static constexpr int SCALE_AHEAD = 4;                          // groups whose scale loads the scale warp keeps in flight
+  static constexpr int SCALE_THREADS = SCALE_WARP_ON ? 32 : 128;  // threads that load and store a group's scales
+  static constexpr int WIDEN_THREADS = SCALE_WARP_ON ? 96 : 128;  // threads that widen the token tile
+  static constexpr int TOK_PER_THREAD = (BN + SCALE_THREADS - 1) / SCALE_THREADS;
   static constexpr int PACK_W = ROWS * 64, PACK_Q = BN * 64;     // bytes per packed group
   static constexpr int EXP_Q = BN * 128 < 1024 ? 1024 : BN * 128;
   static constexpr int SCALE_BYTES = (ROWS + BN) * 2;            // [ROWS] weight-scale halves, [BN] token-scale halves
@@ -140,10 +149,10 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR);
   uint64_t* pack_full = bars;                          // TMA landed the group's packed tiles            (1 + tx)
-  uint64_t* pack_empty = pack_full + C::PACK;          // every warp has read them                       (12)
+  uint64_t* pack_empty = pack_full + C::PACK;          // every warp has read them  (the widening + the 8 consumer warps)
   uint64_t* exp_full = pack_empty + C::PACK;           // token operand + scales of the group in place   (4 producer warps)
   uint64_t* exp_empty = exp_full + C::EXP;             // consumers are done with them                   (8 consumer warps)
-  uint64_t* keep_full = exp_empty + C::EXP;            // keeper tiles + scales landed                   (1 + tx, 4 producer warps)
+  uint64_t* keep_full = exp_empty + C::EXP;            // keeper tiles + scales landed     (1 + tx, the scale-loading warps)
 
   // the warp index through a shuffle: the compiler then knows the role branches below are warp-uniform
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
@@ -177,9 +186,9 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_w4); tma_prefetch_desc(&tm_a4); tma_prefetch_desc(&tm_w8); tma_prefetch_desc(&tm_a8);
-    for (int i = 0; i < C::PACK; ++i) { mbar_init(&pack_full[i], 1); mbar_init(&pack_empty[i], 12); }
+    for (int i = 0; i < C::PACK; ++i) { mbar_init(&pack_full[i], 1); mbar_init(&pack_empty[i], C::SCALE_WARP_ON ? 11 : 12); }
     for (int i = 0; i < C::EXP; ++i) { mbar_init(&exp_full[i], 4); mbar_init(&exp_empty[i], 8); }
-    mbar_init(keep_full, 5);
+    mbar_init(keep_full, C::SCALE_WARP_ON ? 2 : 5);
     fence_barrier_init();
   }
   __syncthreads();
@@ -205,21 +214,6 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
       }
       if (part != 1) tma_load_2d(smem + C::OFF_PACK_Q + ps * C::PACK_Q, &tm_a4, &pack_full[ps], g * 64, m0);
     };
-    // a group's scales: weight scales of the tile's channels (16-B chunks), token scales in token order
-    auto load_scales = [&](const __half* bs_row, const __half* as_row, uint4& sbv, __half& sav) {
-      sbv = make_uint4(0, 0, 0, 0);
-      sav = __ushort_as_half(0);
-      if (t < C::ROWS / 8) {
-        const int seg = t / 16, c = t % 16;                         // gate/up: segment 1 = the up rows
-        if (n0 + 8 * c < n_limit) sbv = ld_cg_v4(bs_row + (size_t)seg * args.gu_rows + n0 + 8 * c);
-      }
-      if (t < BN && m0 + t < (kGrouped ? gtile.y + gtile.z : args.M)) sav = __ushort_as_half(ld_cg_u16(as_row + scale_index(m0 + t)));
-    };
-    auto store_scales = [&](int slot_idx, const uint4& sbv, __half sav) {
-      uint8_t* slot = smem + C::OFF_SCALE + slot_idx * C::SCALE_BYTES;
-      if (t < C::ROWS / 8) reinterpret_cast<uint4*>(slot)[t] = sbv;
-      if (t < BN) reinterpret_cast<__half*>(slot + C::ROWS * 2)[t] = sav;
-    };
     griddep_launch_dependents();
     if (t == 0) {
       const int first = min(C::PACK, n4);
@@ -238,46 +232,110 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
     } else {
       griddep_wait();
     }
-    uint4 sbv;
-    __half sav;
-    if (has_keeper) {
-      load_scales(kGrouped ? args.b_keeper_scale + (size_t)gtile.x * args.expert_rows : args.b_keeper_scale, args.a_keeper_scale, sbv, sav);
-      store_scales(C::EXP, sbv, sav);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(keep_full);
-    }
-    for (int s = 0; s < n4; ++s) {
-      const int ps = s % C::PACK, es = s % C::EXP, g = g_begin + s;
-      load_scales((kGrouped ? args.b_scale + (size_t)gtile.x * args.G * args.ldb_scale : args.b_scale) + (size_t)g * args.ldb_scale, args.a_scale + (size_t)g * args.lda_scale, sbv, sav);
-      if (t == 0 && s >= 1 && s + C::PACK - 1 < n4) {               // refill the slot the previous group has left
-        const int nx = s + C::PACK - 1;
-        mbar_wait(&pack_empty[nx % C::PACK], ((nx / C::PACK) - 1) & 1);
-        issue_stage(nx, 0);
+    // a group's scales: weight scales of the tile's channels (16-B chunks), token scales in token order, loaded by
+    // SCALE_THREADS threads (index si)
+    struct Scales { uint4 b; __half a[C::TOK_PER_THREAD]; };
+    const int si = C::SCALE_WARP_ON ? lane : t;
+    const int m_end = kGrouped ? gtile.y + gtile.z : args.M;
+    auto load_scales = [&](const __half* bs_row, const __half* as_row, Scales& sc) {
+      sc.b = make_uint4(0, 0, 0, 0);
+      if (si < C::ROWS / 8) {
+        const int seg = si / 16, c = si % 16;                         // gate/up: segment 1 = the up rows
+        if (n0 + 8 * c < n_limit) sc.b = ld_cg_v4(bs_row + (size_t)seg * args.gu_rows + n0 + 8 * c);
       }
-      mbar_wait(&pack_full[ps], (s / C::PACK) & 1);
-      if (t == 0) trace_group(args, 0, s);
-      if (s >= C::EXP) mbar_wait(&exp_empty[es], ((s / C::EXP) - 1) & 1);
-      if (t == 0) trace_group(args, 1, s);
-      const uint8_t* packed = smem + C::OFF_PACK_Q + ps * C::PACK_Q;
-      uint8_t* expanded = smem + C::OFF_EXP + es * C::EXP_Q;
 #pragma unroll
-      for (int c = t; c < BN * 4; c += 128) {
-        const int r = c >> 2, qq = c & 3;
-        const uint4 w = *reinterpret_cast<const uint4*>(packed + c * 16);
-        const uint32_t ww[4] = {w.x, w.y, w.z, w.w};
-        uint8_t* row = expanded + (r >> 3) * 1024 + (r & 7) * 128 + 4 * qq;
+      for (int i = 0; i < C::TOK_PER_THREAD; ++i) {
+        const int tk = si + C::SCALE_THREADS * i;
+        sc.a[i] = __ushort_as_half(0);
+        if (tk < BN && m0 + tk < m_end) sc.a[i] = __ushort_as_half(ld_cg_u16(as_row + scale_index(m0 + tk)));
+      }
+    };
+    auto load_group = [&](int s, Scales& sc) {
+      const int g = g_begin + s;
+      load_scales((kGrouped ? args.b_scale + (size_t)gtile.x * args.G * args.ldb_scale : args.b_scale) + (size_t)g * args.ldb_scale,
+                  args.a_scale + (size_t)g * args.lda_scale, sc);
+    };
+    auto store_scales = [&](int slot_idx, const Scales& sc) {
+      uint8_t* slot = smem + C::OFF_SCALE + slot_idx * C::SCALE_BYTES;
+      if (si < C::ROWS / 8) reinterpret_cast<uint4*>(slot)[si] = sc.b;
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          *reinterpret_cast<uint32_t*>(row + (((2 * j) ^ (r & 7)) << 4)) = (ww[j] << 4) & 0xF0F0F0F0u;
-          *reinterpret_cast<uint32_t*>(row + (((2 * j + 1) ^ (r & 7)) << 4)) = ww[j] & 0xF0F0F0F0u;
+      for (int i = 0; i < C::TOK_PER_THREAD; ++i)
+        if (si + C::SCALE_THREADS * i < BN) reinterpret_cast<__half*>(slot + C::ROWS * 2)[si + C::SCALE_THREADS * i] = sc.a[i];
+    };
+    auto load_keeper = [&](Scales& sc) {
+      load_scales(kGrouped ? args.b_keeper_scale + (size_t)gtile.x * args.expert_rows : args.b_keeper_scale, args.a_keeper_scale, sc);
+    };
+    if (C::SCALE_WARP_ON && warp == C::SCALE_WARP) {
+      // ---------------------------------------------------------- scale warp: the per-group weight and token scales
+      // Global loads, each an HBM round trip that the next launch's weight prefetch makes long.  Loaded in line by the
+      // widening warps, which fence the async proxy once per group, they cost one round trip per group; this warp never
+      // fences and keeps SCALE_AHEAD groups of them in flight.
+      Scales keep, ahead[C::SCALE_AHEAD];
+      if (has_keeper) load_keeper(keep);
+#pragma unroll
+      for (int u = 0; u < C::SCALE_AHEAD; ++u)
+        if (u < n4) load_group(u, ahead[u]);
+      if (has_keeper) {
+        store_scales(C::EXP, keep);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(keep_full);
+      }
+      // unrolled by SCALE_AHEAD so that every register set keeps a fixed place
+      for (int s0 = 0; s0 < n4; s0 += C::SCALE_AHEAD) {
+#pragma unroll
+        for (int u = 0; u < C::SCALE_AHEAD; ++u) {
+          const int s = s0 + u, es = s % C::EXP;
+          if (s < n4) {
+            if (s >= C::EXP) mbar_wait(&exp_empty[es], ((s / C::EXP) - 1) & 1);
+            if (lane == 0) trace_group(args, 1, s);
+            store_scales(es, ahead[u]);
+            if (lane == 0) trace_group(args, 2, s);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&exp_full[es]);
+            if (s + C::SCALE_AHEAD < n4) load_group(s + C::SCALE_AHEAD, ahead[u]);
+          }
         }
       }
-      store_scales(es, sbv, sav);
-      if (t == 0) trace_group(args, 2, s);
-      fence_proxy_async_smem();             // generic-proxy stores -> visible to the wgmma operand fetch
-      __syncwarp();
-      if (lane == 0) { mbar_arrive(&pack_empty[ps]); mbar_arrive(&exp_full[es]); }
-      if (t == 0) trace_group(args, 3, s);
+    } else {
+      // ---------------------------------------------------------- widening warps: the token tile into the INT8 operand
+      Scales cur;                            // larger tiles: the group's scales, loaded in line
+      if (!C::SCALE_WARP_ON && has_keeper) {
+        load_keeper(cur);
+        store_scales(C::EXP, cur);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(keep_full);
+      }
+      for (int s = 0; s < n4; ++s) {
+        const int ps = s % C::PACK, es = s % C::EXP;
+        if constexpr (!C::SCALE_WARP_ON) load_group(s, cur);
+        if (t == 0 && s >= 1 && s + C::PACK - 1 < n4) {               // refill the slot the previous group has left
+          const int nx = s + C::PACK - 1;
+          mbar_wait(&pack_empty[nx % C::PACK], ((nx / C::PACK) - 1) & 1);
+          issue_stage(nx, 0);
+        }
+        mbar_wait(&pack_full[ps], (s / C::PACK) & 1);
+        if (t == 0) trace_group(args, 0, s);
+        if (s >= C::EXP) mbar_wait(&exp_empty[es], ((s / C::EXP) - 1) & 1);
+        const uint8_t* packed = smem + C::OFF_PACK_Q + ps * C::PACK_Q;
+        uint8_t* expanded = smem + C::OFF_EXP + es * C::EXP_Q;
+#pragma unroll
+        for (int c = t; c < BN * 4; c += C::WIDEN_THREADS) {
+          const int r = c >> 2, qq = c & 3;
+          const uint4 w = *reinterpret_cast<const uint4*>(packed + c * 16);
+          const uint32_t ww[4] = {w.x, w.y, w.z, w.w};
+          uint8_t* row = expanded + (r >> 3) * 1024 + (r & 7) * 128 + 4 * qq;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            *reinterpret_cast<uint32_t*>(row + (((2 * j) ^ (r & 7)) << 4)) = (ww[j] << 4) & 0xF0F0F0F0u;
+            *reinterpret_cast<uint32_t*>(row + (((2 * j + 1) ^ (r & 7)) << 4)) = ww[j] & 0xF0F0F0F0u;
+          }
+        }
+        if constexpr (!C::SCALE_WARP_ON) store_scales(es, cur);
+        fence_proxy_async_smem();             // generic-proxy stores -> visible to the wgmma operand fetch
+        __syncwarp();
+        if (lane == 0) { mbar_arrive(&pack_empty[ps]); mbar_arrive(&exp_full[es]); }
+        if (t == 0) trace_group(args, 3, s);
+      }
     }
     if constexpr (kSplit > 1) { cluster_wait(); cluster_arrive(); cluster_wait(); cluster_arrive(); cluster_wait(); }
   } else {
