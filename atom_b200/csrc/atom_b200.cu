@@ -23,6 +23,7 @@
 #include "gemm_i4_sm90.cuh"
 #include "kv_kernels.cuh"
 #include "prefill_kernels.cuh"
+#include "cascade_kernels.cuh"
 #include "comm_kernels.cuh"
 #include "quant_kernels.cuh"
 #include "moe_kernels.cuh"
@@ -666,6 +667,38 @@ static int dispatch_decode(const char* what, void* o, const void* q, const atom:
   return launch_decode<G, 8, 0>(what, o, q, kv, log2_theta, split, stream);
 }
 
+// the cascade's suffix pass: batch_decode_kernel<..., DecPrefix>, grid (B, Hkv), the page sizes as dispatch_decode picks them;
+// the DecPrefix argument goes after pdl, so the launch is spelled out
+template <int G, int kMaxTpl, int kP>
+static int launch_decode_shared_k(const char* what, void* o, const void* q, const atom::KvArgs& kv, const atom::DecPrefix& px,
+                                  float log2_theta, cudaStream_t stream) {
+  auto kern = atom::batch_decode_kernel<G, kMaxTpl, kP, false, atom::DecPrefix>;
+  int rc = ensure_dynamic_smem(kern, 100 * 1024, what);
+  if (rc) return rc;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(kv.B, kv.H); cfg.blockDim = dim3(atom::dec_threads(G));
+  cfg.dynamicSmemBytes = atom::batch_decode_smem_bytes(G, kv.P); cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  const int pdl = pdl_enabled() ? 1 : 0;
+  if (pdl) {
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr; cfg.numAttrs = 1;
+  }
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, (__half*)o, (const __half*)q, kv, log2_theta, pdl, px);
+  if (e != cudaSuccess) return fail(ATOM_E_CUDA, "%s launch: %s", what, cudaGetErrorString(e));
+  return check_launch(what);
+}
+
+template <int G>
+static int launch_decode_shared(const char* what, void* o, const void* q, const atom::KvArgs& kv, const atom::DecPrefix& px,
+                                float log2_theta, cudaStream_t stream) {
+  if (kv.P == 16) return launch_decode_shared_k<G, 2, 16>(what, o, q, kv, px, log2_theta, stream);
+  if (kv.P == 32) return launch_decode_shared_k<G, 4, 32>(what, o, q, kv, px, log2_theta, stream);
+  if (G == 1 && kv.P <= 32) return launch_decode_shared_k<1, 4, 0>(what, o, q, kv, px, log2_theta, stream);
+  return launch_decode_shared_k<G, 8, 0>(what, o, q, kv, px, log2_theta, stream);
+}
+
 static int batch_decode(const char* what, void* o, const void* q, const void* kv_data, const void* kv_param, const void* kv_indptr,
                         const void* kv_indices, const void* last_page_offset, int num_layers, int layer_idx, int num_q_heads,
                         int num_kv_heads, int page_size, int batch_size, float rope_theta, int kv_split, void* stream) {
@@ -736,6 +769,55 @@ int atom_batch_decode_split_gqa_i4(void* o, const void* q, const void* kv_data, 
                                    void* stream) {
   return batch_decode("batch_decode_split_gqa_i4", o, q, kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers,
                       layer_idx, num_q_heads, num_kv_heads, page_size, batch_size, rope_theta, kv_split, stream);
+}
+
+// Cascade chunk count: the fewest chunks that give the prefix pass two CTAs per SM when every group takes the row blocks of the
+// whole batch (ceil(batch * G / 64)).  It depends on neither group sizes nor lengths, so a group's chunking -- and the result --
+// is the same whether a launch is sized from the batch it carries or from the bounds of a captured graph; chunks past a short
+// prefix's last tile are empty CTAs.
+int atom_decode_shared_chunks(int num_groups, int batch, int group, int num_kv_heads, int sm_count) {
+  ATOM_REQUIRE(num_groups > 0 && batch > 0 && group > 0 && num_kv_heads > 0 && sm_count > 0,
+               "decode_shared_chunks: num_groups=%d batch=%d group=%d num_kv_heads=%d sm_count=%d must be positive", num_groups, batch,
+               group, num_kv_heads, sm_count);
+  const long long ctas = (long long)num_groups * ((batch * group + 63) / 64) * num_kv_heads;
+  return (int)((2LL * sm_count + ctas - 1) / ctas);
+}
+
+int atom_batch_decode_shared_gqa_i4(void* o, const void* q, const void* kv_data, const void* kv_param, const void* kv_indptr,
+                                    const void* kv_indices, const void* last_page_offset, int num_layers, int layer_idx,
+                                    int num_q_heads, int num_kv_heads, int page_size, int batch_size, float rope_theta,
+                                    const void* group_indptr, const void* group_members, const void* shared_pages, int num_groups,
+                                    int max_group_size, const void* rope_table, float* workspace, int nchunks, void* stream) {
+  const char* what = "batch_decode_shared_gqa_i4";
+  int rc = kv_check(what, kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx, num_kv_heads, page_size,
+                    batch_size);
+  if (rc) return rc;
+  ATOM_REQUIRE(o && q && group_indptr && group_members && shared_pages && rope_table && workspace, "%s: null pointer argument", what);
+  ATOM_REQUIRE(num_q_heads > 0 && num_q_heads % num_kv_heads == 0,
+               "%s: num_q_heads=%d must be a positive multiple of num_kv_heads=%d", what, num_q_heads, num_kv_heads);
+  ATOM_REQUIRE(rope_theta > 1.f && rope_theta < 1e30f, "%s: rope_theta=%g must be a finite base above 1", what, (double)rope_theta);
+  const int group = num_q_heads / num_kv_heads;
+  if (group != 1 && group != 2 && group != 4 && group != 8)
+    return fail(ATOM_E_UNSUPPORTED, "%s: %d query heads per KV head (num_q_heads=%d, num_kv_heads=%d); supported group sizes are 1, 2, "
+                                    "4 and 8", what, group, num_q_heads, num_kv_heads);
+  ATOM_REQUIRE(page_size % 8 == 0 && page_size <= 64, "%s: page_size=%d must be a multiple of 8, at most 64", what, page_size);
+  ATOM_REQUIRE(aligned16(kv_data) && aligned16(kv_param) && aligned16(rope_table) && aligned16(workspace),
+               "%s: KV pool, rope table and workspace must be 16-byte aligned", what);
+  ATOM_REQUIRE(num_groups > 0 && max_group_size >= 2 && max_group_size <= batch_size && nchunks > 0,
+               "%s: num_groups=%d max_group_size=%d nchunks=%d (batch %d)", what, num_groups, max_group_size, nchunks, batch_size);
+  const atom::KvArgs kv{(uint8_t*)kv_data, (__half2*)kv_param, (const int32_t*)kv_indptr, (const int32_t*)kv_indices,
+                        (const int32_t*)last_page_offset, num_layers, layer_idx, num_kv_heads, page_size, batch_size};
+  const atom::DecPrefix px{(const int32_t*)group_indptr, (const int32_t*)group_members, (const int32_t*)shared_pages, workspace, nchunks};
+  const float log2_theta = log2f(rope_theta);
+  const cudaStream_t st = (cudaStream_t)stream;
+  const int row_blocks = (max_group_size * group + atom::PF_BQ - 1) / atom::PF_BQ;
+  rc = launch_k(what, atom::shared_prefix_attn_kernel, dim3(nchunks, num_kv_heads, num_groups * row_blocks), dim3(atom::PF_THREADS), 0,
+                st, (const __half*)q, kv, px, (const float2*)rope_table, log2_theta, group, row_blocks);
+  if (rc) return rc;
+  if (group == 1) return launch_decode_shared<1>(what, o, q, kv, px, log2_theta, st);
+  if (group == 2) return launch_decode_shared<2>(what, o, q, kv, px, log2_theta, st);
+  if (group == 4) return launch_decode_shared<4>(what, o, q, kv, px, log2_theta, st);
+  return launch_decode_shared<8>(what, o, q, kv, px, log2_theta, st);
 }
 
 int atom_append_kv_i4(void* kv_data, void* kv_param, const void* kv_indptr, const void* kv_indices,

@@ -83,7 +83,32 @@ append_kv_kernel(KvArgs kv, const uint8_t* __restrict__ k, const uint8_t* __rest
 // (m, d, acc[32]) per (head g, quarter c) unit in the (then idle) bracket area; after a cluster barrier every rank combines its
 // share of the G*4 units x 8 float4 chunks over ranks 0..C-1 in rank order (FP32, all DSMEM loads in flight together),
 // normalises and stores; a second cluster barrier keeps every CTA resident while its shared memory is read.
+// Cascade decode (Pre = DecPrefix, see cascade_kernels.cuh): a row of a prefix group starts at its first private page -- the page
+// loop and the query bracket skip the row's shared_pages[b] leading pages -- and before the stripe merge each query head folds
+// in the un-normalised prefix partials (m, d, acc[128]) the prefix pass left for it, in chunk order.  A row outside any group
+// (shared_pages 0) computes exactly what the unsplit kernel computes.
 constexpr int DEC_STAGES = 8;
+constexpr int DEC_PART = 130;                       // floats per prefix partial: m, d, acc[128]
+
+struct DecPrefix {
+  const int32_t* group_indptr;      // [groups + 1]
+  const int32_t* group_members;     // rows of each group
+  const int32_t* shared_pages;      // [B] leading pages row b shares with its group (0: no group)
+  float* part;                      // [B][Hq][nchunks][DEC_PART]
+  int nchunks;
+};
+// the prefix pass's tiling of a shared prefix: `tiles` 64-token tiles, `per` consecutive tiles per chunk (the last chunks may
+// be empty); fixed by the shared page count and the host-chosen chunk count alone
+__host__ __device__ __forceinline__ int dec_prefix_tiles(int shared_pages, int P) { return (shared_pages * P + 63) / 64; }
+__host__ __device__ __forceinline__ int dec_prefix_per(int tiles, int nchunks) { return (tiles + nchunks - 1) / nchunks; }
+// leading pages of row b the prefix pass covers: DecPrefix::shared_pages[b], or none (the plain decode kernel).  The kernel adds it
+// where a page index starts instead of shifting its page range once: that form changed the PTX register numbering, and so the
+// schedule, of the split-KV instantiations, which must stay the code they were.
+template <typename... Pre>
+__device__ __forceinline__ int dec_shared_pages(int b, const Pre&... pre) {
+  if constexpr (sizeof...(Pre) == 1) return (pre.shared_pages[b], ...);
+  else return 0;
+}
 
 // consumer warps of batch_decode_kernel<G, ...>: four page stripes for G = 1 (4 CTAs per SM), G heads x 8/G stripes otherwise
 // (2 CTAs per SM): 16 consumer warps per SM either way
@@ -139,13 +164,16 @@ __device__ __forceinline__ void flush_pv(float (&acc)[32], __half2 (&pv)[16]) {
   }
 }
 
+// Pre: empty, or one DecPrefix (the cascade's suffix pass; unsplit only).
 // kMaxTpl: tokens per lane per page = P / 8 <= kMaxTpl.  kP: page size as a compile-time constant (16 / 32: the sizes the harness
 // uses -- all table strides and the token loops become immediates) or 0 = read it from the arguments.  kSplit: the sequence's
 // pages are spread over a cluster of C CTAs (see above); false is the one-CTA-per-(sequence, KV head) kernel.
-template <int G, int kMaxTpl, int kP, bool kSplit>
+template <int G, int kMaxTpl, int kP, bool kSplit, typename... Pre>
 __global__ void __launch_bounds__(dec_threads(G), G == 1 ? 4 : 2)
-batch_decode_kernel(__half* __restrict__ o, const __half* __restrict__ q, KvArgs kv, float log2_theta, int pdl) {
+batch_decode_kernel(__half* __restrict__ o, const __half* __restrict__ q, KvArgs kv, float log2_theta, int pdl, Pre... pre) {
   static_assert(G == 1 || G == 2 || G == 4 || G == 8, "the consumer warps are split into G heads x S page stripes");
+  constexpr bool kPre = sizeof...(Pre) == 1;
+  static_assert(sizeof...(Pre) <= 1 && !(kPre && kSplit), "the cascade's suffix pass takes one DecPrefix and is unsplit");
   constexpr int kConsumers = dec_consumers(G), kThreads = dec_threads(G), S = kConsumers / G;
   int rank = 0, nranks = 1;                                        // split-KV: this CTA's rank and the cluster size C
   if constexpr (kSplit) { rank = (int)cluster_ctarank(); nranks = (int)cluster_nctarank(); }
@@ -204,7 +232,9 @@ batch_decode_kernel(__half* __restrict__ o, const __half* __restrict__ q, KvArgs
       const int i = 16 * c + ja + 4 * x;
       const float f = exp2f(-(float)i * kFreqStep);
       const float xr = __half2float(qh[i]), xi = __half2float(qh[i + 64]);
-      float sn, cs; sincosf((float)(seq_len - 1 - (rank * S + stripe) * P) * f, &sn, &cs);
+      float sn, cs;
+      if constexpr (kPre) sincosf((float)(seq_len - 1 - (dec_shared_pages(b, pre...) + stripe) * P) * f, &sn, &cs);
+      else sincosf((float)(seq_len - 1 - (rank * S + stripe) * P) * f, &sn, &cs);
       v2[x] = make_float2(xr * cs - xi * sn, xi * cs + xr * sn);
       brk[warp * 64 + i] = v2[x];
     }
@@ -218,7 +248,7 @@ batch_decode_kernel(__half* __restrict__ o, const __half* __restrict__ q, KvArgs
     if (lane == 0) {
       // the CTA's lp-th page (its ring slot order) is global page lp, or split (lp / S) * S * C + rank * S + lp % S
       for (int lp = 0;; ++lp) {
-        const int pg = kSplit ? (lp / S) * S * nranks + rank * S + lp % S : lp;
+        const int pg = kSplit ? (lp / S) * S * nranks + rank * S + lp % S : lp + dec_shared_pages(b, pre...);
         if (pg >= npages) break;
         const int s = lp % DEC_STAGES;
         mbar_wait(&empty[s], ((lp / DEC_STAGES) & 1) ^ 1);
@@ -249,7 +279,7 @@ batch_decode_kernel(__half* __restrict__ o, const __half* __restrict__ q, KvArgs
   uint2* mybrkh = brkh + (warp * 4 + c) * 8;
 
   // global page pg of the stripe is the CTA's lp-th (lp = pg unsplit)
-  for (int pg = rank * S + stripe, lp = stripe; pg < npages; pg += S * nranks, lp += S) {
+  for (int pg = dec_shared_pages(b, pre...) + rank * S + stripe, lp = stripe; pg < npages; pg += S * nranks, lp += S) {
     const int s = lp % DEC_STAGES;
     const int valid = (pg == npages - 1) ? last_valid : P;
     // this page's query bracket as half2 couples (j, j+4); then every lane advances its own couple to the stripe's next
@@ -394,6 +424,20 @@ batch_decode_kernel(__half* __restrict__ o, const __half* __restrict__ q, KvArgs
     float dd = 0.f, out[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) out[i] = 0.f;
+    if constexpr (kPre) {      // the prefix partials of query head hkv*G + warp, chunk by chunk, then the stripes
+      const DecPrefix& px = (pre, ...);
+      const int tiles = dec_prefix_tiles(dec_shared_pages(b, pre...), P), per = dec_prefix_per(tiles, px.nchunks);
+      const int nck = tiles ? (tiles + per - 1) / per : 0;
+      const float* part = px.part + ((size_t)b * Hq + hkv * G + warp) * px.nchunks * DEC_PART;
+      for (int k = 0; k < nck; ++k) mm = fmaxf(mm, part[k * DEC_PART]);
+      for (int k = 0; k < nck; ++k) {
+        const float* src = part + k * DEC_PART;
+        const float sx = exp2f(src[0] - mm);
+        dd = fmaf(src[1], sx, dd);
+#pragma unroll
+        for (int i = 0; i < 32; ++i) out[i] = fmaf(src[2 + 32 * c + i], sx, out[i]);
+      }
+    }
 #pragma unroll
     for (int w = 0; w < S; ++w) {
       const float* src = merge + ((w * G + warp) * 4 + c) * 34;

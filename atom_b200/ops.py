@@ -280,12 +280,20 @@ def batch_decode_i4(q, kv, layer_idx, rope_theta=10000.0, kv_split=0):
     (query head h attends KV head h // G), and `rope_theta` is the RoPE base; one query head per KV head at the default base
     is the reference's operator.  EXTENSION (split-KV): `kv_split` spreads each sequence's pages over a cluster of that many
     CTAs -- 0 = automatic (`decode_kv_split`: only grids of fewer (sequence, KV head) pairs than SMs split), 1 = never,
-    2 / 4 / 8 = forced; other values raise."""
+    2 / 4 / 8 = forced; other values raise.  EXTENSION (shared-prefix decode): when `kv` carries prefix groups (a
+    BatchedKvCacheInt4 over forked sequences) and `decode_cascade` picks it, kv_split=0 runs the cascade: each group's shared
+    pages are attended once per KV head for all its members on tensor cores, then each row's private pages by the decode kernel;
+    rows outside the groups get exactly what kv_split=1 gives them."""
     _req_cuda(q, kv.data, kv.param, kv.indptr, kv.indicies, kv.last_page_offset)
     L, H, P = _kv_dims(kv)
     if q.dim() != 3 or q.size(2) != 128 or kv.indptr.size(0) != q.size(0) + 1 or kv.last_page_offset.size(0) != q.size(0):
         raise RuntimeError("batch_decode_i4: shape mismatch")
     o = torch.empty(q.shape, dtype=q.dtype, device=q.device)
+    groups = getattr(kv, "groups", None)
+    if groups and kv_split == 0:
+        sms = torch.cuda.get_device_properties(q.device).multi_processor_count
+        if decode_cascade(groups, q.size(0), P, H, q.size(1) // H, sms):
+            return _batch_decode_shared(o, q, kv, groups, L, H, P, layer_idx, rope_theta, sms)
     with torch.cuda.device(q.device):
         _lib.check(_lib.lib().atom_batch_decode_split_gqa_i4(o.data_ptr(), q.data_ptr(), kv.data.data_ptr(), kv.param.data_ptr(),
                                                              kv.indptr.data_ptr(), kv.indicies.data_ptr(),
@@ -302,6 +310,53 @@ def decode_kv_split(batch, num_kv_heads, group, device=None):
     c = _lib.lib().atom_decode_kv_split(int(batch), int(num_kv_heads), int(group), int(sms))
     _lib.check(min(c, 0), "decode_kv_split")
     return c
+
+
+# Shared-prefix decode rule, from host-known sizes only (a captured graph replays it with new lengths): the cascade runs when
+#   (1) more than half of the batch's rows are group members,
+#   (2) every group has at least DECODE_CASCADE_MIN_ROWS query rows per KV head (members x G): the prefix pass's MMAs take 64
+#       rows, and fewer leave the tile mostly empty while the pages are streamed at the same cost, and
+#   (3) the token-heads it saves, num_kv_heads x sum over groups of (members - 1) x shared tokens, reach
+#       DECODE_CASCADE_MIN_PER_SM per SM: enough to pay for the prefix pass's launch and the partial merge.
+# (1) because the suffix pass runs unsplit: lone rows (of unknown length) keep the time a batch of them takes, and a small
+# grid loses the split-KV the plain kernel would get.  Thresholds measured on an H100 with tools/shared_prefix_bench.py
+# (DESIGN.md section 6).
+DECODE_CASCADE_MIN_ROWS = 16
+DECODE_CASCADE_MIN_PER_SM = 256
+
+
+def decode_cascade(groups, batch, page_size, num_kv_heads, group, sm_count):
+    """Whether `batch_decode_i4(..., kv_split=0)` runs the cascade for a batch of `batch` rows with these prefix groups ((rows,
+    shared pages) pairs, as BatchedKvCacheInt4.groups holds them), `num_kv_heads` KV heads, `group` query heads per KV head, on
+    a device of `sm_count` SMs."""
+    members = sum(len(rows) for rows, _ in groups)
+    saved = num_kv_heads * sum((len(rows) - 1) * n * page_size for rows, n in groups)
+    return bool(groups) and 2 * members > batch and min(len(rows) for rows, _ in groups) * group >= DECODE_CASCADE_MIN_ROWS \
+        and saved >= DECODE_CASCADE_MIN_PER_SM * sm_count
+
+
+def _batch_decode_shared(o, q, kv, groups, L, H, P, layer_idx, rope_theta, sms):
+    """The cascade: prefix pass over each group's shared pages, then the decode kernel over the private pages."""
+    b, hq = q.size(0), q.size(1)
+    # a table in static buffers (a CUDA-graph replay) states bounds that hold for every step it will carry: (members of a group,
+    # shared pages) at most; the launch is sized from them, so the replay stays valid as members and lengths change
+    bounds = getattr(kv, "group_bounds", None)
+    if bounds is not None:
+        max_size, max_shared = int(bounds[0]), int(bounds[1]) * P
+    else:
+        max_size, max_shared = max(len(rows) for rows, _ in groups), max(n for _, n in groups) * P
+    lib = _lib.lib()
+    nchunks = lib.atom_decode_shared_chunks(len(groups), b, hq // H, H, sms)
+    _lib.check(min(nchunks, 0), "decode_shared_chunks")
+    ws = torch.empty((b, hq, nchunks, 130), dtype=torch.float32, device=q.device)
+    table = rope_table(max_shared, q.device, rope_theta)
+    with torch.cuda.device(q.device):
+        _lib.check(lib.atom_batch_decode_shared_gqa_i4(
+            o.data_ptr(), q.data_ptr(), kv.data.data_ptr(), kv.param.data_ptr(), kv.indptr.data_ptr(), kv.indicies.data_ptr(),
+            kv.last_page_offset.data_ptr(), L, layer_idx, hq, H, P, b, float(rope_theta), kv.group_indptr.data_ptr(),
+            kv.group_members.data_ptr(), kv.shared_pages.data_ptr(), len(groups), max_size, table.data_ptr(), ws.data_ptr(), nchunks,
+            _stream(q)), "batch_decode_i4 (shared prefix)")
+    return o
 
 
 _rope_tables = {}

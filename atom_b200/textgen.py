@@ -23,7 +23,7 @@ import numpy as np
 import torch
 
 from .cat_tensor import BatchLenInfo
-from .kvcache import BatchedKvCacheInt4, KvCacheInt4, KvPoolInt4
+from .kvcache import BatchedKvCacheInt4, KvCacheInt4, KvPoolInt4, prefix_groups
 
 SEED = 0xABCDABCD987
 
@@ -80,6 +80,7 @@ MODEL_CFGS = {
 class TextGenConfig:
     batch_size: int
     prefill_chunk: Optional[int] = None     # at most this many prompt tokens per step (chunked prefill); None = whole prompts
+    shared_prefix: int = 0                  # tokens of one system prompt before every request's prompt, prefilled once and forked
 
 
 @dataclasses.dataclass
@@ -90,6 +91,7 @@ class TextGenBenchResult:
     steps: int = 0
     tokens: Optional[List[List[int]]] = None
     graphed_steps: int = 0
+    peak_pages: int = 0                     # most KV pages in use after any step's admission
 
 
 @dataclasses.dataclass
@@ -128,12 +130,20 @@ class TextGenScheduler:
     (chunked prefill): a step carries at most N prompt tokens in all -- first the next chunks of the requests that are partly
     prefilled, FCFS, then the first chunks of newly admitted ones -- so that a long prompt no longer stalls every running
     sequence's decode for one long step.  A chunk is the tail of its sequence's cached tokens; the model's prefill attention then
-    also reads the chunks before it from the cache.  A request gets its first token from the step that completes its prompt."""
+    also reads the chunks before it from the cache.  A request gets its first token from the step that completes its prompt.
+
+    shared_prefix=N (> 0): every request's prompt is preceded by one common N-token system prompt, drawn from a seeded stream of
+    its own (the request set and the requests' prompts are those of N = 0).  It is prefilled once, first, as a root sequence that
+    produces no token (chunked under prefill_chunk like any prompt); each request admitted after that is `root.fork()` followed
+    by its own prompt as a continuation, and admission counts only the pages the fork takes.  The root is released when the last
+    request finishes.  Decode batches of forked requests carry prefix groups (kvcache.BatchedKvCacheInt4)."""
 
     def __init__(self, rs: RequestSet, batch_size: int, pool: KvPoolInt4, device, vocab_size: int = 32000,
-                 prefill_chunk: Optional[int] = None):
+                 prefill_chunk: Optional[int] = None, shared_prefix: int = 0):
         if prefill_chunk is not None and int(prefill_chunk) < 1:
             raise ValueError("prefill_chunk must be a positive number of tokens (or None)")
+        if int(shared_prefix) < 0:
+            raise ValueError("shared_prefix must be a non-negative number of tokens")
         self.rs, self.batch_size, self.pool, self.device = rs, batch_size, pool, device
         self.vocab_size = vocab_size
         self.prefill_chunk = None if prefill_chunk is None else int(prefill_chunk)
@@ -145,6 +155,12 @@ class TextGenScheduler:
         self._admitted = False
         self._blen = None
         self._rng = np.random.Generator(np.random.PCG64(seed=SEED))
+        self.shared_prefix = int(shared_prefix)
+        self._root: Optional[_Prefill] = None          # the system prompt's sequence (req_idx -1), prefilled before any request
+        if self.shared_prefix:
+            system = np.random.Generator(np.random.PCG64(seed=SEED + 1)).integers(0, vocab_size, self.shared_prefix).tolist()
+            self._root = _Prefill(-1, system, KvCacheInt4(pool, 0))
+            self._prefilling.append(self._root)
 
     @property
     def finished(self) -> bool:
@@ -156,12 +172,16 @@ class TextGenScheduler:
         return sum(n for _, _, n in self._new)
 
     def _pages_needed(self, prompt_len: int) -> int:
-        # the prompt's pages plus one spare: the first generated token may open a new page
-        return (prompt_len + self.pool.block_len - 1) // self.pool.block_len + 1
+        # the prompt's pages plus one spare: the first generated token may open a new page.  Behind a shared prefix of N tokens
+        # a fork takes the pages from N // P on: a copy of the partly filled page, if any, and the pages its prompt adds
+        n, bl = self.shared_prefix, self.pool.block_len
+        return (n + prompt_len + bl - 1) // bl - n // bl + 1
 
     def _outstanding(self, p: _Prefill) -> int:
-        # pages a request being prefilled will still take: the rest of its prompt and the spare
-        return self._pages_needed(len(p.prompt)) - len(p.kvcache.indicies)
+        # pages a request being prefilled will still take: the rest of its prompt and the spare (the root: the rest of it)
+        if p.req_idx < 0:
+            return -(-len(p.prompt) // self.pool.block_len) - len(p.kvcache.indicies)
+        return self._pages_needed(len(p.prompt)) - (len(p.kvcache.indicies) - self.shared_prefix // self.pool.block_len)
 
     def admit(self) -> int:
         """Continue the partly prefilled requests, then admit waiting ones (FCFS) while the batch has room, the step has prompt
@@ -180,7 +200,8 @@ class TextGenScheduler:
             reserve -= len(p.kvcache.indicies) - before
             self._new.append((p, p.done, n))
             budget = None if budget is None else budget - n
-        while len(self.workset) + len(self._prefilling) < self.batch_size and self.next_req_idx < len(self.rs) and \
+        root_done = self._root is None or self._root.done == len(self._root.prompt)
+        while root_done and len(self.workset) + len(self._prefilling) < self.batch_size and self.next_req_idx < len(self.rs) and \
                 (budget is None or budget > 0):
             plen = int(self.rs.prompt_lens[self.next_req_idx])
             if self.pool.num_free_blocks - reserve < self._pages_needed(plen):
@@ -191,7 +212,12 @@ class TextGenScheduler:
             self.next_req_idx += 1
             prompt = self._rng.integers(0, self.vocab_size, plen).tolist()
             n = plen if budget is None else min(plen, budget)
-            p = _Prefill(idx, prompt, KvCacheInt4(self.pool, n))
+            if self._root is None:
+                kv = KvCacheInt4(self.pool, n)
+            else:
+                kv = self._root.kvcache.fork()
+                kv.acquire(n)
+            p = _Prefill(idx, prompt, kv)
             self._prefilling.append(p)
             self._new.append((p, 0, n))
             reserve += self._outstanding(p)
@@ -220,13 +246,13 @@ class TextGenScheduler:
         rows = [] if blen.indptr is None else (blen.indptr[1:] - 1).tolist()
         chunks = getattr(self, "_new", None)        # None: a bare step description, whole prompts only
         if chunks is not None:
-            rows = [r for r, (p, s, n) in zip(rows, chunks) if s + n == len(p.prompt)]
+            rows = [r for r, (p, s, n) in zip(rows, chunks) if s + n == len(p.prompt) and p.req_idx >= 0]
         return rows + list(range(blen.doff, blen.doff + blen.decode))
 
     def commit(self, next_tokens, t1: float, t2: float) -> int:
         """next_tokens: one id per row of last_token_rows().  Returns the number of tokens this step processed."""
         completes = [s + n == len(p.prompt) for p, s, n in self._new]
-        n_first = sum(completes)
+        n_first = sum(c for (p, _, _), c in zip(self._new, completes) if p.req_idx >= 0)
         assert len(next_tokens) == n_first + len(self.workset)
         processed = sum(n for _, _, n in self._new) + len(self.workset)
         new_workset: List[RequestContext] = []
@@ -238,6 +264,8 @@ class TextGenScheduler:
             if not c:
                 continue
             self._prefilling.remove(p)
+            if p.req_idx < 0:                               # the system prompt: cached, no token
+                continue
             req = RequestContext(p.req_idx, p.kvcache, [int(next_tokens[b])], encode_latency=t2 - p.start_at, decode_start_at=p.start_at)
             b += 1
             self._finish_or_continue(req, t2, new_workset)
@@ -252,6 +280,8 @@ class TextGenScheduler:
             req.decode_latency = t2 - req.decode_start_at
             req.kvcache.release()
             self.done.append(req)
+            if self._root is not None and self.finished:
+                self._root.kvcache.release()
         else:
             req.kvcache.acquire_one()
             new_workset.append(req)
@@ -275,7 +305,7 @@ class _StaticKv:
 
 
 class DecodeGraphRunner:
-    """Decode-only steps replayed from CUDA graphs, one graph per batch size.
+    """Decode-only steps replayed from CUDA graphs, one graph per (batch size, number of prefix groups).
 
     In steady state almost every step of the serving loop is decode-only (outputs are ~50x longer than prompts in the
     reference's request set) and a 32-layer step is ~500 kernel launches: launch-bound from Python.  All per-step state of
@@ -284,6 +314,10 @@ class DecodeGraphRunner:
     with a single pinned H2D copy, after which the captured step (embedding, all layers: fused norm+quantise, INT4 GEMMs,
     KV append, INT4 decode attention, lm_head, argmax) is replayed.  The kernels read the page table from device memory and
     their grids depend only on B, so the graph stays valid as sequences grow and change pages.
+    A batch of forked sequences (shared_prefix) has prefix groups (kvcache.prefix_groups); with G > 0 of them the buffer goes on
+    with  [group_indptr(G+1) | group_members(B) | shared_pages(B)]  and the graph's shared-prefix decode is sized from bounds
+    that hold under the key -- at most B members in a group, at most max_pages shared pages -- so it stays valid as members join
+    or leave a group and as lengths grow.  Without groups the buffer is exactly the layout above.
 
     capture=False runs the same buffers through the model eagerly (the CPU tests use it; it is also the warm-up path)."""
 
@@ -292,22 +326,28 @@ class DecodeGraphRunner:
         self.max_pages, self.capture = max_pages_per_seq, capture
         self._entries = {}
 
-    def _layout(self, b):
+    def _layout(self, b, ng=0):
         o_ids, o_indptr, o_last, o_ind = 0, b, 2 * b + 1, 3 * b + 1
-        return o_ids, o_indptr, o_last, o_ind, 3 * b + 1 + b * self.max_pages
+        o_grp = 3 * b + 1 + b * self.max_pages
+        return o_ids, o_indptr, o_last, o_ind, o_grp, o_grp + (ng + 1 + 2 * b if ng else 0)
 
-    def _entry(self, b):
-        e = self._entries.get(b)
+    def _entry(self, b, ng):
+        e = self._entries.get((b, ng))
         if e is None:
-            o_ids, o_indptr, o_last, o_ind, total = self._layout(b)
+            o_ids, o_indptr, o_last, o_ind, o_grp, total = self._layout(b, ng)
             host = torch.zeros(total, dtype=torch.int32)
             if self.device.type == "cuda":
                 host = host.pin_memory()
             dev = torch.zeros(total, dtype=torch.int32, device=self.device)
             kv = _StaticKv(self.pool, dev[o_indptr:o_indptr + b + 1], dev[o_ind:o_ind + b * self.max_pages], dev[o_last:o_last + b])
+            if ng:
+                kv.group_indptr = dev[o_grp:o_grp + ng + 1]
+                kv.group_members = dev[o_grp + ng + 1:o_grp + ng + 1 + b]
+                kv.shared_pages = dev[o_grp + ng + 1 + b:o_grp + ng + 1 + 2 * b]
+                kv.group_bounds = (b, self.max_pages)
             e = {"host": host, "dev": dev, "ids": dev[o_ids:o_ids + b], "kv": kv, "blen": BatchLenInfo([], b, self.device),
                  "graph": None, "out": None}
-            self._entries[b] = e
+            self._entries[(b, ng)] = e
         return e
 
     def _step(self, e):
@@ -316,8 +356,10 @@ class DecodeGraphRunner:
 
     def run(self, last_tokens: List[int], kvs: List[KvCacheInt4]) -> np.ndarray:
         b = len(kvs)
-        e = self._entry(b)
-        o_ids, o_indptr, o_last, o_ind, _ = self._layout(b)
+        groups = prefix_groups(kvs)
+        ng = len(groups)
+        e = self._entry(b, ng)
+        o_ids, o_indptr, o_last, o_ind, o_grp, _ = self._layout(b, ng)
         h = e["host"].numpy()
         h[o_ids:o_ids + b] = last_tokens
         n = 0
@@ -330,6 +372,15 @@ class DecodeGraphRunner:
             n += len(pages)
             h[o_indptr + i + 1] = n
             h[o_last + i] = (c.seqlen - 1) % self.pool.block_len + 1
+        if ng:
+            members = [r for rows, _ in groups for r in rows]
+            h[o_grp:o_grp + ng + 1] = np.cumsum([0] + [len(rows) for rows, _ in groups])
+            h[o_grp + ng + 1:o_grp + ng + 1 + b] = members + [0] * (b - len(members))
+            shared = h[o_grp + ng + 1 + b:o_grp + ng + 1 + 2 * b]
+            shared[:] = 0
+            for rows, n in groups:
+                shared[rows] = n
+            e["kv"].groups = groups              # the host view: it decides, when the step is captured, which decode runs
         e["dev"].copy_(e["host"], non_blocking=True)
         if not self.capture:
             return self._step(e).cpu().numpy()
@@ -368,12 +419,14 @@ def run_textgen(model: Callable, rs: RequestSet, cfg: TextGenConfig, pool: KvPoo
     """Drive `model(input_ids, blen, prefill_kv, decode_kv) -> (logits, hidden)` through the whole request set.
     Latencies are wall-clock around the step *including* the device->host read of the next tokens (which synchronises),
     as in the reference.  With a `decode_runner`, steps that carry no prompt tokens are replayed from its CUDA graphs.
-    cfg.prefill_chunk: see TextGenScheduler."""
-    sched = TextGenScheduler(rs, cfg.batch_size, pool, device, vocab_size=_vocab_size(model), prefill_chunk=cfg.prefill_chunk)
-    steps = graphed = 0
+    cfg.prefill_chunk, cfg.shared_prefix: see TextGenScheduler."""
+    sched = TextGenScheduler(rs, cfg.batch_size, pool, device, vocab_size=_vocab_size(model), prefill_chunk=cfg.prefill_chunk,
+                             shared_prefix=cfg.shared_prefix)
+    steps = graphed = peak = 0
     t_start = time.perf_counter()
     while not sched.finished:
         sched.admit()
+        peak = max(peak, pool.capacity - pool.num_free_blocks)
         t1 = time.perf_counter()
         if decode_runner is not None and sched.prompt_tokens == 0:
             next_tokens = decode_runner.run([int(r.output[-1]) for r in sched.workset], [r.kvcache for r in sched.workset])
@@ -393,11 +446,13 @@ def run_textgen(model: Callable, rs: RequestSet, cfg: TextGenConfig, pool: KvPoo
             progress(n)
     res = sched.result(time.perf_counter() - t_start, steps, keep_tokens)
     res.graphed_steps = graphed
+    res.peak_pages = peak
     return res
 
 
 def report(rs: RequestSet, cfg: TextGenConfig, res: TextGenBenchResult) -> dict:
-    """The figures bench_textgen.py:509-528 prints, as a dict (throughput = (prompt + new tokens) / duration)."""
+    """The figures bench_textgen.py:509-528 prints, as a dict (throughput = (prompt + new tokens) / duration; the shared system
+    prompt's tokens are not counted), plus the peak of KV pages in use."""
     per_prompt_tok = res.encode_latency / rs.prompt_lens
     per_new_tok = res.decode_latency / rs.output_lens
     total = int(rs.prompt_lens.sum()) + int(rs.output_lens.sum())
@@ -407,5 +462,6 @@ def report(rs: RequestSet, cfg: TextGenConfig, res: TextGenBenchResult) -> dict:
         "encode_latency_ms_per_token": [float(per_prompt_tok.mean() * 1e3), float(per_prompt_tok.std() * 1e3)],
         "decode_latency_ms_per_token": [float(per_new_tok.mean() * 1e3), float(per_new_tok.std() * 1e3)],
         "total_prompt_tokens": int(rs.prompt_lens.sum()), "total_new_tokens": int(rs.output_lens.sum()),
-        "duration_s": res.duration, "throughput_tokens_per_s": total / res.duration,
+        "duration_s": res.duration, "throughput_tokens_per_s": total / res.duration, "peak_kv_pages_in_use": res.peak_pages,
+        "shared_prefix": cfg.shared_prefix,
     }

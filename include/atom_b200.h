@@ -179,6 +179,30 @@ ATOM_API int atom_batch_decode_split_gqa_i4(void* o, const void* q, const void* 
  * validated.  Returns C, or ATOM_E_INVALID for non-positive sizes or another group. */
 ATOM_API int atom_decode_kv_split(int batch, int num_kv_heads, int group, int sm_count);
 
+/* EXTENSION (shared-prefix decode): atom_batch_decode_gqa_i4 for a batch whose rows form prefix groups -- rows forked from one
+ * sequence that begin on the same (full) pages.  Two launches on `stream`:
+ *   prefix pass: each group's shared pages are streamed once per KV head, dequantised and rotated into FP16 tiles and attended by
+ *     all members x G query rows with tensor-core MMAs (FP32 online softmax); the un-normalised (m, d, acc[128]) of every row and
+ *     chunk goes to `workspace`;
+ *   suffix pass: the decode kernel over each row's private pages, merging the row's prefix partials in chunk order first.
+ * Rows outside every group (shared_pages 0) are computed exactly as atom_batch_decode_split_gqa_i4 with kv_split = 1 computes them.
+ *   group_indptr i32 [num_groups+1], group_members i32: the rows of group i are group_members[group_indptr[i] .. group_indptr[i+1]]
+ *   (at most max_group_size of them, at least two); shared_pages i32 [B]: leading pages row b shares with its group, equal for
+ *   every member, 0 outside groups; rope_table f32 [>= longest shared prefix, 64, 2] as for atom_prefill_attention_i4 with base
+ *   rope_theta; workspace f32 [B, num_q_heads, nchunks, 130]; nchunks from atom_decode_shared_chunks.
+ * Everything else as atom_batch_decode_gqa_i4.  Deterministic: the result depends on nchunks, never on where the pages sit. */
+ATOM_API int atom_batch_decode_shared_gqa_i4(void* o, const void* q, const void* kv_data, const void* kv_param, const void* kv_indptr,
+                                             const void* kv_indices, const void* last_page_offset, int num_layers, int layer_idx,
+                                             int num_q_heads, int num_kv_heads, int page_size, int batch_size, float rope_theta,
+                                             const void* group_indptr, const void* group_members, const void* shared_pages,
+                                             int num_groups, int max_group_size, const void* rope_table, float* workspace, int nchunks,
+                                             void* stream);
+
+/* The prefix-pass chunk count of atom_batch_decode_shared_gqa_i4: the fewest chunks with which num_groups x ceil(batch * group / 64)
+ * x num_kv_heads x chunks reaches 2 * sm_count CTAs (group: query heads per KV head; a group's prefix is cut into that many runs
+ * of whole 64-token tiles, short prefixes leave some empty).  Returns the count, or ATOM_E_INVALID for non-positive sizes. */
+ATOM_API int atom_decode_shared_chunks(int num_groups, int batch, int group, int num_kv_heads, int sm_count);
+
 /* EXTENSION (SURVEY.md 8 f3): the prefill attention the reference leaves as a placeholder
  * (punica/models/llama.py:171-190, SDPA over torch.randn K/V): causal attention of every prompt over its own just-quantised
  * K/V -- the o4 outputs of the k/v projections, x = nibble * scale - zero (quantization.cuh:76) -- with RoPE(theta 1e4) on q

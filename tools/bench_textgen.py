@@ -49,6 +49,8 @@ def main():
     ap.add_argument("--no-cuda-graphs", action="store_true", help="run decode-only steps eagerly too (the reference's way)")
     ap.add_argument("--prefill-chunk", type=int, default=None,
                     help="chunked prefill: at most this many prompt tokens per step (default: whole prompts)")
+    ap.add_argument("--shared-prefix", type=int, default=0, metavar="N",
+                    help="precede every prompt with one common N-token system prompt, prefilled once and shared by forking")
     ap.add_argument("--warmup-batches", type=int, default=1,
                     help="untimed request batches served first (first-use costs: lazy kernel loading, attribute calls, graph "
                          "capture); 0 = time the cold process like the reference's script")
@@ -62,11 +64,13 @@ def main():
     torch.manual_seed(tg.SEED)
     model = build_model(mc, layers)
     rs = tg.generate_request_set(args.batch_size * args.num_batches, args.maxlen)
-    cfg = tg.TextGenConfig(args.batch_size, prefill_chunk=args.prefill_chunk)
+    cfg = tg.TextGenConfig(args.batch_size, prefill_chunk=args.prefill_chunk, shared_prefix=args.shared_prefix)
+    shared_pages = -(-args.shared_prefix // args.block_len)           # the system prompt's pages, held once
     pool = KvPoolInt4(layers, mc.kv_heads, mc.hidden_size // mc.num_heads,     # the cache holds KV heads (grouped-query: fewer)
-                      tg.pool_capacity(args.batch_size, args.maxlen, args.block_len), args.block_len, device)
+                      tg.pool_capacity(args.batch_size, args.maxlen, args.block_len) + shared_pages + args.batch_size * (shared_pages > 0),
+                      args.block_len, device)
     runner = None if args.no_cuda_graphs else tg.DecodeGraphRunner(
-        model, pool, device, max_pages_per_seq=(args.maxlen + args.block_len - 1) // args.block_len + 1)
+        model, pool, device, max_pages_per_seq=(args.maxlen + args.block_len - 1) // args.block_len + 1 + shared_pages)
     if args.warmup_batches > 0:
         wrs = tg.generate_request_set(args.batch_size * args.warmup_batches, args.maxlen)
         tg.run_textgen(model, wrs, cfg, pool, device, sync=torch.cuda.synchronize, decode_runner=runner)
@@ -84,6 +88,7 @@ def main():
     print("total new tokens:", rep["total_new_tokens"])
     print("duration:", f"{rep['duration_s']:.3f}s")
     print("throughput ((prompt+new)/duration):", f"{rep['throughput_tokens_per_s']:.3f} token/s")
+    print("peak KV pages in use:", rep["peak_kv_pages_in_use"], f"of {pool.capacity}")
     rep.update({"model": args.model, "layers": layers, "maxlen": args.maxlen, "kv_pool_pages": pool.buf.size(0),
                 "kv_pool_GB": round((pool.buf.numel() + 2 * pool.param.numel()) / 1e9, 2)})
     print(json.dumps(rep))
