@@ -48,6 +48,7 @@ _SIGNATURES = {
     "atom_gemm_i4_gateup_act_grouped": (_I, [_P] * 13 + [_I, _I, _I64, _I64, _I64, _I64, _P]),
     "atom_gemm_i4_o16_grouped": (_I, [_P] * 10 + [_I, _I, _I64, _I64, _I64, _I64, _P]),
     "atom_moe_combine_f16": (_I, [_P] * 4 + [_I, _I, _I, _P, _P]),
+    "atom_sample_f16": (_I, [_P, _I64, _I, _I] + [_P] * 7),
 }
 
 _lib = None

@@ -27,6 +27,7 @@
 #include "comm_kernels.cuh"
 #include "quant_kernels.cuh"
 #include "moe_kernels.cuh"
+#include "sample_kernels.cuh"
 
 namespace {
 
@@ -993,6 +994,42 @@ int atom_moe_combine_f16(const void* y, const void* topk_ids, const void* topk_w
   return launch_k("moe_combine_f16", atom::moe_combine_kernel, dim3(seq_len), dim3(atom::COMBINE_THREADS), 0, (cudaStream_t)stream,
                   (const __half*)y, (const int32_t*)topk_ids, (const __half*)topk_weights, (const int32_t*)dest_row, top_k, hidden_dim,
                   (__half*)out);
+}
+
+int atom_sample_f16(const void* logits, int64_t ld, int batch, int vocab, const void* temperature, const void* top_k, const void* top_p,
+                    const void* key, const void* counter, void* out, void* stream) {
+  ATOM_REQUIRE(logits && temperature && top_k && top_p && key && counter && out, "sample_f16: null pointer argument");
+  ATOM_REQUIRE(batch > 0 && vocab > 0 && vocab <= atom::SAMPLE_MAX_CLUSTER * atom::SAMPLE_SLICE_MAX,
+               "sample_f16: batch=%d must be positive, vocab=%d in [1, %d]", batch, vocab,
+               atom::SAMPLE_MAX_CLUSTER * atom::SAMPLE_SLICE_MAX);
+  ATOM_REQUIRE(ld >= vocab || batch == 1, "sample_f16: ld=%lld must be >= vocab=%d", (long long)ld, vocab);
+  ATOM_REQUIRE((reinterpret_cast<uintptr_t>(logits) & 1) == 0 && (reinterpret_cast<uintptr_t>(key) & 7) == 0 &&
+               (reinterpret_cast<uintptr_t>(counter) & 7) == 0 && (reinterpret_cast<uintptr_t>(temperature) & 3) == 0 &&
+               (reinterpret_cast<uintptr_t>(top_k) & 3) == 0 && (reinterpret_cast<uintptr_t>(top_p) & 3) == 0 &&
+               (reinterpret_cast<uintptr_t>(out) & 3) == 0, "sample_f16: misaligned pointer (logits 2, key / counter 8, the rest 4 bytes)");
+  ATOM_REQUIRE((long long)batch * atom::SAMPLE_MAX_CLUSTER < (1ll << 31), "sample_f16: batch=%d too large", batch);
+  const int C = atom::sample_cluster(vocab), slice = atom::sample_slice(vocab);
+  const size_t smem = atom::SAMPLE_SMEM_FIXED + (size_t)slice * sizeof(uint16_t);
+  int rc = ensure_dynamic_smem(atom::sample_kernel, (int)(atom::SAMPLE_SMEM_FIXED + atom::SAMPLE_SLICE_MAX * sizeof(uint16_t)), "sample_f16");
+  if (rc) return rc;
+  atom::SampleArgs args{(const __half*)logits, (long long)ld, vocab, slice, (const float*)temperature, (const int32_t*)top_k,
+                        (const float*)top_p, (const unsigned long long*)key, (const unsigned long long*)counter, (int32_t*)out};
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3((unsigned)(C * batch)); cfg.blockDim = dim3(atom::SAMPLE_THREADS); cfg.dynamicSmemBytes = smem;
+  cfg.stream = (cudaStream_t)stream;
+  cudaLaunchAttribute attr[2];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = C; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr; cfg.numAttrs = 1;
+  const int pdl = pdl_enabled() ? 1 : 0;
+  if (pdl) {
+    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[1].val.programmaticStreamSerializationAllowed = 1;
+    cfg.numAttrs = 2;
+  }
+  cudaError_t e = cudaLaunchKernelEx(&cfg, atom::sample_kernel, args, pdl);
+  if (e != cudaSuccess) return fail(ATOM_E_CUDA, "sample_f16 launch (cluster %d): %s", C, cudaGetErrorString(e));
+  return check_launch("sample_f16");
 }
 
 }  // extern "C"

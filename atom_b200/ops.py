@@ -611,3 +611,65 @@ def moe_combine_f16(y, topk_ids, topk_weights, dest_row):
         _lib.check(_lib.lib().atom_moe_combine_f16(y.data_ptr(), topk_ids.data_ptr(), topk_weights.data_ptr(), dest_row.data_ptr(), t,
                                                    y.size(1), k, out.data_ptr(), _stream(y)), "moe_combine_f16")
     return out
+
+
+def _sample_param(name, v, b, dtype, device, check):
+    """One per-row parameter of sample_tokens: a CUDA tensor of `b` elements (values read on the device), or a host sequence /
+    scalar that is checked here and copied."""
+    if isinstance(v, torch.Tensor):
+        _req_cuda(v)
+        want = torch.int64 if dtype in (torch.int64, torch.uint64) else dtype
+        if v.dtype != want and not (want == torch.int64 and v.dtype == torch.uint64):
+            raise RuntimeError(f"atom_b200.ops.sample_tokens: `{name}` must be {want}, got {v.dtype}")
+        shape = (b, 2) if name == "keys" else (b,)
+        if tuple(v.shape) != shape:
+            raise RuntimeError(f"atom_b200.ops.sample_tokens: `{name}` must have shape {shape}, got {tuple(v.shape)}")
+        if v.device != device:
+            raise RuntimeError(f"atom_b200.ops.sample_tokens: `{name}` must be on {device}")
+        return v
+    import numpy as np
+    if dtype in (torch.int64, torch.uint64):                    # 64-bit words: any integer in [0, 2^64)
+        ints = np.array(v, dtype=object).reshape(-1)
+        if not all(isinstance(x, (int, np.integer)) and 0 <= int(x) < 1 << 64 for x in ints):
+            raise RuntimeError(f"atom_b200.ops.sample_tokens: `{name}` must hold integers in [0, 2^64)")
+        a = np.array([int(x) for x in ints], dtype=np.uint64).view(np.int64)
+        shape = (b, 2) if name == "keys" else (b,)
+        if a.size != int(np.prod(shape)):
+            raise RuntimeError(f"atom_b200.ops.sample_tokens: `{name}` must have {shape} entries, got {a.size}")
+        return torch.from_numpy(a.reshape(shape)).to(device)
+    a = np.broadcast_to(np.asarray(v, dtype=np.float64), (b,)) if np.ndim(v) == 0 else np.asarray(v, dtype=np.float64)
+    if a.shape != (b,):
+        raise RuntimeError(f"atom_b200.ops.sample_tokens: `{name}` must have {b} entries, got shape {a.shape}")
+    bad = check(a)
+    if bad.any():
+        raise RuntimeError(f"atom_b200.ops.sample_tokens: `{name}` out of range at row {int(np.argmax(bad))}: {a[np.argmax(bad)]!r}")
+    return torch.from_numpy(np.ascontiguousarray(a)).to(dtype).to(device)
+
+
+def sample_tokens(logits, temperature, top_k, top_p, keys, counters):
+    """EXTENSION: one token id per row of f16 logits [B, V] (rows may have any pitch), int32 [B].  Per row: temperature
+    (0 = argmax), top_k (0 = off, on the raw logits), top_p (1 = off), Philox key (key0, key1) and counter; the semantics are
+    atom_sample_f16's (include/atom_b200.h, DESIGN section 5.6).  Each parameter is a CUDA tensor with one entry per row (keys:
+    [B, 2]; keys and counters int64 holding the uint64 bit patterns) whose values are read on the device -- so a captured graph
+    replays with new ones -- or a host sequence or scalar, which is validated (T finite and >= 0, top_k >= 0, top_p in (0, 1])
+    and copied.  Rows with NaN / +inf logits, only -inf logits, or out-of-range device parameters give -1."""
+    if not (isinstance(logits, torch.Tensor) and logits.is_cuda):
+        raise RuntimeError("atom_b200.ops: all tensors must live on a CUDA device (there is no CPU path)")
+    if logits.dtype != torch.float16 or logits.dim() != 2 or logits.stride(1) != 1:
+        raise RuntimeError("atom_b200.ops.sample_tokens: logits must be float16 [B, V] with unit stride along V")
+    b, v = logits.shape
+    dev = logits.device
+    import numpy as np
+    t = _sample_param("temperature", temperature, b, torch.float32, dev, lambda a: ~np.isfinite(a) | (a < 0))
+    k = _sample_param("top_k", top_k, b, torch.int32, dev, lambda a: (a < 0) | (a != np.floor(a)) | (a >= 1 << 31))
+    p = _sample_param("top_p", top_p, b, torch.float32, dev, lambda a: ~((a > 0) & (a <= 1)))
+    key = _sample_param("keys", keys, b, torch.int64, dev, None)
+    ctr = _sample_param("counters", counters, b, torch.int64, dev, None)
+    out = torch.empty((b,), dtype=torch.int32, device=dev)
+    if b == 0:
+        return out
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().atom_sample_f16(logits.data_ptr(), logits.stride(0) if b > 1 else v, b, v, t.data_ptr(), k.data_ptr(),
+                                              p.data_ptr(), key.data_ptr(), ctr.data_ptr(), out.data_ptr(), _stream(logits)),
+                   "sample_tokens")
+    return out

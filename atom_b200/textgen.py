@@ -77,10 +77,28 @@ MODEL_CFGS = {
 
 
 @dataclasses.dataclass
+class SamplingParams:
+    """Sampled decoding (ops.sample_tokens): every request draws its tokens at this temperature (0 = greedy), top_k (0 = off)
+    and top_p (1 = off).  Request r's Philox key is (seed, r) and the counter of a token is the number of tokens r generated
+    before it, so its tokens depend on its own logits only -- not on batching, chunking, shared prefixes or graphs."""
+    temperature: float
+    top_k: int = 0
+    top_p: float = 1.0
+    seed: int = 0
+
+    def __post_init__(self):
+        if not (np.isfinite(self.temperature) and self.temperature >= 0):
+            raise ValueError(f"temperature must be finite and >= 0, got {self.temperature}")
+        if int(self.top_k) < 0 or not (0 < self.top_p <= 1) or not (0 <= int(self.seed) < 1 << 64):
+            raise ValueError(f"need top_k >= 0, top_p in (0, 1] and a seed in [0, 2^64): {self}")
+
+
+@dataclasses.dataclass
 class TextGenConfig:
     batch_size: int
     prefill_chunk: Optional[int] = None     # at most this many prompt tokens per step (chunked prefill); None = whole prompts
     shared_prefix: int = 0                  # tokens of one system prompt before every request's prompt, prefilled once and forked
+    sampling: Optional[SamplingParams] = None   # None: greedy (argmax)
 
 
 @dataclasses.dataclass
@@ -249,6 +267,13 @@ class TextGenScheduler:
             rows = [r for r, (p, s, n) in zip(rows, chunks) if s + n == len(p.prompt) and p.req_idx >= 0]
         return rows + list(range(blen.doff, blen.doff + blen.decode))
 
+    def sample_slots(self) -> List[tuple]:
+        """(request index, counter) of every row of last_token_rows(), in its order: the counter is the number of tokens the
+        request has generated so far (0 for the row that completes its prompt)."""
+        chunks = getattr(self, "_new", None) or []
+        first = [(p.req_idx, 0) for p, s, n in chunks if s + n == len(p.prompt) and p.req_idx >= 0]
+        return first + [(r.req_idx, len(r.output)) for r in self.workset]
+
     def commit(self, next_tokens, t1: float, t2: float) -> int:
         """next_tokens: one id per row of last_token_rows().  Returns the number of tokens this step processed."""
         completes = [s + n == len(p.prompt) for p, s, n in self._new]
@@ -319,11 +344,22 @@ class DecodeGraphRunner:
     that hold under the key -- at most B members in a group, at most max_pages shared pages -- so it stays valid as members join
     or leave a group and as lengths grow.  Without groups the buffer is exactly the layout above.
 
+    With `sampling` (SamplingParams) the step samples instead of taking the argmax, and the buffer goes on, from the next even
+    offset (8-byte aligned: the buffer's base is), with  [keys(2B x u64) | counters(B x u64) | top_k(B) | T(B) | top_p(B)],
+    T and top_p as FP32 bit patterns -- still one H2D copy.  `sample_op` (ops.sample_tokens' signature) is the sampler the
+    step calls; host-only tests substitute a reference.  Without sampling the buffer is exactly the layout above.
+
     capture=False runs the same buffers through the model eagerly (the CPU tests use it; it is also the warm-up path)."""
 
-    def __init__(self, model: Callable, pool: KvPoolInt4, device, max_pages_per_seq: int, capture: bool = True):
+    def __init__(self, model: Callable, pool: KvPoolInt4, device, max_pages_per_seq: int, capture: bool = True,
+                 sampling: Optional[SamplingParams] = None, sample_op: Callable = None):
         self.model, self.pool, self.device = model, pool, torch.device(device)
         self.max_pages, self.capture = max_pages_per_seq, capture
+        self.sampling = sampling
+        if sample_op is None and sampling is not None:
+            from . import ops
+            sample_op = ops.sample_tokens
+        self.sample_op = sample_op
         self._entries = {}
 
     def _layout(self, b, ng=0):
@@ -331,10 +367,19 @@ class DecodeGraphRunner:
         o_grp = 3 * b + 1 + b * self.max_pages
         return o_ids, o_indptr, o_last, o_ind, o_grp, o_grp + (ng + 1 + 2 * b if ng else 0)
 
+    def _sampling_layout(self, b, ng=0):
+        """int32 offsets of keys, counters, top_k, T, top_p and the buffer's total size, when sampling."""
+        o_key = (self._layout(b, ng)[-1] + 1) // 2 * 2
+        o_ctr = o_key + 4 * b
+        o_k = o_ctr + 2 * b
+        return o_key, o_ctr, o_k, o_k + b, o_k + 2 * b, o_k + 3 * b
+
     def _entry(self, b, ng):
         e = self._entries.get((b, ng))
         if e is None:
             o_ids, o_indptr, o_last, o_ind, o_grp, total = self._layout(b, ng)
+            if self.sampling is not None:
+                total = self._sampling_layout(b, ng)[-1]
             host = torch.zeros(total, dtype=torch.int32)
             if self.device.type == "cuda":
                 host = host.pin_memory()
@@ -347,14 +392,21 @@ class DecodeGraphRunner:
                 kv.group_bounds = (b, self.max_pages)
             e = {"host": host, "dev": dev, "ids": dev[o_ids:o_ids + b], "kv": kv, "blen": BatchLenInfo([], b, self.device),
                  "graph": None, "out": None}
+            if self.sampling is not None:
+                o_key, o_ctr, o_k, o_t, o_p, _ = self._sampling_layout(b, ng)
+                e["sample"] = (dev[o_t:o_t + b].view(torch.float32), dev[o_k:o_k + b], dev[o_p:o_p + b].view(torch.float32),
+                               dev[o_key:o_ctr].view(torch.int64).view(b, 2), dev[o_ctr:o_k].view(torch.int64))
             self._entries[(b, ng)] = e
         return e
 
     def _step(self, e):
         logits, _ = self.model(e["ids"], e["blen"], None, e["kv"])
+        if self.sampling is not None:
+            return self.sample_op(logits, *e["sample"])
         return torch.argmax(logits, dim=-1)
 
-    def run(self, last_tokens: List[int], kvs: List[KvCacheInt4]) -> np.ndarray:
+    def run(self, last_tokens: List[int], kvs: List[KvCacheInt4], slots: Optional[List[tuple]] = None) -> np.ndarray:
+        """slots: (request index, counter) per sequence, needed with sampling (TextGenScheduler.sample_slots)."""
         b = len(kvs)
         groups = prefix_groups(kvs)
         ng = len(groups)
@@ -381,6 +433,15 @@ class DecodeGraphRunner:
             for rows, n in groups:
                 shared[rows] = n
             e["kv"].groups = groups              # the host view: it decides, when the step is captured, which decode runs
+        if self.sampling is not None:
+            o_key, o_ctr, o_k, o_t, o_p, _ = self._sampling_layout(b, ng)
+            sp = self.sampling
+            words = np.array([w for r, _ in slots for w in (int(sp.seed), r)], dtype=np.uint64)
+            h[o_key:o_ctr] = words.view(np.int32)
+            h[o_ctr:o_k] = np.array([c for _, c in slots], dtype=np.uint64).view(np.int32)
+            h[o_k:o_t] = int(sp.top_k)
+            h[o_t:o_p] = np.float32(sp.temperature).view(np.int32)
+            h[o_p:o_p + b] = np.float32(sp.top_p).view(np.int32)
         e["dev"].copy_(e["host"], non_blocking=True)
         if not self.capture:
             return self._step(e).cpu().numpy()
@@ -415,11 +476,20 @@ def pool_capacity(batch_size: int, maxlen: int, block_len: int) -> int:
 
 @torch.inference_mode()
 def run_textgen(model: Callable, rs: RequestSet, cfg: TextGenConfig, pool: KvPoolInt4, device, sync: Callable = None,
-                keep_tokens: bool = False, progress: Callable = None, decode_runner: DecodeGraphRunner = None) -> TextGenBenchResult:
+                keep_tokens: bool = False, progress: Callable = None, decode_runner: DecodeGraphRunner = None,
+                sample_op: Callable = None) -> TextGenBenchResult:
     """Drive `model(input_ids, blen, prefill_kv, decode_kv) -> (logits, hidden)` through the whole request set.
     Latencies are wall-clock around the step *including* the device->host read of the next tokens (which synchronises),
     as in the reference.  With a `decode_runner`, steps that carry no prompt tokens are replayed from its CUDA graphs.
-    cfg.prefill_chunk, cfg.shared_prefix: see TextGenScheduler."""
+    cfg.prefill_chunk, cfg.shared_prefix: see TextGenScheduler.  cfg.sampling: the eager steps call `sample_op` (default
+    ops.sample_tokens) on the rows whose logits are needed, with each row's key (seed, request) and counter; the runner, which
+    must have been built with the same SamplingParams, samples in its graphs."""
+    sp = cfg.sampling
+    if sp is not None and sample_op is None:
+        from . import ops
+        sample_op = ops.sample_tokens
+    if decode_runner is not None and decode_runner.sampling != sp:
+        raise ValueError("decode_runner was built for other sampling parameters than cfg.sampling")
     sched = TextGenScheduler(rs, cfg.batch_size, pool, device, vocab_size=_vocab_size(model), prefill_chunk=cfg.prefill_chunk,
                              shared_prefix=cfg.shared_prefix)
     steps = graphed = peak = 0
@@ -429,14 +499,21 @@ def run_textgen(model: Callable, rs: RequestSet, cfg: TextGenConfig, pool: KvPoo
         peak = max(peak, pool.capacity - pool.num_free_blocks)
         t1 = time.perf_counter()
         if decode_runner is not None and sched.prompt_tokens == 0:
-            next_tokens = decode_runner.run([int(r.output[-1]) for r in sched.workset], [r.kvcache for r in sched.workset])
+            next_tokens = decode_runner.run([int(r.output[-1]) for r in sched.workset], [r.kvcache for r in sched.workset],
+                                            sched.sample_slots() if sp is not None else None)
             graphed += 1
         else:
             batch = sched.next_batch()
             ids = torch.tensor(batch.input_ids, dtype=torch.long, device=device)
             logits, _ = model(ids, batch.blen, batch.prefill_kv, batch.decode_kv)
             rows = torch.tensor(sched.last_token_rows(), dtype=torch.long, device=logits.device)
-            next_tokens = torch.argmax(logits.index_select(0, rows), dim=-1).cpu().numpy()
+            if sp is None:
+                next_tokens = torch.argmax(logits.index_select(0, rows), dim=-1).cpu().numpy()
+            else:
+                slots = sched.sample_slots()
+                n = len(slots)
+                next_tokens = sample_op(logits.index_select(0, rows), [sp.temperature] * n, [sp.top_k] * n, [sp.top_p] * n,
+                                        [(int(sp.seed), r) for r, _ in slots], [c for _, c in slots]).cpu().numpy()
         if sync is not None:
             sync()
         t2 = time.perf_counter()
@@ -464,4 +541,5 @@ def report(rs: RequestSet, cfg: TextGenConfig, res: TextGenBenchResult) -> dict:
         "total_prompt_tokens": int(rs.prompt_lens.sum()), "total_new_tokens": int(rs.output_lens.sum()),
         "duration_s": res.duration, "throughput_tokens_per_s": total / res.duration, "peak_kv_pages_in_use": res.peak_pages,
         "shared_prefix": cfg.shared_prefix,
+        "sampling": None if cfg.sampling is None else dataclasses.asdict(cfg.sampling),
     }

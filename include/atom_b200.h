@@ -317,6 +317,26 @@ ATOM_API int atom_gemm_i4_o16_grouped(const void* a, const void* b, const void* 
 ATOM_API int atom_moe_combine_f16(const void* y, const void* topk_ids, const void* topk_weights, const void* dest_row, int seq_len, int hidden_dim,
                          int top_k, void* out, void* stream);
 
+/* atom_sample_f16: one token id per row of FP16 logits, sampled with per-row temperature, top-k and top-p from a counter-based
+ * Philox stream (new: the reference only takes the argmax).
+ *   logits f16 [batch, ld] (row b at logits + b*ld, the first vocab entries used; vocab <= 262144)
+ *   temperature f32 [batch], top_k i32 [batch] (0 = off), top_p f32 [batch] (1 = off), key u64 [batch][2], counter u64 [batch],
+ *   out i32 [batch].  All parameters are read on the device, after the preceding kernel has completed.
+ * One total order throughout: value descending, then index ascending (-0 == +0).  Per row:
+ *   1. A NaN or +inf logit, all logits -inf, or parameters out of range (T not finite or < 0, top_k < 0, top_p not in (0, 1])
+ *      give -1.  A -inf logit is masked: it is never drawn.
+ *   2. T == 0 or top_k == 1: the first index of the maximum (torch.argmax).
+ *   3. top_k = k > 0: exactly the first k tokens of the order on the raw FP16 logits (ties at the k-th value to lower indices).
+ *   4. top_p = p < 1: over the top-k survivors with weights w = round(expf(fl(fl(l - max) / T)) * 2^40) (FP32, then an exact
+ *      integer), keep the tokens of the order whose exclusive mass is below ceil(p * Z), Z their total: the shortest prefix
+ *      whose mass reaches p.  The top token is always kept.
+ *   5. The draw: u = (w0 >> 11) * 2^-53, w0 = word 0 of the Philox4x64-10 block at counter (counter[b], 0, 0, 0) under key
+ *      (key[b][0], key[b][1]); the token is the first kept index, ascending, whose running sum of weights exceeds floor(u * Z).
+ * The result of a row depends only on that row's logits, parameters, key and counter: not on batch, its position, ld or the
+ * launch.  No state: a captured graph replays with new device values. */
+ATOM_API int atom_sample_f16(const void* logits, int64_t ld, int batch, int vocab, const void* temperature, const void* top_k,
+                             const void* top_p, const void* key, const void* counter, void* out, void* stream);
+
 /* replaces append_kv_i4 (punica_ops.cc:166-209 -> FlashInferAppendKvKernel_i4<128>, flashinfer_impl.cuh:73-96)
  *   k,v u8 [B,H,64]  k_param,v_param f16 [B,H,2] */
 ATOM_API int atom_append_kv_i4(void* kv_data, void* kv_param, const void* kv_indptr, const void* kv_indices,

@@ -51,6 +51,11 @@ def main():
                     help="chunked prefill: at most this many prompt tokens per step (default: whole prompts)")
     ap.add_argument("--shared-prefix", type=int, default=0, metavar="N",
                     help="precede every prompt with one common N-token system prompt, prefilled once and shared by forking")
+    ap.add_argument("--temperature", type=float, default=None,
+                    help="sample at this temperature on the device (ops.sample_tokens); default: greedy (argmax)")
+    ap.add_argument("--top-k", type=int, default=0, help="with sampling: keep the k largest logits (0 = off)")
+    ap.add_argument("--top-p", type=float, default=1.0, help="with sampling: keep the smallest set of mass >= p (1 = off)")
+    ap.add_argument("--seed", type=int, default=0, help="with sampling: request r draws from the Philox key (seed, r)")
     ap.add_argument("--warmup-batches", type=int, default=1,
                     help="untimed request batches served first (first-use costs: lazy kernel loading, attribute calls, graph "
                          "capture); 0 = time the cold process like the reference's script")
@@ -64,13 +69,17 @@ def main():
     torch.manual_seed(tg.SEED)
     model = build_model(mc, layers)
     rs = tg.generate_request_set(args.batch_size * args.num_batches, args.maxlen)
-    cfg = tg.TextGenConfig(args.batch_size, prefill_chunk=args.prefill_chunk, shared_prefix=args.shared_prefix)
+    if args.temperature is None and (args.top_k or args.top_p != 1.0):
+        ap.error("--top-k / --top-p need --temperature")
+    sampling = None if args.temperature is None else tg.SamplingParams(args.temperature, args.top_k, args.top_p, args.seed)
+    cfg = tg.TextGenConfig(args.batch_size, prefill_chunk=args.prefill_chunk, shared_prefix=args.shared_prefix, sampling=sampling)
     shared_pages = -(-args.shared_prefix // args.block_len)           # the system prompt's pages, held once
     pool = KvPoolInt4(layers, mc.kv_heads, mc.hidden_size // mc.num_heads,     # the cache holds KV heads (grouped-query: fewer)
                       tg.pool_capacity(args.batch_size, args.maxlen, args.block_len) + shared_pages + args.batch_size * (shared_pages > 0),
                       args.block_len, device)
     runner = None if args.no_cuda_graphs else tg.DecodeGraphRunner(
-        model, pool, device, max_pages_per_seq=(args.maxlen + args.block_len - 1) // args.block_len + 1 + shared_pages)
+        model, pool, device, max_pages_per_seq=(args.maxlen + args.block_len - 1) // args.block_len + 1 + shared_pages,
+        sampling=sampling)
     if args.warmup_batches > 0:
         wrs = tg.generate_request_set(args.batch_size * args.warmup_batches, args.maxlen)
         tg.run_textgen(model, wrs, cfg, pool, device, sync=torch.cuda.synchronize, decode_runner=runner)
