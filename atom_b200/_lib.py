@@ -49,6 +49,8 @@ _SIGNATURES = {
     "atom_gemm_i4_o16_grouped": (_I, [_P] * 10 + [_I, _I, _I64, _I64, _I64, _I64, _P]),
     "atom_moe_combine_f16": (_I, [_P] * 4 + [_I, _I, _I, _P, _P]),
     "atom_sample_f16": (_I, [_P, _I64, _I, _I] + [_P] * 7),
+    "atom_sample_ex_f16": (_I, [_P, _I64, _I, _I] + [_P] * 11 + [_I64, _P, _P, _I, _P, _P, _P]),
+    "atom_sample_slot_init": (_I, [_P, _I64, _I, _I, _P, _I, _P]),
 }
 
 _lib = None

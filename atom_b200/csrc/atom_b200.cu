@@ -996,27 +996,22 @@ int atom_moe_combine_f16(const void* y, const void* topk_ids, const void* topk_w
                   (__half*)out);
 }
 
-int atom_sample_f16(const void* logits, int64_t ld, int batch, int vocab, const void* temperature, const void* top_k, const void* top_p,
-                    const void* key, const void* counter, void* out, void* stream) {
-  ATOM_REQUIRE(logits && temperature && top_k && top_p && key && counter && out, "sample_f16: null pointer argument");
-  ATOM_REQUIRE(batch > 0 && vocab > 0 && vocab <= atom::SAMPLE_MAX_CLUSTER * atom::SAMPLE_SLICE_MAX,
-               "sample_f16: batch=%d must be positive, vocab=%d in [1, %d]", batch, vocab,
-               atom::SAMPLE_MAX_CLUSTER * atom::SAMPLE_SLICE_MAX);
-  ATOM_REQUIRE(ld >= vocab || batch == 1, "sample_f16: ld=%lld must be >= vocab=%d", (long long)ld, vocab);
-  ATOM_REQUIRE((reinterpret_cast<uintptr_t>(logits) & 1) == 0 && (reinterpret_cast<uintptr_t>(key) & 7) == 0 &&
-               (reinterpret_cast<uintptr_t>(counter) & 7) == 0 && (reinterpret_cast<uintptr_t>(temperature) & 3) == 0 &&
-               (reinterpret_cast<uintptr_t>(top_k) & 3) == 0 && (reinterpret_cast<uintptr_t>(top_p) & 3) == 0 &&
-               (reinterpret_cast<uintptr_t>(out) & 3) == 0, "sample_f16: misaligned pointer (logits 2, key / counter 8, the rest 4 bytes)");
-  ATOM_REQUIRE((long long)batch * atom::SAMPLE_MAX_CLUSTER < (1ll << 31), "sample_f16: batch=%d too large", batch);
-  const int C = atom::sample_cluster(vocab), slice = atom::sample_slice(vocab);
-  const size_t smem = atom::SAMPLE_SMEM_FIXED + (size_t)slice * sizeof(uint16_t);
-  int rc = ensure_dynamic_smem(atom::sample_kernel, (int)(atom::SAMPLE_SMEM_FIXED + atom::SAMPLE_SLICE_MAX * sizeof(uint16_t)), "sample_f16");
+}  // extern "C"
+
+namespace {
+
+template <bool PEN, bool EXT>
+int sample_launch(const atom::SampleArgs& args, const atom::SampleExArgs& x, int batch, cudaStream_t stream) {
+  const int C = atom::sample_cluster(args.V);
+  const size_t fixed = EXT ? atom::sample_ex_offset(args.slice) + sizeof(atom::SampleExShared)
+                           : atom::SAMPLE_SMEM_FIXED + (size_t)args.slice * sizeof(uint16_t);
+  const int most = (int)(EXT ? atom::sample_ex_offset(atom::SAMPLE_SLICE_MAX) + sizeof(atom::SampleExShared)
+                             : atom::SAMPLE_SMEM_FIXED + atom::SAMPLE_SLICE_MAX * sizeof(uint16_t));
+  int rc = ensure_dynamic_smem(atom::sample_kernel<PEN, EXT>, most, "sample_f16");
   if (rc) return rc;
-  atom::SampleArgs args{(const __half*)logits, (long long)ld, vocab, slice, (const float*)temperature, (const int32_t*)top_k,
-                        (const float*)top_p, (const unsigned long long*)key, (const unsigned long long*)counter, (int32_t*)out};
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(C * batch)); cfg.blockDim = dim3(atom::SAMPLE_THREADS); cfg.dynamicSmemBytes = smem;
-  cfg.stream = (cudaStream_t)stream;
+  cfg.gridDim = dim3((unsigned)(C * batch)); cfg.blockDim = dim3(atom::SAMPLE_THREADS); cfg.dynamicSmemBytes = fixed;
+  cfg.stream = stream;
   cudaLaunchAttribute attr[2];
   attr[0].id = cudaLaunchAttributeClusterDimension;
   attr[0].val.clusterDim.x = C; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
@@ -1027,9 +1022,82 @@ int atom_sample_f16(const void* logits, int64_t ld, int batch, int vocab, const 
     attr[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.numAttrs = 2;
   }
-  cudaError_t e = cudaLaunchKernelEx(&cfg, atom::sample_kernel, args, pdl);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, atom::sample_kernel<PEN, EXT>, args, pdl, x);
   if (e != cudaSuccess) return fail(ATOM_E_CUDA, "sample_f16 launch (cluster %d): %s", C, cudaGetErrorString(e));
   return check_launch("sample_f16");
+}
+
+int sample_check(const void* logits, int64_t ld, int batch, int vocab, const void* temperature, const void* top_k, const void* top_p,
+                 const void* key, const void* counter, void* out) {
+  ATOM_REQUIRE(logits && temperature && top_k && top_p && key && counter && out, "sample_f16: null pointer argument");
+  ATOM_REQUIRE(batch > 0 && vocab > 0 && vocab <= atom::SAMPLE_MAX_CLUSTER * atom::SAMPLE_SLICE_MAX,
+               "sample_f16: batch=%d must be positive, vocab=%d in [1, %d]", batch, vocab,
+               atom::SAMPLE_MAX_CLUSTER * atom::SAMPLE_SLICE_MAX);
+  ATOM_REQUIRE(ld >= vocab || batch == 1, "sample_f16: ld=%lld must be >= vocab=%d", (long long)ld, vocab);
+  ATOM_REQUIRE((reinterpret_cast<uintptr_t>(logits) & 1) == 0 && (reinterpret_cast<uintptr_t>(key) & 7) == 0 &&
+               (reinterpret_cast<uintptr_t>(counter) & 7) == 0 && (reinterpret_cast<uintptr_t>(temperature) & 3) == 0 &&
+               (reinterpret_cast<uintptr_t>(top_k) & 3) == 0 && (reinterpret_cast<uintptr_t>(top_p) & 3) == 0 &&
+               (reinterpret_cast<uintptr_t>(out) & 3) == 0, "sample_f16: misaligned pointer (logits 2, key / counter 8, the rest 4 bytes)");
+  ATOM_REQUIRE((long long)batch * atom::SAMPLE_MAX_CLUSTER < (1ll << 31), "sample_f16: batch=%d too large", batch);
+  return ATOM_OK;
+}
+
+atom::SampleArgs sample_args(const void* logits, int64_t ld, int vocab, const void* temperature, const void* top_k, const void* top_p,
+                             const void* key, const void* counter, void* out) {
+  return atom::SampleArgs{(const __half*)logits, (long long)ld, vocab, atom::sample_slice(vocab), (const float*)temperature,
+                          (const int32_t*)top_k, (const float*)top_p, (const unsigned long long*)key,
+                          (const unsigned long long*)counter, (int32_t*)out};
+}
+
+bool aligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
+
+}  // namespace
+
+extern "C" {
+
+int atom_sample_f16(const void* logits, int64_t ld, int batch, int vocab, const void* temperature, const void* top_k, const void* top_p,
+                    const void* key, const void* counter, void* out, void* stream) {
+  int rc = sample_check(logits, ld, batch, vocab, temperature, top_k, top_p, key, counter, out);
+  if (rc) return rc;
+  return sample_launch<false, false>(sample_args(logits, ld, vocab, temperature, top_k, top_p, key, counter, out),
+                                     atom::SampleExArgs{}, batch, (cudaStream_t)stream);
+}
+
+int atom_sample_ex_f16(const void* logits, int64_t ld, int batch, int vocab, const void* temperature, const void* top_k,
+                       const void* top_p, const void* key, const void* counter, const void* min_p, const void* rep, const void* freq,
+                       const void* pres, const void* slots, void* table, int64_t table_ld, void* out, void* logprob_out, int top_n,
+                       void* top_ids, void* top_logprobs, void* stream) {
+  int rc = sample_check(logits, ld, batch, vocab, temperature, top_k, top_p, key, counter, out);
+  if (rc) return rc;
+  const bool pen = table != nullptr;
+  ATOM_REQUIRE(pen ? (rep && freq && pres && slots) : !(rep || freq || pres || slots),
+               "sample_ex_f16: rep, freq, pres and slots are given with a table and only then");
+  ATOM_REQUIRE(!pen || (table_ld >= vocab && (reinterpret_cast<uintptr_t>(table) & 1) == 0),
+               "sample_ex_f16: table_ld=%lld must be >= vocab=%d and the table 2-byte aligned", (long long)table_ld, vocab);
+  ATOM_REQUIRE(top_n >= 0 && top_n <= atom::SAMPLE_TOP_N_MAX && (top_n == 0 || (top_ids && top_logprobs)),
+               "sample_ex_f16: top_n=%d must be in [0, %d], with top_ids and top_logprobs", top_n, atom::SAMPLE_TOP_N_MAX);
+  ATOM_REQUIRE(aligned4(min_p) && aligned4(rep) && aligned4(freq) && aligned4(pres) && aligned4(slots) && aligned4(logprob_out) &&
+               aligned4(top_ids) && aligned4(top_logprobs), "sample_ex_f16: misaligned pointer (4 bytes)");
+  const atom::SampleArgs args = sample_args(logits, ld, vocab, temperature, top_k, top_p, key, counter, out);
+  const atom::SampleExArgs x{(const float*)min_p, (const float*)rep, (const float*)freq, (const float*)pres, (const int32_t*)slots,
+                             (uint16_t*)table, (long long)table_ld, (float*)logprob_out, top_n, (int32_t*)top_ids,
+                             (float*)top_logprobs};
+  const bool ext = min_p || logprob_out || top_n;
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (pen) return ext ? sample_launch<true, true>(args, x, batch, st) : sample_launch<true, false>(args, x, batch, st);
+  return ext ? sample_launch<false, true>(args, x, batch, st) : sample_launch<false, false>(args, x, batch, st);
+}
+
+int atom_sample_slot_init(void* table, int64_t table_ld, int vocab, int slot, const void* prompt, int prompt_len, void* stream) {
+  ATOM_REQUIRE(table && (reinterpret_cast<uintptr_t>(table) & 15) == 0 && table_ld >= vocab && table_ld % 8 == 0 && vocab > 0 &&
+               slot >= 0, "sample_slot_init: need a 16-byte aligned table, vocab=%d > 0, table_ld=%lld >= vocab and a multiple "
+               "of 8, slot=%d >= 0", vocab, (long long)table_ld, slot);
+  ATOM_REQUIRE(prompt_len >= 0 && (prompt_len == 0 || (prompt && aligned4(prompt))), "sample_slot_init: prompt_len=%d, prompt "
+               "i32 4-byte aligned", prompt_len);
+  const int chunk = atom::SAMPLE_INIT_CHUNK;
+  return launch_k("sample_slot_init", atom::sample_slot_init_kernel, dim3((unsigned)((table_ld + chunk - 1) / chunk)),
+                  dim3(atom::SAMPLE_INIT_THREADS), 0, (cudaStream_t)stream, (uint16_t*)table + (long long)slot * table_ld,
+                  (long long)table_ld, vocab, (const int32_t*)prompt, prompt_len);
 }
 
 }  // extern "C"

@@ -646,13 +646,89 @@ def _sample_param(name, v, b, dtype, device, check):
     return torch.from_numpy(np.ascontiguousarray(a)).to(dtype).to(device)
 
 
-def sample_tokens(logits, temperature, top_k, top_p, keys, counters):
+SAMPLE_TOP_N_MAX = 20
+
+
+def penalty_table(slots, vocab, device):
+    """EXTENSION: a zeroed penalty table for `slots` requests over a `vocab`-token vocabulary, for sample_tokens' penalties:
+    int16 [slots, ld] holding the u16 entries of atom_sample_ex_f16 (bit 15: the token is in the request's prompt; bits 0-14:
+    how often the request has generated it, saturating at 0x7FFF), ld = vocab rounded up to a multiple of 8."""
+    if int(slots) < 1 or int(vocab) < 1:
+        raise RuntimeError(f"atom_b200.ops.penalty_table: need slots >= 1 and vocab >= 1, got {slots}, {vocab}")
+    return torch.zeros((int(slots), (int(vocab) + 7) // 8 * 8), dtype=torch.int16, device=device)
+
+
+def _check_table(table):
+    if not (isinstance(table, torch.Tensor) and table.is_cuda):
+        raise RuntimeError("atom_b200.ops: all tensors must live on a CUDA device (there is no CPU path)")
+    if table.dtype not in (torch.int16, torch.uint16) or table.dim() != 2 or table.stride(1) != 1 or table.stride(0) % 8 or \
+            table.data_ptr() % 16:
+        raise RuntimeError("atom_b200.ops: a penalty table is 16-bit [slots, ld] with unit stride along ld, a row pitch that is a "
+                           "multiple of 8 and a 16-byte aligned base (ops.penalty_table)")
+
+
+def init_penalty_slot(table, slot, prompt):
+    """EXTENSION: set up `slot` of a penalty table for a new request in one launch: zero its row and mark every token of `prompt`
+    (all the request's prompt, a shared system prompt included) as a prompt token.  prompt: token ids, a host sequence (checked
+    to lie in [0, ld)) or an int32 CUDA tensor (ids outside it are ignored)."""
+    _check_table(table)
+    if not 0 <= int(slot) < table.size(0):
+        raise RuntimeError(f"atom_b200.ops.init_penalty_slot: slot {slot} outside [0, {table.size(0)})")
+    if isinstance(prompt, torch.Tensor):
+        _req_cuda(prompt)
+        if prompt.dtype != torch.int32 or prompt.dim() != 1 or not prompt.is_contiguous():
+            raise RuntimeError("atom_b200.ops.init_penalty_slot: a prompt tensor must be contiguous int32 [n]")
+        ids = prompt
+    else:
+        import numpy as np
+        a = np.asarray(prompt, dtype=np.int64).reshape(-1)
+        if a.size and (a.min() < 0 or a.max() >= table.size(1)):
+            raise RuntimeError(f"atom_b200.ops.init_penalty_slot: prompt ids must lie in [0, {table.size(1)})")
+        ids = torch.from_numpy(a.astype(np.int32)).to(table.device)
+    with torch.cuda.device(table.device):
+        _lib.check(_lib.lib().atom_sample_slot_init(table.data_ptr(), table.stride(0), table.size(1), int(slot),
+                                                    ids.data_ptr() if ids.numel() else None, ids.numel(), _stream(table)),
+                   "init_penalty_slot")
+
+
+def _neutral(v, value):
+    import numpy as np
+    return not isinstance(v, torch.Tensor) and bool(np.all(np.asarray(v, dtype=np.float64) == value))
+
+
+def _sample_slots(slots, b, table, device):
+    if isinstance(slots, torch.Tensor):
+        _req_cuda(slots)
+        if slots.dtype != torch.int32 or tuple(slots.shape) != (b,) or slots.device != device:
+            raise RuntimeError(f"atom_b200.ops.sample_tokens: `slots` must be int32 [{b}] on {device}")
+        return slots
+    import numpy as np
+    a = np.asarray(slots, dtype=np.int64).reshape(-1)
+    if a.shape != (b,) or (a < -1).any() or (a >= table.size(0)).any():
+        raise RuntimeError(f"atom_b200.ops.sample_tokens: `slots` must hold {b} entries in [-1, {table.size(0)})")
+    used = a[a >= 0]
+    if len(np.unique(used)) != len(used):
+        raise RuntimeError("atom_b200.ops.sample_tokens: the rows of one call must use distinct slots")
+    return torch.from_numpy(a.astype(np.int32)).to(device)
+
+
+def sample_tokens(logits, temperature, top_k, top_p, keys, counters, *, min_p=0.0, repetition_penalty=1.0, frequency_penalty=0.0,
+                  presence_penalty=0.0, penalty_table=None, slots=None, logprobs=None):
     """EXTENSION: one token id per row of f16 logits [B, V] (rows may have any pitch), int32 [B].  Per row: temperature
     (0 = argmax), top_k (0 = off, on the raw logits), top_p (1 = off), Philox key (key0, key1) and counter; the semantics are
     atom_sample_f16's (include/atom_b200.h, DESIGN section 5.6).  Each parameter is a CUDA tensor with one entry per row (keys:
     [B, 2]; keys and counters int64 holding the uint64 bit patterns) whose values are read on the device -- so a captured graph
     replays with new ones -- or a host sequence or scalar, which is validated (T finite and >= 0, top_k >= 0, top_p in (0, 1])
-    and copied.  Rows with NaN / +inf logits, only -inf logits, or out-of-range device parameters give -1."""
+    and copied.  Rows with NaN / +inf logits, only -inf logits, or out-of-range device parameters give -1.
+
+    The keyword options (atom_sample_ex_f16; at their defaults the call and its result are exactly the above), each per row like
+    the parameters:
+      min_p in [0, 1] (0 = off); repetition_penalty > 0 (1 = off), frequency_penalty and presence_penalty finite (0 = off),
+      which need penalty_table (ops.penalty_table) and slots (int32 [B], -1 = no state, distinct in one call): the kernel
+      penalises each row's logits by its slot's history and records the drawn token in that slot;
+      logprobs = n in [0, 20]: also return, per row, the log-probability of the chosen token (float32 [B]) and the first n
+      tokens of the order on the penalised logits with theirs (int32 / float32 [B, n]), a log-softmax at temperature 1.
+    With logprobs the result is (tokens, logprob, top_ids, top_logprobs)."""
     if not (isinstance(logits, torch.Tensor) and logits.is_cuda):
         raise RuntimeError("atom_b200.ops: all tensors must live on a CUDA device (there is no CPU path)")
     if logits.dtype != torch.float16 or logits.dim() != 2 or logits.stride(1) != 1:
@@ -665,6 +741,15 @@ def sample_tokens(logits, temperature, top_k, top_p, keys, counters):
     p = _sample_param("top_p", top_p, b, torch.float32, dev, lambda a: ~((a > 0) & (a <= 1)))
     key = _sample_param("keys", keys, b, torch.int64, dev, None)
     ctr = _sample_param("counters", counters, b, torch.int64, dev, None)
+    pen = penalty_table is not None
+    if not pen and (slots is not None or not (_neutral(repetition_penalty, 1) and _neutral(frequency_penalty, 0) and
+                                              _neutral(presence_penalty, 0))):
+        raise RuntimeError("atom_b200.ops.sample_tokens: penalties need a penalty_table and slots")
+    if logprobs is not None and not (isinstance(logprobs, (int, np.integer)) and 0 <= int(logprobs) <= SAMPLE_TOP_N_MAX):
+        raise RuntimeError(f"atom_b200.ops.sample_tokens: logprobs must be an integer in [0, {SAMPLE_TOP_N_MAX}], got {logprobs!r}")
+    if pen or logprobs is not None or not _neutral(min_p, 0):
+        return _sample_ex(logits, t, k, p, key, ctr, min_p, repetition_penalty, frequency_penalty, presence_penalty, penalty_table,
+                          slots, logprobs)
     out = torch.empty((b,), dtype=torch.int32, device=dev)
     if b == 0:
         return out
@@ -673,3 +758,35 @@ def sample_tokens(logits, temperature, top_k, top_p, keys, counters):
                                               p.data_ptr(), key.data_ptr(), ctr.data_ptr(), out.data_ptr(), _stream(logits)),
                    "sample_tokens")
     return out
+
+
+def _sample_ex(logits, t, k, p, key, ctr, min_p, rep, freq, pres, table, slots, logprobs):
+    import numpy as np
+    b, v = logits.shape
+    dev = logits.device
+    m = None if _neutral(min_p, 0) else _sample_param("min_p", min_p, b, torch.float32, dev, lambda a: ~((a >= 0) & (a <= 1)))
+    pen = table is not None
+    if pen:
+        _check_table(table)
+        if table.device != dev or table.size(1) < v:
+            raise RuntimeError(f"atom_b200.ops.sample_tokens: penalty_table must be on {dev} with at least {v} columns")
+        if slots is None:
+            raise RuntimeError("atom_b200.ops.sample_tokens: penalty_table needs slots")
+        sl = _sample_slots(slots, b, table, dev)
+        r = _sample_param("repetition_penalty", rep, b, torch.float32, dev, lambda a: ~np.isfinite(a) | (a <= 0))
+        f = _sample_param("frequency_penalty", freq, b, torch.float32, dev, lambda a: ~np.isfinite(a))
+        q = _sample_param("presence_penalty", pres, b, torch.float32, dev, lambda a: ~np.isfinite(a))
+    n = 0 if logprobs is None else int(logprobs)
+    out = torch.empty((b,), dtype=torch.int32, device=dev)
+    lp = torch.empty((b,), dtype=torch.float32, device=dev) if logprobs is not None else None
+    top_ids = torch.empty((b, n), dtype=torch.int32, device=dev)
+    top_lp = torch.empty((b, n), dtype=torch.float32, device=dev)
+    if b:
+        ptr = lambda x: None if x is None else x.data_ptr()      # noqa: E731
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().atom_sample_ex_f16(
+                logits.data_ptr(), logits.stride(0) if b > 1 else v, b, v, t.data_ptr(), k.data_ptr(), p.data_ptr(), key.data_ptr(),
+                ctr.data_ptr(), ptr(m), ptr(r) if pen else None, ptr(f) if pen else None, ptr(q) if pen else None,
+                ptr(sl) if pen else None, ptr(table) if pen else None, table.stride(0) if pen else 0, out.data_ptr(), ptr(lp), n,
+                top_ids.data_ptr() if n else None, top_lp.data_ptr() if n else None, _stream(logits)), "sample_tokens")
+    return out if logprobs is None else (out, lp, top_ids, top_lp)

@@ -16,8 +16,9 @@ Same workload: the request set (prompt ~ lognorm(0.8, -1, 18) clipped to [1, max
   * admission checks the pool for free pages instead of assuming capacity.
 """
 import dataclasses
+import heapq
 import time
-from typing import Callable, List, Optional
+from typing import Callable, List, Optional, Tuple
 
 import numpy as np
 import torch
@@ -80,17 +81,58 @@ MODEL_CFGS = {
 class SamplingParams:
     """Sampled decoding (ops.sample_tokens): every request draws its tokens at this temperature (0 = greedy), top_k (0 = off)
     and top_p (1 = off).  Request r's Philox key is (seed, r) and the counter of a token is the number of tokens r generated
-    before it, so its tokens depend on its own logits only -- not on batching, chunking, shared prefixes or graphs."""
+    before it, so its tokens depend on its own logits only -- not on batching, chunking, shared prefixes or graphs.
+
+    min_p (0 = off), repetition_penalty (1 = off), frequency_penalty and presence_penalty (0 = off) and logprobs (None = off,
+    else the top-n list's length, 0 to 20) are ops.sample_tokens' options.  With any penalty every request holds a slot of a
+    device penalty table (its prompt tokens and a count of each token it generated), which the sampler reads and updates."""
     temperature: float
     top_k: int = 0
     top_p: float = 1.0
     seed: int = 0
+    min_p: float = 0.0
+    repetition_penalty: float = 1.0
+    frequency_penalty: float = 0.0
+    presence_penalty: float = 0.0
+    logprobs: Optional[int] = None
+
+    _EXTRAS = {"min_p": 0.0, "repetition_penalty": 1.0, "frequency_penalty": 0.0, "presence_penalty": 0.0, "logprobs": None}
 
     def __post_init__(self):
         if not (np.isfinite(self.temperature) and self.temperature >= 0):
             raise ValueError(f"temperature must be finite and >= 0, got {self.temperature}")
         if int(self.top_k) < 0 or not (0 < self.top_p <= 1) or not (0 <= int(self.seed) < 1 << 64):
             raise ValueError(f"need top_k >= 0, top_p in (0, 1] and a seed in [0, 2^64): {self}")
+        if not (0 <= self.min_p <= 1) or not (np.isfinite(self.repetition_penalty) and self.repetition_penalty > 0) or \
+                not np.isfinite(self.frequency_penalty) or not np.isfinite(self.presence_penalty):
+            raise ValueError(f"need min_p in [0, 1], repetition_penalty finite and > 0, finite frequency and presence penalties: {self}")
+        if self.logprobs is not None and not (isinstance(self.logprobs, (int, np.integer)) and 0 <= self.logprobs <= 20):
+            raise ValueError(f"logprobs must be None or an integer in [0, 20], got {self.logprobs!r}")
+
+    @property
+    def penalties(self) -> bool:
+        """Whether any penalty is on (the requests then hold penalty-table slots)."""
+        return self.repetition_penalty != 1 or self.frequency_penalty != 0 or self.presence_penalty != 0
+
+    @property
+    def extended(self) -> bool:
+        """Whether the sampler is called with options beyond temperature, top-k and top-p."""
+        return self.penalties or self.min_p != 0 or self.logprobs is not None
+
+    def options(self, n: int, table=None, slots=None) -> dict:
+        """ops.sample_tokens' keyword options for n rows (host values) with the given table and row slots."""
+        o = {"min_p": [self.min_p] * n}
+        if self.penalties:
+            o.update(repetition_penalty=[self.repetition_penalty] * n, frequency_penalty=[self.frequency_penalty] * n,
+                     presence_penalty=[self.presence_penalty] * n, penalty_table=table, slots=slots)
+        if self.logprobs is not None:
+            o["logprobs"] = int(self.logprobs)
+        return o
+
+    def asdict(self) -> dict:
+        """The settings; the options beyond temperature, top-k, top-p and seed only when they are not at their defaults."""
+        d = dataclasses.asdict(self)
+        return {k: v for k, v in d.items() if k not in self._EXTRAS or v != self._EXTRAS[k]}
 
 
 @dataclasses.dataclass
@@ -99,6 +141,7 @@ class TextGenConfig:
     prefill_chunk: Optional[int] = None     # at most this many prompt tokens per step (chunked prefill); None = whole prompts
     shared_prefix: int = 0                  # tokens of one system prompt before every request's prompt, prefilled once and forked
     sampling: Optional[SamplingParams] = None   # None: greedy (argmax)
+    stop_token_ids: Tuple[int, ...] = ()        # a request that emits one of these finishes on it (greedy or sampled)
 
 
 @dataclasses.dataclass
@@ -110,6 +153,9 @@ class TextGenBenchResult:
     tokens: Optional[List[List[int]]] = None
     graphed_steps: int = 0
     peak_pages: int = 0                     # most KV pages in use after any step's admission
+    output_lens: Optional[np.ndarray] = None    # tokens each request generated (fewer than asked when it met a stop id)
+    logprobs: Optional[List[List[float]]] = None    # with SamplingParams.logprobs and keep_tokens: each token's log-probability
+    top_logprobs: Optional[List[List[Tuple[List[int], List[float]]]]] = None    # ... and each token's top-n (ids, logprobs)
 
 
 @dataclasses.dataclass
@@ -120,6 +166,9 @@ class RequestContext:
     encode_latency: float = 0.0
     decode_start_at: float = 0.0
     decode_latency: float = 0.0
+    slot: int = -1                          # its penalty-table slot (-1: none)
+    logprobs: List[float] = dataclasses.field(default_factory=list)
+    top_logprobs: List[tuple] = dataclasses.field(default_factory=list)
 
 
 @dataclasses.dataclass(eq=False)
@@ -130,6 +179,7 @@ class _Prefill:
     kvcache: KvCacheInt4
     done: int = 0                           # prompt tokens already in the cache
     start_at: Optional[float] = None        # start of the step that carried its first chunk
+    slot: int = -1                          # its penalty-table slot (-1: none)
 
 
 @dataclasses.dataclass
@@ -154,10 +204,16 @@ class TextGenScheduler:
     its own (the request set and the requests' prompts are those of N = 0).  It is prefilled once, first, as a root sequence that
     produces no token (chunked under prefill_chunk like any prompt); each request admitted after that is `root.fork()` followed
     by its own prompt as a continuation, and admission counts only the pages the fork takes.  The root is released when the last
-    request finishes.  Decode batches of forked requests carry prefix groups (kvcache.BatchedKvCacheInt4)."""
+    request finishes.  Decode batches of forked requests carry prefix groups (kvcache.BatchedKvCacheInt4).
+
+    stop_token_ids: a request that emits one of them finishes on that token (its pages and slot are released).
+    penalty_slots=True: every admitted request takes a slot of a penalty table of batch_size slots (the smallest free one), to be
+    set up with its whole prompt -- the system prompt and its own -- before its first token is drawn: `slot_inits` lists the
+    (slot, prompt tokens) the driver must apply after each admit().  The slot is freed when the request finishes; the system
+    prompt's root sequence has none."""
 
     def __init__(self, rs: RequestSet, batch_size: int, pool: KvPoolInt4, device, vocab_size: int = 32000,
-                 prefill_chunk: Optional[int] = None, shared_prefix: int = 0):
+                 prefill_chunk: Optional[int] = None, shared_prefix: int = 0, stop_token_ids=(), penalty_slots: bool = False):
         if prefill_chunk is not None and int(prefill_chunk) < 1:
             raise ValueError("prefill_chunk must be a positive number of tokens (or None)")
         if int(shared_prefix) < 0:
@@ -179,6 +235,9 @@ class TextGenScheduler:
             system = np.random.Generator(np.random.PCG64(seed=SEED + 1)).integers(0, vocab_size, self.shared_prefix).tolist()
             self._root = _Prefill(-1, system, KvCacheInt4(pool, 0))
             self._prefilling.append(self._root)
+        self.stop_token_ids = frozenset(int(t) for t in stop_token_ids)
+        self._free_slots = list(range(batch_size)) if penalty_slots else None
+        self.slot_inits: List[tuple] = []
 
     @property
     def finished(self) -> bool:
@@ -236,6 +295,9 @@ class TextGenScheduler:
                 kv = self._root.kvcache.fork()
                 kv.acquire(n)
             p = _Prefill(idx, prompt, kv)
+            if self._free_slots is not None:
+                p.slot = heapq.heappop(self._free_slots)
+                self.slot_inits.append((p.slot, (self._root.prompt if self._root is not None else []) + prompt))
             self._prefilling.append(p)
             self._new.append((p, 0, n))
             reserve += self._outstanding(p)
@@ -274,8 +336,14 @@ class TextGenScheduler:
         first = [(p.req_idx, 0) for p, s, n in chunks if s + n == len(p.prompt) and p.req_idx >= 0]
         return first + [(r.req_idx, len(r.output)) for r in self.workset]
 
-    def commit(self, next_tokens, t1: float, t2: float) -> int:
-        """next_tokens: one id per row of last_token_rows().  Returns the number of tokens this step processed."""
+    def row_slots(self) -> List[int]:
+        """The penalty-table slot of every row of last_token_rows(), in its order (-1: none)."""
+        chunks = getattr(self, "_new", None) or []
+        return [p.slot for p, s, n in chunks if s + n == len(p.prompt) and p.req_idx >= 0] + [r.slot for r in self.workset]
+
+    def commit(self, next_tokens, t1: float, t2: float, logprobs=None) -> int:
+        """next_tokens: one id per row of last_token_rows(); logprobs: None or (logprob [R], top_ids [R, n], top_logprobs [R, n])
+        for the same rows.  Returns the number of tokens this step processed."""
         completes = [s + n == len(p.prompt) for p, s, n in self._new]
         n_first = sum(c for (p, _, _), c in zip(self._new, completes) if p.req_idx >= 0)
         assert len(next_tokens) == n_first + len(self.workset)
@@ -291,19 +359,31 @@ class TextGenScheduler:
             self._prefilling.remove(p)
             if p.req_idx < 0:                               # the system prompt: cached, no token
                 continue
-            req = RequestContext(p.req_idx, p.kvcache, [int(next_tokens[b])], encode_latency=t2 - p.start_at, decode_start_at=p.start_at)
+            req = RequestContext(p.req_idx, p.kvcache, [int(next_tokens[b])], encode_latency=t2 - p.start_at, decode_start_at=p.start_at,
+                                 slot=p.slot)
+            self._keep_logprobs(req, logprobs, b)
             b += 1
             self._finish_or_continue(req, t2, new_workset)
         for i, req in enumerate(self.workset):
             req.output.append(int(next_tokens[n_first + i]))
+            self._keep_logprobs(req, logprobs, n_first + i)
             self._finish_or_continue(req, t2, new_workset)
         self.workset, self._new, self._admitted = new_workset, [], False
         return processed
 
+    @staticmethod
+    def _keep_logprobs(req, logprobs, row):
+        if logprobs is not None:
+            lp, ids, lps = logprobs
+            req.logprobs.append(float(lp[row]))
+            req.top_logprobs.append(([int(t) for t in ids[row]], [float(x) for x in lps[row]]))
+
     def _finish_or_continue(self, req, t2, new_workset):
-        if len(req.output) >= int(self.rs.output_lens[req.req_idx]):
+        if len(req.output) >= int(self.rs.output_lens[req.req_idx]) or req.output[-1] in self.stop_token_ids:
             req.decode_latency = t2 - req.decode_start_at
             req.kvcache.release()
+            if req.slot >= 0:
+                heapq.heappush(self._free_slots, req.slot)
             self.done.append(req)
             if self._root is not None and self.finished:
                 self._root.kvcache.release()
@@ -313,8 +393,13 @@ class TextGenScheduler:
 
     def result(self, duration: float, steps: int, keep_tokens: bool = False) -> TextGenBenchResult:
         done = sorted(self.done, key=lambda r: r.req_idx)
-        return TextGenBenchResult(np.array([r.encode_latency for r in done]), np.array([r.decode_latency for r in done]),
-                                  duration, steps, [r.output for r in done] if keep_tokens else None)
+        res = TextGenBenchResult(np.array([r.encode_latency for r in done]), np.array([r.decode_latency for r in done]),
+                                 duration, steps, [r.output for r in done] if keep_tokens else None)
+        res.output_lens = np.array([len(r.output) for r in done], dtype=np.int32)
+        if keep_tokens and any(r.logprobs for r in done):
+            res.logprobs = [r.logprobs for r in done]
+            res.top_logprobs = [r.top_logprobs for r in done]
+        return res
 
 
 class _StaticKv:
@@ -348,6 +433,9 @@ class DecodeGraphRunner:
     offset (8-byte aligned: the buffer's base is), with  [keys(2B x u64) | counters(B x u64) | top_k(B) | T(B) | top_p(B)],
     T and top_p as FP32 bit patterns -- still one H2D copy.  `sample_op` (ops.sample_tokens' signature) is the sampler the
     step calls; host-only tests substitute a reference.  Without sampling the buffer is exactly the layout above.
+    When the SamplingParams have penalties, min-p or logprobs (`extended`), it goes on with  [slots(B) | min_p(B) | rep(B) |
+    freq(B) | pres(B)]  (FP32 bit patterns), the step also passes `penalty_table` (set by run_textgen) and, with logprobs, returns
+    (tokens, logprob, top_ids, top_logprobs).  Otherwise the buffer and the step are exactly the above.
 
     capture=False runs the same buffers through the model eagerly (the CPU tests use it; it is also the warm-up path)."""
 
@@ -360,7 +448,14 @@ class DecodeGraphRunner:
             from . import ops
             sample_op = ops.sample_tokens
         self.sample_op = sample_op
+        self.penalty_table = None
         self._entries = {}
+
+    def use_table(self, table):
+        """The penalty table the sampling step reads and updates; graphs captured with another one are dropped."""
+        if table is not self.penalty_table:
+            self.penalty_table = table
+            self._entries = {}
 
     def _layout(self, b, ng=0):
         o_ids, o_indptr, o_last, o_ind = 0, b, 2 * b + 1, 3 * b + 1
@@ -374,12 +469,19 @@ class DecodeGraphRunner:
         o_k = o_ctr + 2 * b
         return o_key, o_ctr, o_k, o_k + b, o_k + 2 * b, o_k + 3 * b
 
+    def _ext_layout(self, b, ng=0):
+        """int32 offsets of slots, min_p, rep, freq, pres and the buffer's total size, with extended sampling."""
+        o = self._sampling_layout(b, ng)[-1]
+        return tuple(o + i * b for i in range(6))
+
     def _entry(self, b, ng):
         e = self._entries.get((b, ng))
         if e is None:
             o_ids, o_indptr, o_last, o_ind, o_grp, total = self._layout(b, ng)
             if self.sampling is not None:
                 total = self._sampling_layout(b, ng)[-1]
+                if self.sampling.extended:
+                    total = self._ext_layout(b, ng)[-1]
             host = torch.zeros(total, dtype=torch.int32)
             if self.device.type == "cuda":
                 host = host.pin_memory()
@@ -396,17 +498,31 @@ class DecodeGraphRunner:
                 o_key, o_ctr, o_k, o_t, o_p, _ = self._sampling_layout(b, ng)
                 e["sample"] = (dev[o_t:o_t + b].view(torch.float32), dev[o_k:o_k + b], dev[o_p:o_p + b].view(torch.float32),
                                dev[o_key:o_ctr].view(torch.int64).view(b, 2), dev[o_ctr:o_k].view(torch.int64))
+                if self.sampling.extended:
+                    sp = self.sampling
+                    o_sl, o_m, o_r, o_f, o_q, _ = self._ext_layout(b, ng)
+                    f32 = lambda o: dev[o:o + b].view(torch.float32)      # noqa: E731
+                    ext = {"min_p": f32(o_m)} if sp.min_p != 0 else {}
+                    if sp.penalties:
+                        ext.update(repetition_penalty=f32(o_r), frequency_penalty=f32(o_f), presence_penalty=f32(o_q),
+                                   penalty_table=self.penalty_table, slots=dev[o_sl:o_sl + b])
+                    if sp.logprobs is not None:
+                        ext["logprobs"] = int(sp.logprobs)
+                    e["ext"] = ext
             self._entries[(b, ng)] = e
         return e
 
     def _step(self, e):
         logits, _ = self.model(e["ids"], e["blen"], None, e["kv"])
         if self.sampling is not None:
-            return self.sample_op(logits, *e["sample"])
+            return self.sample_op(logits, *e["sample"], **e.get("ext", {}))
         return torch.argmax(logits, dim=-1)
 
-    def run(self, last_tokens: List[int], kvs: List[KvCacheInt4], slots: Optional[List[tuple]] = None) -> np.ndarray:
-        """slots: (request index, counter) per sequence, needed with sampling (TextGenScheduler.sample_slots)."""
+    def run(self, last_tokens: List[int], kvs: List[KvCacheInt4], slots: Optional[List[tuple]] = None,
+            row_slots: Optional[List[int]] = None):
+        """slots: (request index, counter) per sequence, needed with sampling (TextGenScheduler.sample_slots); row_slots: the
+        penalty-table slot per sequence, needed with penalties (TextGenScheduler.row_slots).  Returns the tokens, or with
+        logprobs (tokens, logprob, top_ids, top_logprobs), as numpy arrays."""
         b = len(kvs)
         groups = prefix_groups(kvs)
         ng = len(groups)
@@ -442,14 +558,23 @@ class DecodeGraphRunner:
             h[o_k:o_t] = int(sp.top_k)
             h[o_t:o_p] = np.float32(sp.temperature).view(np.int32)
             h[o_p:o_p + b] = np.float32(sp.top_p).view(np.int32)
+            if sp.extended:
+                o_sl, o_m, o_r, o_f, o_q, _ = self._ext_layout(b, ng)
+                h[o_sl:o_m] = row_slots if sp.penalties else -1
+                for o, v in ((o_m, sp.min_p), (o_r, sp.repetition_penalty), (o_f, sp.frequency_penalty), (o_q, sp.presence_penalty)):
+                    h[o:o + b] = np.float32(v).view(np.int32)
         e["dev"].copy_(e["host"], non_blocking=True)
         if not self.capture:
-            return self._step(e).cpu().numpy()
+            return _to_numpy(self._step(e))
         if e["graph"] is None:
             side = torch.cuda.Stream(self.device)
             side.wait_stream(torch.cuda.current_stream(self.device))
             with torch.cuda.stream(side):
+                table = self.penalty_table if self.sampling is not None and self.sampling.penalties else None
+                saved = None if table is None else table.clone()
                 self._step(e)                       # warm-up on real data (lazy initialisations must not be captured)
+                if saved is not None:
+                    table.copy_(saved)              # the warm-up's draw was recorded: the replay below is the step's draw
                 side.synchronize()
                 g = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(g, stream=side):
@@ -457,7 +582,11 @@ class DecodeGraphRunner:
             torch.cuda.current_stream(self.device).wait_stream(side)
             e["graph"] = g
         e["graph"].replay()
-        return e["out"].cpu().numpy()               # synchronises: the caller needs the tokens to go on
+        return _to_numpy(e["out"])                  # synchronises: the caller needs the tokens to go on
+
+
+def _to_numpy(out):
+    return tuple(x.cpu().numpy() for x in out) if isinstance(out, tuple) else out.cpu().numpy()
 
 
 def _vocab_size(model) -> int:
@@ -477,30 +606,52 @@ def pool_capacity(batch_size: int, maxlen: int, block_len: int) -> int:
 @torch.inference_mode()
 def run_textgen(model: Callable, rs: RequestSet, cfg: TextGenConfig, pool: KvPoolInt4, device, sync: Callable = None,
                 keep_tokens: bool = False, progress: Callable = None, decode_runner: DecodeGraphRunner = None,
-                sample_op: Callable = None) -> TextGenBenchResult:
+                sample_op: Callable = None, slot_init_op: Callable = None) -> TextGenBenchResult:
     """Drive `model(input_ids, blen, prefill_kv, decode_kv) -> (logits, hidden)` through the whole request set.
     Latencies are wall-clock around the step *including* the device->host read of the next tokens (which synchronises),
     as in the reference.  With a `decode_runner`, steps that carry no prompt tokens are replayed from its CUDA graphs.
     cfg.prefill_chunk, cfg.shared_prefix: see TextGenScheduler.  cfg.sampling: the eager steps call `sample_op` (default
     ops.sample_tokens) on the rows whose logits are needed, with each row's key (seed, request) and counter; the runner, which
-    must have been built with the same SamplingParams, samples in its graphs."""
+    must have been built with the same SamplingParams, samples in its graphs.  With penalties a penalty table of
+    cfg.batch_size slots is made on `device` (ops.penalty_table) and each admitted request's slot is set up by `slot_init_op`
+    (default ops.init_penalty_slot) before its first token; the runner is given the same table.  cfg.stop_token_ids: see
+    TextGenScheduler."""
     sp = cfg.sampling
     if sp is not None and sample_op is None:
         from . import ops
         sample_op = ops.sample_tokens
     if decode_runner is not None and decode_runner.sampling != sp:
         raise ValueError("decode_runner was built for other sampling parameters than cfg.sampling")
-    sched = TextGenScheduler(rs, cfg.batch_size, pool, device, vocab_size=_vocab_size(model), prefill_chunk=cfg.prefill_chunk,
-                             shared_prefix=cfg.shared_prefix)
+    vocab = _vocab_size(model)
+    table = None
+    if sp is not None and sp.penalties:
+        from . import ops
+        table = ops.penalty_table(cfg.batch_size, vocab, device)
+        old = None if decode_runner is None else decode_runner.penalty_table
+        if old is not None and old.shape == table.shape and old.device == table.device:
+            table = old                     # its graphs stay valid; every slot is set up again at admission
+        if slot_init_op is None:
+            slot_init_op = ops.init_penalty_slot
+        if decode_runner is not None:
+            decode_runner.use_table(table)
+    sched = TextGenScheduler(rs, cfg.batch_size, pool, device, vocab_size=vocab, prefill_chunk=cfg.prefill_chunk,
+                             shared_prefix=cfg.shared_prefix, stop_token_ids=cfg.stop_token_ids, penalty_slots=table is not None)
     steps = graphed = peak = 0
     t_start = time.perf_counter()
     while not sched.finished:
         sched.admit()
+        for slot, prompt in sched.slot_inits:
+            slot_init_op(table, slot, prompt)
+        sched.slot_inits.clear()
         peak = max(peak, pool.capacity - pool.num_free_blocks)
         t1 = time.perf_counter()
+        logprobs = None
         if decode_runner is not None and sched.prompt_tokens == 0:
             next_tokens = decode_runner.run([int(r.output[-1]) for r in sched.workset], [r.kvcache for r in sched.workset],
-                                            sched.sample_slots() if sp is not None else None)
+                                            sched.sample_slots() if sp is not None else None,
+                                            sched.row_slots() if table is not None else None)
+            if isinstance(next_tokens, tuple):
+                next_tokens, logprobs = next_tokens[0], next_tokens[1:]
             graphed += 1
         else:
             batch = sched.next_batch()
@@ -512,12 +663,17 @@ def run_textgen(model: Callable, rs: RequestSet, cfg: TextGenConfig, pool: KvPoo
             else:
                 slots = sched.sample_slots()
                 n = len(slots)
-                next_tokens = sample_op(logits.index_select(0, rows), [sp.temperature] * n, [sp.top_k] * n, [sp.top_p] * n,
-                                        [(int(sp.seed), r) for r, _ in slots], [c for _, c in slots]).cpu().numpy()
+                args = (logits.index_select(0, rows), [sp.temperature] * n, [sp.top_k] * n, [sp.top_p] * n,
+                        [(int(sp.seed), r) for r, _ in slots], [c for _, c in slots])
+                if not sp.extended:
+                    next_tokens = sample_op(*args).cpu().numpy()
+                else:
+                    out = _to_numpy(sample_op(*args, **sp.options(n, table, sched.row_slots())))
+                    next_tokens, logprobs = (out[0], out[1:]) if isinstance(out, tuple) else (out, None)
         if sync is not None:
             sync()
         t2 = time.perf_counter()
-        n = sched.commit(next_tokens, t1, t2)
+        n = sched.commit(next_tokens, t1, t2) if logprobs is None else sched.commit(next_tokens, t1, t2, logprobs)
         steps += 1
         if progress is not None:
             progress(n)
@@ -529,17 +685,22 @@ def run_textgen(model: Callable, rs: RequestSet, cfg: TextGenConfig, pool: KvPoo
 
 def report(rs: RequestSet, cfg: TextGenConfig, res: TextGenBenchResult) -> dict:
     """The figures bench_textgen.py:509-528 prints, as a dict (throughput = (prompt + new tokens) / duration; the shared system
-    prompt's tokens are not counted), plus the peak of KV pages in use."""
+    prompt's tokens are not counted), plus the peak of KV pages in use.  New tokens are those each request generated: the
+    request set's output lengths, unless a stop id ended a request early."""
+    gen = rs.output_lens if res.output_lens is None else res.output_lens
     per_prompt_tok = res.encode_latency / rs.prompt_lens
-    per_new_tok = res.decode_latency / rs.output_lens
-    total = int(rs.prompt_lens.sum()) + int(rs.output_lens.sum())
-    return {
+    per_new_tok = res.decode_latency / gen
+    total = int(rs.prompt_lens.sum()) + int(gen.sum())
+    out = {
         "num_requests": len(rs), "batch_size": cfg.batch_size, "steps": res.steps, "graphed_decode_steps": res.graphed_steps,
         "encode_latency_ms_per_request": [float(res.encode_latency.mean() * 1e3), float(res.encode_latency.std() * 1e3)],
         "encode_latency_ms_per_token": [float(per_prompt_tok.mean() * 1e3), float(per_prompt_tok.std() * 1e3)],
         "decode_latency_ms_per_token": [float(per_new_tok.mean() * 1e3), float(per_new_tok.std() * 1e3)],
-        "total_prompt_tokens": int(rs.prompt_lens.sum()), "total_new_tokens": int(rs.output_lens.sum()),
+        "total_prompt_tokens": int(rs.prompt_lens.sum()), "total_new_tokens": int(gen.sum()),
         "duration_s": res.duration, "throughput_tokens_per_s": total / res.duration, "peak_kv_pages_in_use": res.peak_pages,
         "shared_prefix": cfg.shared_prefix,
-        "sampling": None if cfg.sampling is None else dataclasses.asdict(cfg.sampling),
+        "sampling": None if cfg.sampling is None else cfg.sampling.asdict(),
     }
+    if cfg.stop_token_ids:
+        out["stop_token_ids"] = [int(t) for t in cfg.stop_token_ids]
+    return out

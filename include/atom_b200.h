@@ -337,6 +337,42 @@ ATOM_API int atom_moe_combine_f16(const void* y, const void* topk_ids, const voi
 ATOM_API int atom_sample_f16(const void* logits, int64_t ld, int batch, int vocab, const void* temperature, const void* top_k,
                              const void* top_p, const void* key, const void* counter, void* out, void* stream);
 
+/* atom_sample_ex_f16: atom_sample_f16 with penalties, min-p and log-probabilities (new: the reference only takes the argmax).
+ * The arguments of atom_sample_f16, plus, all read on the device after the preceding kernel has completed:
+ *   min_p f32 [batch] or null (off);
+ *   rep, freq, pres f32 [batch], slots i32 [batch], table u16 [*][table_ld >= vocab]: all null (no penalties) or all given;
+ *   logprob_out f32 [batch] or null; top_n in [0, 20]; top_ids i32 [batch][top_n], top_logprobs f32 [batch][top_n].
+ * Penalty state: row b names a slot s = slots[b] of the table, or -1 (none).  An entry holds bit 15 = the token occurs in the
+ * request's prompt (a shared system prompt included) and bits 0-14 = how often the request has generated it, saturating at
+ * 0x7FFF.  Slots in one call must be distinct.
+ * Penalised logit, per token of a row with a slot, from its FP16 value l, each step one IEEE FP32 operation:
+ *   1. -inf stays -inf;
+ *   2. repetition r, if the token is in the prompt or its count c > 0:  l = l > 0 ? fl(l / r) : fl(l * r);
+ *   3. frequency f:  l = fl(l - fl(c * f));
+ *   4. presence p, if c > 0:  l = fl(l - p);
+ *   5. l' = FP16 round-to-nearest of min(max(l, -65504), 65504) (fmin / fmax: a NaN from inf - inf becomes -65504).
+ * Rules 1-5 of atom_sample_f16 then apply to l' instead of the raw logits; the NaN / +inf / all -inf test of rule 1 is still made
+ * on the raw row.  Also:
+ *   - min-p m in [0, 1], after top-k and before top-p: keep the survivors whose weight W_i >= ceil(m * 2^40) (the top token's
+ *     weight is exactly 2^40); top-p then works over what is left.  m = 0 is off.
+ *   - Log-probabilities: a log-softmax of l' at temperature 1 over the whole row (independent of T, top-k, top-p and min-p):
+ *     lp_i = (fl(l'_i - max l') - ln(Z1 * 2^-40)) in double, rounded to FP32, Z1 = sum over the row of
+ *     round(expf(l'_j - max) * 2^40), exact.  logprob_out[b] is the chosen token's lp; top_ids / top_logprobs the first top_n
+ *     tokens of the order on l' with theirs, padded with id -1 and lp -inf past the finite tokens.  An invalid row (token -1)
+ *     gives lp NaN, ids -1 and top lps NaN.
+ *   - Recording: with a slot and a token, the kernel adds one to the token's count in the slot, saturating, in the same launch.
+ *   - Parameters out of range give -1, as in rule 1: also r not finite or <= 0, f or p not finite, m not in [0, 1].
+ * With no table, no min_p, no logprob_out and top_n = 0 this is atom_sample_f16. */
+ATOM_API int atom_sample_ex_f16(const void* logits, int64_t ld, int batch, int vocab, const void* temperature, const void* top_k,
+                                const void* top_p, const void* key, const void* counter, const void* min_p, const void* rep,
+                                const void* freq, const void* pres, const void* slots, void* table, int64_t table_ld, void* out,
+                                void* logprob_out, int top_n, void* top_ids, void* top_logprobs, void* stream);
+
+/* atom_sample_slot_init: set up slot `slot` of a penalty table u16 [*][table_ld] (16-byte aligned, table_ld >= vocab a multiple
+ * of 8) for a new request in one launch: zero the row, then set bit 15 of every token in prompt i32 [prompt_len] (ids outside
+ * [0, vocab) are ignored). */
+ATOM_API int atom_sample_slot_init(void* table, int64_t table_ld, int vocab, int slot, const void* prompt, int prompt_len, void* stream);
+
 /* replaces append_kv_i4 (punica_ops.cc:166-209 -> FlashInferAppendKvKernel_i4<128>, flashinfer_impl.cuh:73-96)
  *   k,v u8 [B,H,64]  k_param,v_param f16 [B,H,2] */
 ATOM_API int atom_append_kv_i4(void* kv_data, void* kv_param, const void* kv_indptr, const void* kv_indices,

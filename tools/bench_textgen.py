@@ -56,6 +56,14 @@ def main():
     ap.add_argument("--top-k", type=int, default=0, help="with sampling: keep the k largest logits (0 = off)")
     ap.add_argument("--top-p", type=float, default=1.0, help="with sampling: keep the smallest set of mass >= p (1 = off)")
     ap.add_argument("--seed", type=int, default=0, help="with sampling: request r draws from the Philox key (seed, r)")
+    ap.add_argument("--min-p", type=float, default=0.0, help="with sampling: drop tokens below m times the top one's weight (0 = off)")
+    ap.add_argument("--repetition-penalty", type=float, default=1.0, help="with sampling: on prompt and generated tokens (1 = off)")
+    ap.add_argument("--frequency-penalty", type=float, default=0.0, help="with sampling: times a token's count (0 = off)")
+    ap.add_argument("--presence-penalty", type=float, default=0.0, help="with sampling: on generated tokens (0 = off)")
+    ap.add_argument("--logprobs", type=int, default=None, metavar="N",
+                    help="with sampling: each token's log-probability and the top N (0 to 20)")
+    ap.add_argument("--stop-token", type=int, action="append", default=[], metavar="ID",
+                    help="a request that emits this id finishes on it (repeatable)")
     ap.add_argument("--warmup-batches", type=int, default=1,
                     help="untimed request batches served first (first-use costs: lazy kernel loading, attribute calls, graph "
                          "capture); 0 = time the cold process like the reference's script")
@@ -71,8 +79,13 @@ def main():
     rs = tg.generate_request_set(args.batch_size * args.num_batches, args.maxlen)
     if args.temperature is None and (args.top_k or args.top_p != 1.0):
         ap.error("--top-k / --top-p need --temperature")
-    sampling = None if args.temperature is None else tg.SamplingParams(args.temperature, args.top_k, args.top_p, args.seed)
-    cfg = tg.TextGenConfig(args.batch_size, prefill_chunk=args.prefill_chunk, shared_prefix=args.shared_prefix, sampling=sampling)
+    extra = dict(min_p=args.min_p, repetition_penalty=args.repetition_penalty, frequency_penalty=args.frequency_penalty,
+                 presence_penalty=args.presence_penalty, logprobs=args.logprobs)
+    if args.temperature is None and tg.SamplingParams(1.0, **extra).extended:
+        ap.error("--min-p, the penalties and --logprobs need --temperature")
+    sampling = None if args.temperature is None else tg.SamplingParams(args.temperature, args.top_k, args.top_p, args.seed, **extra)
+    cfg = tg.TextGenConfig(args.batch_size, prefill_chunk=args.prefill_chunk, shared_prefix=args.shared_prefix, sampling=sampling,
+                           stop_token_ids=tuple(args.stop_token))
     shared_pages = -(-args.shared_prefix // args.block_len)           # the system prompt's pages, held once
     pool = KvPoolInt4(layers, mc.kv_heads, mc.hidden_size // mc.num_heads,     # the cache holds KV heads (grouped-query: fewer)
                       tg.pool_capacity(args.batch_size, args.maxlen, args.block_len) + shared_pages + args.batch_size * (shared_pages > 0),

@@ -4,6 +4,11 @@ top-k mask, softmax at T, cumulative sum, top-p mask, inverse CDF in index order
 GEMM that produces the logits (hidden 4096).  Needs a GPU; there is no CPU path.
 
     python tools/sample_bench.py [--batch 1 16 32 64] [--vocab 32000 128256] [--out result.json]
+    python tools/sample_bench.py --features [--batch 1 32 256] [--vocab 32000 128256]
+
+--features times the plain call (T = 0.8, top-p 0.9) against the same call with each option of atom_sample_ex_f16 added, one
+at a time and all together: +penalties (every row with a slot of a table holding prompt bits and counts), +min-p 0.05,
++logprobs with n = 0 and n = 20, and all of them; same method, all variants alternated in one run.
 
 Method (that of tools/decode_attn_bench.py): for every shape each variant is captured into one CUDA graph holding one call per
 logits set; the sets are distinct buffers that together cover at least 256 MB where that takes at most 256 sets (the H100's L2
@@ -74,6 +79,53 @@ def timed(g):
     return a.elapsed_time(b) * 1e3
 
 
+FEATURES = {"plain": {}, "+penalties": {"pen": True}, "+min-p": {"min_p": 0.05}, "+logprobs n=0": {"logprobs": 0},
+            "+logprobs n=20": {"logprobs": 20}, "all": {"pen": True, "min_p": 0.05, "logprobs": 20}}
+
+
+def features(args, dev, name, limit):
+    gen = torch.Generator(device=dev).manual_seed(1)
+    rows = []
+    for V in args.vocab:
+        for B in args.batch:
+            nbytes = 2 * B * V
+            nsets = max(4, min(256, -(-L2_SWEEP_BYTES // nbytes)))
+            sets = [(torch.randn((B, V), device=dev, generator=gen) * 4).half() for _ in range(nsets)]
+            prm = [torch.full((B,), 0.8, dtype=torch.float32, device=dev), torch.zeros(B, dtype=torch.int32, device=dev),
+                   torch.full((B,), 0.9, dtype=torch.float32, device=dev),
+                   torch.stack([torch.zeros(B, dtype=torch.int64, device=dev), torch.arange(B, device=dev)], 1),
+                   torch.arange(B, dtype=torch.int64, device=dev)]
+            table = ops.penalty_table(B, V, dev)
+            table[:, :V] = torch.where(torch.rand((B, V), device=dev, generator=gen) < 0.02, -0x8000, 0).short()
+            table[:, :V] += torch.where(torch.rand((B, V), device=dev, generator=gen) < 0.01, 3, 0).short()
+            full = lambda x: torch.full((B,), x, dtype=torch.float32, device=dev)     # noqa: E731
+            pen = dict(repetition_penalty=full(1.2), frequency_penalty=full(0.3), presence_penalty=full(0.4), penalty_table=table,
+                       slots=torch.arange(B, dtype=torch.int32, device=dev))
+
+            def call(f):
+                kw = dict(pen) if f.get("pen") else {}
+                if "min_p" in f:
+                    kw["min_p"] = full(f["min_p"])
+                if "logprobs" in f:
+                    kw["logprobs"] = f["logprobs"]
+                return lambda l: ops.sample_tokens(l, *prm, **kw)
+            variants = {t: capture(call(f), sets) for t, f in FEATURES.items()}
+            for g in variants.values():
+                for _ in range(3):
+                    g.replay()
+            torch.cuda.synchronize()
+            ts = {t: [] for t in variants}
+            for _ in range(args.reps):
+                for t, g in variants.items():
+                    ts[t].append(timed(g) / nsets)
+            med = {t: statistics.median(v) for t, v in ts.items()}
+            r = {"B": B, "V": V, "sets": nsets, **{f"{t}_us": round(m, 2) for t, m in med.items()}, "card": name, "power_limit": limit}
+            rows.append(r)
+            print(f"B={B:3d} V={V:6d} " + "  ".join(f"{t} {m:7.2f}" for t, m in med.items()) + " us", flush=True)
+            del sets, table
+    return rows
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, nargs="+", default=[1, 16, 32, 64])
@@ -81,12 +133,20 @@ def main():
     ap.add_argument("--hidden", type=int, default=4096)
     ap.add_argument("--reps", type=int, default=15)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--features", action="store_true", help="time each option of atom_sample_ex_f16 against the plain call")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("sample_bench: needs a CUDA device")
     dev = torch.device("cuda:0")
     name, limit = card()
     print(f"card: {name}, power limit {limit}; share of peak against the data sheet's 3.35 TB/s")
+    if args.features:
+        rows = features(args, dev, name, limit)
+        if args.out:
+            with open(args.out, "w") as f:
+                json.dump(rows, f, indent=1)
+        print(json.dumps({"rows": len(rows), "card": name, "power_limit": limit}))
+        return
     gen = torch.Generator(device=dev).manual_seed(0)
     rows = []
     for V in args.vocab:
