@@ -33,6 +33,8 @@ _SIGNATURES = {
     "atom_decode_kv_split": (_I, [_I] * 4),
     "atom_batch_decode_shared_gqa_i4": (_I, [_P] * 7 + [_I] * 6 + [_F] + [_P] * 3 + [_I] * 2 + [_P] * 2 + [_I, _P]),
     "atom_decode_shared_chunks": (_I, [_I] * 5),
+    "atom_batch_verify_gqa_i4": (_I, [_P] * 7 + [_I] * 7 + [_F] + [_P] * 2 + [_I, _P]),
+    "atom_verify_chunks": (_I, [_I] * 3),
     "atom_prefill_attention_i4": (_I, [_P] * 11 + [_I] * 4 + [_P]),
     "atom_prefill_attention_gqa_i4": (_I, [_P] * 11 + [_I] * 5 + [_P]),
     "atom_prefill_attention_ctx_gqa_i4": (_I, [_P] * 11 + [_I] * 5 + [_P] * 5 + [_I] * 3 + [_P]),

@@ -24,6 +24,7 @@
 #include "kv_kernels.cuh"
 #include "prefill_kernels.cuh"
 #include "cascade_kernels.cuh"
+#include "verify_kernels.cuh"
 #include "comm_kernels.cuh"
 #include "quant_kernels.cuh"
 #include "moe_kernels.cuh"
@@ -819,6 +820,48 @@ int atom_batch_decode_shared_gqa_i4(void* o, const void* q, const void* kv_data,
   if (group == 2) return launch_decode_shared<2>(what, o, q, kv, px, log2_theta, st);
   if (group == 4) return launch_decode_shared<4>(what, o, q, kv, px, log2_theta, st);
   return launch_decode_shared<8>(what, o, q, kv, px, log2_theta, st);
+}
+
+// Verify chunk rule: an unsplit grid that already gives every SM a CTA is kept; a smaller one is cut into the fewest chunks that
+// give the verify kernel two CTAs per SM (its occupancy), 64 at most.  Host-known sizes only, as atom_decode_kv_split.
+int atom_verify_chunks(int batch, int num_kv_heads, int sm_count) {
+  ATOM_REQUIRE(batch > 0 && num_kv_heads > 0 && sm_count > 0, "verify_chunks: batch=%d num_kv_heads=%d sm_count=%d must be positive",
+               batch, num_kv_heads, sm_count);
+  const long long ctas = (long long)batch * num_kv_heads;
+  if (ctas >= sm_count) return 1;
+  return (int)std::min<long long>(64, (2LL * sm_count + ctas - 1) / ctas);
+}
+
+int atom_batch_verify_gqa_i4(void* o, const void* q, const void* kv_data, const void* kv_param, const void* kv_indptr,
+                             const void* kv_indices, const void* last_page_offset, int num_layers, int layer_idx, int num_q_heads,
+                             int num_kv_heads, int page_size, int batch_size, int tokens_per_seq, float rope_theta,
+                             const void* rope_table, float* workspace, int nchunks, void* stream) {
+  const char* what = "batch_verify_gqa_i4";
+  int rc = kv_check(what, kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx, num_kv_heads, page_size,
+                    batch_size);
+  if (rc) return rc;
+  ATOM_REQUIRE(o && q && rope_table, "%s: null pointer argument", what);
+  ATOM_REQUIRE(num_q_heads > 0 && num_q_heads % num_kv_heads == 0,
+               "%s: num_q_heads=%d must be a positive multiple of num_kv_heads=%d", what, num_q_heads, num_kv_heads);
+  ATOM_REQUIRE(rope_theta > 1.f && rope_theta < 1e30f, "%s: rope_theta=%g must be a finite base above 1", what, (double)rope_theta);
+  const int group = num_q_heads / num_kv_heads;
+  if (group != 1 && group != 2 && group != 4 && group != 8)
+    return fail(ATOM_E_UNSUPPORTED, "%s: %d query heads per KV head (num_q_heads=%d, num_kv_heads=%d); supported group sizes are 1, 2, "
+                                    "4 and 8", what, group, num_q_heads, num_kv_heads);
+  ATOM_REQUIRE(tokens_per_seq >= 1 && tokens_per_seq <= 8, "%s: tokens_per_seq=%d must be in [1, 8]", what, tokens_per_seq);
+  ATOM_REQUIRE(page_size % 8 == 0 && page_size <= 64, "%s: page_size=%d must be a multiple of 8, at most 64", what, page_size);
+  ATOM_REQUIRE(nchunks >= 1 && nchunks <= 64 && (nchunks == 1 || workspace), "%s: nchunks=%d must be in [1, 64], with a workspace above 1",
+               what, nchunks);
+  ATOM_REQUIRE(aligned16(kv_data) && aligned16(kv_param) && aligned16(rope_table) && aligned16(workspace),
+               "%s: KV pool, rope table and workspace must be 16-byte aligned", what);
+  const atom::KvArgs kv{(uint8_t*)kv_data, (__half2*)kv_param, (const int32_t*)kv_indptr, (const int32_t*)kv_indices,
+                        (const int32_t*)last_page_offset, num_layers, layer_idx, num_kv_heads, page_size, batch_size};
+  const cudaStream_t st = (cudaStream_t)stream;
+  rc = launch_k(what, atom::verify_attn_kernel, dim3(nchunks, num_kv_heads, batch_size), dim3(atom::PF_THREADS), 0, st, (__half*)o,
+                (const __half*)q, kv, (const float2*)rope_table, log2f(rope_theta), tokens_per_seq, group, workspace, nchunks);
+  if (rc || nchunks == 1) return rc;
+  return launch_k("batch_verify_gqa_i4 (merge)", atom::verify_merge_kernel, dim3(batch_size * tokens_per_seq, num_q_heads), dim3(128), 0,
+                  st, (__half*)o, (const float*)workspace, kv, tokens_per_seq, num_q_heads, nchunks);
 }
 
 int atom_append_kv_i4(void* kv_data, void* kv_param, const void* kv_indptr, const void* kv_indices,

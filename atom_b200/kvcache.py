@@ -134,6 +134,25 @@ class KvCacheInt4:
             raise ValueError("acquire: n must be non-negative")
         self._grow_to(self._seqlen + int(n))
 
+    def truncate(self, n: int) -> List[int]:
+        """Drop the tokens past the first n (the rejected drafts of a verify step) and return the pages that no longer hold one
+        of this sequence's tokens; this sequence's hold on each is given back to the pool.  The bytes past n stay as they are
+        and are overwritten by the next write, as any slot past the length.  Refuses to leave the length inside a shared page:
+        the next token would be written into it."""
+        n = int(n)
+        if not 0 <= n <= self._seqlen:
+            raise ValueError(f"truncate: n={n} outside [0, {self._seqlen}]")
+        P = self._pool.block_len
+        keep = -(-n // P)
+        if n % P and n < self._seqlen and self._pool.refcount(self._pages[keep - 1]) > 1:
+            raise ValueError(f"truncate: n={n} cuts into shared page {self._pages[keep - 1]}")
+        dropped = self._pages[keep:]
+        del self._pages[keep:]
+        for page in reversed(dropped):
+            self._pool.free_block(page)
+        self._seqlen = n
+        return dropped
+
     def fork(self, n=None) -> "KvCacheInt4":
         """A new sequence holding this one's first `n` tokens (default: all).  It shares the full pages among them; a partly
         filled last page is copied, every layer and K/V block, into a fresh page of its own (one device copy on the current

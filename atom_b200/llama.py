@@ -237,7 +237,20 @@ class LlamaAttention(nn.Module):
                                                   v_proj[0][:blen.doff], v_proj[1][:blen.doff], blen.indptr, seqlens=list(blen.prefills),
                                                   rope_theta=self.rope_theta, **ctx))
             nvtx.range_pop()
-        if blen.decode > 0:
+        if blen.decode > 0 and getattr(blen, "decode_len", 1) > 1:
+            # a verify step: every sequence carries S tokens, written to the cache at stride S and attended together
+            S, n = blen.decode_len, blen.decode * blen.decode_len
+            nvtx.range_push("init_kv")
+            assert decode_kv is not None
+            ops.init_kv_i4(decode_kv, k_proj[0][blen.doff:].view(n, nh, hd // 2), v_proj[0][blen.doff:].view(n, nh, hd // 2),
+                           k_proj[1][blen.doff:].view(n, nh, hd // 128 * 2), v_proj[1][blen.doff:].view(n, nh, hd // 128 * 2),
+                           blen.decode_indptr, self.layer_idx)
+            nvtx.range_pop()
+            nvtx.range_push("batch_verify")
+            stack.append(ops.batch_verify_i4(q_proj[blen.doff:].view(n, nq, hd), decode_kv, self.layer_idx, S, rope_theta=self.rope_theta,
+                                             max_len=blen.max_len).view(n, self.hidden_size))
+            nvtx.range_pop()
+        elif blen.decode > 0:
             q = q_proj[blen.doff:].view(blen.decode, nq, hd)
             k = k_proj[0][blen.doff:].view(blen.decode, nh, hd // 2)
             v = v_proj[0][blen.doff:].view(blen.decode, nh, hd // 2)

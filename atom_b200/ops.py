@@ -359,6 +359,54 @@ def _batch_decode_shared(o, q, kv, groups, L, H, P, layer_idx, rope_theta, sms):
     return o
 
 
+def verify_chunks(batch, num_kv_heads, device=None):
+    """The chunk count `batch_verify_i4(..., nchunks=0)` uses for `batch` sequences of `num_kv_heads` KV heads on `device`
+    (default: the current CUDA device): 1 when the (sequence, KV head) grid already gives every SM a CTA."""
+    dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    c = _lib.lib().atom_verify_chunks(int(batch), int(num_kv_heads), int(sms))
+    _lib.check(min(c, 0), "verify_chunks")
+    return c
+
+
+def batch_verify_i4(q, kv, layer_idx, tokens_per_seq, rope_theta=10000.0, max_len=None, nchunks=0):
+    """EXTENSION (speculative decoding): multi-token decode attention of a verify step.  Sequence b of `kv` ends with S =
+    `tokens_per_seq` query tokens (1 <= S <= 8) whose K/V are already in the pages (init_kv_i4 with a stride-S indptr), at
+    positions len_b - S .. len_b - 1; token i attends to every cached token before the tail and, causally, to the tail up to
+    itself.  q f16 [B*S, Hq, 128], sequence-major and token-minor (row b*S + i); returns the same shape.  Query head counts per
+    KV head of 1, 2, 4 or 8, as batch_decode_i4.  Positions come from the page table on the device; `max_len` bounds every
+    sequence's length and sizes the RoPE table (a CUDA graph captured with a bound replays as lengths grow up to it); without it
+    the bound is read from `kv.seqlens` (a BatchedKvCacheInt4).  nchunks: 0 = automatic (`verify_chunks`), n = cut each
+    sequence's tiles into n runs merged in order (1 = unsplit)."""
+    _req_width("batch_verify_i4", f16_q_2=q)
+    _req_cuda(q, kv.data, kv.param, kv.indptr, kv.indicies, kv.last_page_offset)
+    L, H, P = _kv_dims(kv)
+    S = int(tokens_per_seq)
+    if not 1 <= S <= 8:
+        raise RuntimeError(f"batch_verify_i4: tokens_per_seq={S} must be in [1, 8]")
+    B = kv.last_page_offset.size(0)
+    if q.dim() != 3 or q.size(2) != 128 or q.size(0) != B * S or kv.indptr.size(0) != B + 1:
+        raise RuntimeError(f"batch_verify_i4: q {tuple(q.shape)} does not hold {S} tokens of 128 per head for each of {B} sequences")
+    if max_len is None:
+        lens = getattr(kv, "seqlens", None)
+        if lens is None:
+            raise RuntimeError("batch_verify_i4: pass `max_len` or a `kv` with host sequence lengths (`seqlens`)")
+        if min(lens) < S:
+            raise RuntimeError(f"batch_verify_i4: a sequence holds {min(lens)} tokens, fewer than its {S} query tokens")
+        max_len = max(lens)
+    hq = q.size(1)
+    nchunks = int(nchunks) if nchunks else verify_chunks(B, H, q.device)
+    ws = torch.empty((B * S, hq, nchunks, 130), dtype=torch.float32, device=q.device) if nchunks > 1 else None
+    table = rope_table(max_len, q.device, rope_theta)
+    o = torch.empty_like(q)
+    with torch.cuda.device(q.device):
+        _lib.check(_lib.lib().atom_batch_verify_gqa_i4(
+            o.data_ptr(), q.data_ptr(), kv.data.data_ptr(), kv.param.data_ptr(), kv.indptr.data_ptr(), kv.indicies.data_ptr(),
+            kv.last_page_offset.data_ptr(), L, int(layer_idx), hq, H, P, B, S, float(rope_theta), table.data_ptr(),
+            None if ws is None else ws.data_ptr(), nchunks, _stream(q)), "batch_verify_i4")
+    return o
+
+
 _rope_tables = {}
 
 

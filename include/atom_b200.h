@@ -203,6 +203,26 @@ ATOM_API int atom_batch_decode_shared_gqa_i4(void* o, const void* q, const void*
  * of whole 64-token tiles, short prefixes leave some empty).  Returns the count, or ATOM_E_INVALID for non-positive sizes. */
 ATOM_API int atom_decode_shared_chunks(int num_groups, int batch, int group, int num_kv_heads, int sm_count);
 
+/* EXTENSION (speculative decoding): multi-token decode attention for a verify step.  Sequence b of the cache ends with
+ * tokens_per_seq = S query tokens (1 <= S <= 8) at positions len_b - S .. len_b - 1 whose K/V are already in the pages; token i
+ * attends to every key at a position <= len_b - S + i.  q, o f16 [batch_size * S, num_q_heads, 128], row b * S + i = token i of
+ * sequence b.  One launch (two when nchunks > 1): each (chunk, KV head, sequence) CTA streams its share of the sequence's pages
+ * once for all S x G query rows of that KV head, on tensor cores.  Positions come from the page table on the device.
+ *   rope_table f32 [>= max_b len_b, 64, 2] as for atom_prefill_attention_i4 with base rope_theta; workspace f32 [batch_size * S,
+ *   num_q_heads, nchunks, 130] (may be NULL when nchunks == 1); nchunks from atom_verify_chunks.
+ * Precondition: len_b >= S for every sequence (the device holds the lengths, so it is not checked on the host); the rows of a
+ * sequence that breaks it are zeros, and none of its pages is read.
+ * Everything else as atom_batch_decode_gqa_i4.  Deterministic: the result depends on nchunks, never on where the pages sit. */
+ATOM_API int atom_batch_verify_gqa_i4(void* o, const void* q, const void* kv_data, const void* kv_param, const void* kv_indptr,
+                                      const void* kv_indices, const void* last_page_offset, int num_layers, int layer_idx,
+                                      int num_q_heads, int num_kv_heads, int page_size, int batch_size, int tokens_per_seq,
+                                      float rope_theta, const void* rope_table, float* workspace, int nchunks, void* stream);
+
+/* The chunk count of atom_batch_verify_gqa_i4: 1 when batch * num_kv_heads >= sm_count, otherwise the fewest chunks with which
+ * batch x num_kv_heads x chunks reaches 2 * sm_count CTAs, 64 at most (a sequence's 64-token tiles are cut into that many runs;
+ * short sequences leave some empty).  Returns the count, or ATOM_E_INVALID for non-positive sizes. */
+ATOM_API int atom_verify_chunks(int batch, int num_kv_heads, int sm_count);
+
 /* EXTENSION (SURVEY.md 8 f3): the prefill attention the reference leaves as a placeholder
  * (punica/models/llama.py:171-190, SDPA over torch.randn K/V): causal attention of every prompt over its own just-quantised
  * K/V -- the o4 outputs of the k/v projections, x = nibble * scale - zero (quantization.cuh:76) -- with RoPE(theta 1e4) on q
