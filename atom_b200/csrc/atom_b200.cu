@@ -251,6 +251,15 @@ int gemm_dispatch(const GemmOperands& op, const atom::GemmArgs& args, uint32_t f
       }
     }
   }
+  // A split 16-token tile whose every rank holds at most PACK INT4 groups keeps its K slice resident (EPI_RESIDENT).
+  if constexpr (kEpi == atom::EPI_O16 || kEpi == atom::EPI_PUSH) {
+    constexpr int kRes = kEpi | atom::EPI_RESIDENT;
+    if (bn == 16 && ksplit > 1 && (groups + ksplit - 1) / ksplit <= atom::GemmCfg<16, 2, kRes>::PACK) {
+      if (ksplit == 8) return launch_gemm<16, 8, kRes>(op, args, stream, out_channels);
+      if (ksplit == 4) return launch_gemm<16, 4, kRes>(op, args, stream, out_channels);
+      return launch_gemm<16, 2, kRes>(op, args, stream, out_channels);
+    }
+  }
 #define ATOM_BN(BN_)                                                                                  \
   do {                                                                                                \
     if constexpr (kEpi == atom::EPI_O16 || kEpi == atom::EPI_PUSH) {                                  \
@@ -297,6 +306,7 @@ int gemm_common(const void* a, const void* b, const void* a_scale, const void* b
   args.d = o4 ? nullptr : (__half*)d; args.d4 = o4 ? (uint8_t*)d : nullptr; args.d_scale = (__half2*)d_scale;
   args.M = (int)M; args.N = (int)N; args.G = (int)(K / 128 - 1); args.lda_scale = atom::scale_size((int)M); args.trace = g_trace;
   args.ldb_scale = (int)N;
+  args.a4 = (const uint8_t*)a; args.a8 = (const uint8_t*)a_keeper;
   if (ar != nullptr) { args.ar = *ar; return gemm_dispatch<atom::EPI_PUSH>(op, args, flags, (cudaStream_t)stream); }
   return o4 ? gemm_dispatch<atom::EPI_O4>(op, args, flags, (cudaStream_t)stream) : gemm_dispatch<atom::EPI_O16>(op, args, flags, (cudaStream_t)stream);
 }

@@ -52,6 +52,9 @@ struct GemmArgs {
   // (valid rows 0 = empty); the weights of all experts are stacked, `expert_rows` rows per expert (2I gate/up, H down)
   const int4* tiles;
   int expert_rows;
+  // EPI_RESIDENT: the packed INT4 tokens [M][G * 64] and the INT8 keeper tokens [M][128] (tm_a4 / tm_a8), read with L2 loads
+  const uint8_t* a4;
+  const uint8_t* a8;
 };
 
 // timeline stamps for pipeline debugging (tools/gemm_phase_trace.py), 128 clock64 slots per CTA:
@@ -62,6 +65,8 @@ struct GemmArgs {
 //   producer thread 0:  0 pack_full passed | 3 exp_full (token tile widened)
 //   scale warp, lane 0: 1 scale slot free (exp_empty) | 2 scales stored (their loads returned)
 //   consumer warp 0:    4 pack_full passed | 5 exp_full passed | 6 group dequantised
+// The resident variant (EPI_RESIDENT) stamps 3 once the producers have received everything (group 0's slot), 5 once the
+// consumers have (group 0's slot), 4 and 6 per group, and slot 3 of the launch stamps past the cluster barrier before its push.
 // A compile-time switch: even untaken, a runtime branch in the per-group loops costs the 16-token split-K launch about
 // 0.6 us (H100 80GB HBM3, 700 W).
 #ifdef ATOM_GEMM_TRACE_GROUPS
@@ -93,18 +98,27 @@ __host__ __device__ __forceinline__ int scale_size(int m) { return m / 16 * 64 +
 // tile of the token-tile table selects the expert (weight rows and scales) and the rows of the permuted activations; rows
 // past the tile's valid count are not stored.  A bit of the epilogue parameter rather than a parameter of its own, so that
 // every other instantiation keeps its symbol and its code.
-enum { EPI_O16 = 0, EPI_O4 = 1, EPI_QKV = 2, EPI_GATEUP = 3, EPI_PUSH = 4, EPI_GROUPED = 8 };
+// EPI_RESIDENT: a mode bit or-ed into EPI_O16 / EPI_PUSH for 16-token tiles split over K whose every rank holds at most PACK
+// INT4 groups.  The rank's whole K slice then stays in shared memory, one slot per group: the static operands (weights and
+// weight scales) are all requested before griddepcontrol.wait, the dynamic ones (token tiles and token scales) in one burst
+// after it, the producers widen every token tile and arrive once, and the consumers run the groups with no ring handshakes.
+// The split-K partials are pushed to the rank that stores them (st.async) instead of being staged and read remotely.
+enum { EPI_O16 = 0, EPI_O4 = 1, EPI_QKV = 2, EPI_GATEUP = 3, EPI_PUSH = 4, EPI_GROUPED = 8, EPI_RESIDENT = 16 };
 
 template <int BN, int kSplit, int kEpi>
 struct GemmCfg {
-  static constexpr int ROWS = (kEpi & ~EPI_GROUPED) == EPI_GATEUP ? 256 : 128;    // weight rows per CTA
+  static constexpr int EPI = kEpi & ~(EPI_GROUPED | EPI_RESIDENT);   // the epilogue
+  static constexpr bool RESIDENT = (kEpi & EPI_RESIDENT) != 0;
+  static constexpr int ROWS = EPI == EPI_GATEUP ? 256 : 128;    // weight rows per CTA
   static constexpr int MT = ROWS / 128;                          // 64-row wgmma tiles per consumer warpgroup
   static constexpr int THREADS = 384;                            // producer warpgroup + two consumer warpgroups
   static constexpr int PACK = BN <= 32 ? 8 : 4;                  // packed ring depth (groups): decode shapes are a weight stream
-  static constexpr int EXP = BN <= 64 ? 4 : 3;                   // expanded token tiles / scale slots
+  // expanded token tiles / scale slots; resident: one per packed slot
+  static constexpr int EXP = RESIDENT ? PACK : (BN <= 64 ? 4 : 3);
   // Decode tiles (BN <= 32) load the scales in a producer warp of their own (SCALE_WARP), SCALE_AHEAD groups ahead, and
   // widen the token tile with the other three; larger tiles need all four warps to widen and load the scales in line.
-  static constexpr bool SCALE_WARP_ON = BN <= 32;
+  // The resident variant loads all its scales up front and widens with all four warps.
+  static constexpr bool SCALE_WARP_ON = BN <= 32 && !RESIDENT;
   static constexpr int SCALE_WARP = 3;
   static constexpr int SCALE_AHEAD = 4;                          // groups whose scale loads the scale warp keeps in flight
   static constexpr int SCALE_THREADS = SCALE_WARP_ON ? 32 : 128;  // threads that load and store a group's scales
@@ -120,15 +134,22 @@ struct GemmCfg {
   static constexpr int OFF_PACK_Q = OFF_PACK_W + PACK * PACK_W;
   static constexpr int OFF_SCALE = OFF_PACK_Q + PACK * PACK_Q;
   static constexpr int OFF_BAR = OFF_SCALE + (EXP + 1) * SCALE_BYTES;   // slot EXP: the keeper's scales
-  static constexpr int NUM_BARS = 2 * PACK + 2 * EXP + 1;
+  static constexpr int NUM_BARS = 2 * PACK + 2 * EXP + 1 + (RESIDENT ? 1 : 0);   // resident: + the split-K receive barrier
   static constexpr int SMEM_BYTES = OFF_BAR + NUM_BARS * 8 + 1024;   // + slack for the 1024-B alignment fix-up
   static constexpr int TILE_PITCH = ROWS + 4;                    // floats per token row of the staged output tile
   static constexpr int KEEP_TX = ROWS * 128 + BN * 128;
+  // resident: rank r receives row tk (tk % kSplit == r) of rank k's FP32 partial tile in slot [k][tk / kSplit] of ROWS floats,
+  // over the packed token slots, which this variant does not use (its token tiles are loaded into registers)
+  static constexpr int RECV_TX = BN * ROWS * 4;
   static_assert(BN == 16 || BN == 32 || BN == 64 || BN == 128, "token tile");
   static_assert(BN * TILE_PITCH * 4 <= OFF_SCALE, "the output tile is staged over the idle operand rings");
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
-  static_assert(kSplit == 1 || kEpi == EPI_O16 || kEpi == EPI_PUSH, "the quantising epilogues work on un-split FP32 sums");
+  static_assert(kSplit == 1 || EPI == EPI_O16 || EPI == EPI_PUSH, "the quantising epilogues work on un-split FP32 sums");
   static_assert(!(kEpi & EPI_GROUPED) || (kSplit == 1 && BN <= 64), "grouped mode: token tiles of 16 / 32 / 64, no K split");
+  static_assert(!RESIDENT || (BN == 16 && kSplit > 1 && !(kEpi & EPI_GROUPED)), "resident: split 16-token tiles, not grouped");
+  static_assert(!RESIDENT || RECV_TX <= PACK * PACK_Q, "resident: the receive slots fit over the packed token tiles");
+  // the next launch's CTA prefetches its weights beside this one: two CTAs per SM (228 KB, 1 KB reserved per CTA)
+  static_assert(!RESIDENT || 2 * (SMEM_BYTES + 1024) <= 228 * 1024, "resident: two CTAs per SM");
 };
 
 template <int BN, int kSplit, int kEpi>
@@ -140,7 +161,7 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
                const GemmArgs args) {
   using C = GemmCfg<BN, kSplit, kEpi>;
   constexpr bool kGrouped = (kEpi & EPI_GROUPED) != 0;
-  constexpr int kE = kEpi & ~EPI_GROUPED;                    // the epilogue
+  constexpr int kE = C::EPI;
   constexpr int NR = BN / 2;                                // accumulator registers per 64-row tile
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024-B alignment (SWIZZLE_128B atoms) by offsetting the shared array, NOT by integer-casting the pointer:
@@ -153,6 +174,9 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
   uint64_t* exp_full = pack_empty + C::PACK;           // token operand + scales of the group in place   (4 producer warps)
   uint64_t* exp_empty = exp_full + C::EXP;             // consumers are done with them                   (8 consumer warps)
   uint64_t* keep_full = exp_empty + C::EXP;            // keeper tiles + scales landed     (1 + tx, the scale-loading warps)
+  // resident: exp_full[0] = every token tile widened and every scale stored (4 producer warps); keep_full = keeper weights
+  // landed (1 + tx); recv_bar = every rank's partials of this rank's token rows landed (1 + RECV_TX, st.async)
+  uint64_t* recv_bar = keep_full + 1;
 
   // the warp index through a shuffle: the compiler then knows the role branches below are warp-uniform
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
@@ -188,12 +212,14 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
     tma_prefetch_desc(&tm_w4); tma_prefetch_desc(&tm_a4); tma_prefetch_desc(&tm_w8); tma_prefetch_desc(&tm_a8);
     for (int i = 0; i < C::PACK; ++i) { mbar_init(&pack_full[i], 1); mbar_init(&pack_empty[i], C::SCALE_WARP_ON ? 11 : 12); }
     for (int i = 0; i < C::EXP; ++i) { mbar_init(&exp_full[i], 4); mbar_init(&exp_empty[i], 8); }
-    mbar_init(keep_full, C::SCALE_WARP_ON ? 2 : 5);
+    mbar_init(keep_full, C::RESIDENT ? 1 : (C::SCALE_WARP_ON ? 2 : 5));
+    if constexpr (C::RESIDENT) mbar_init(recv_bar, 1);
     fence_barrier_init();
+    if constexpr (C::RESIDENT) mbar_arrive_expect_tx(recv_bar, C::RECV_TX);   // armed before the cluster barrier below
   }
   __syncthreads();
   // split-K: a CTA's shared memory may only be read remotely while that CTA is alive -- every thread arrives here (cheap,
-  // non-blocking) and waits before the reduction
+  // non-blocking) and waits before the reduction (resident: before its first remote write)
   if constexpr (kSplit > 1) cluster_arrive_relaxed();
   if (threadIdx.x == 0) trace_stamp(args, 1);
 
@@ -215,6 +241,89 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
       if (part != 1) tma_load_2d(smem + C::OFF_PACK_Q + ps * C::PACK_Q, &tm_a4, &pack_full[ps], g * 64, m0);
     };
     griddep_launch_dependents();
+    if constexpr (C::RESIDENT) {
+      // ---------------------------------------------------------- resident slice: slot s = INT4 group g_begin + s, the
+      // keeper's scales in slot PACK.  PDL contract: the weight tiles, the keeper weights and the weight scales are static
+      // operands of the layer and are read before griddepcontrol.wait; the token tiles and token scales come after it.
+      if (t == 0) {
+        for (int s = 0; s < n4; ++s) {
+          mbar_arrive_expect_tx(&pack_full[s], C::PACK_W);
+          tma_load_2d(smem + C::OFF_PACK_W + s * C::PACK_W, &tm_w4, &pack_full[s], (g_begin + s) * 64, n0);
+        }
+        if (has_keeper) {
+          mbar_arrive_expect_tx(keep_full, C::ROWS * 128);
+          tma_load_2d(smem + C::OFF_KEEP_W, &tm_w8, keep_full, 0, n0);
+        }
+      }
+      // chunk c of the scales: slot c / 16, weight-scale chunk (8 channels) and token c % 16
+      constexpr int CHUNKS = (C::PACK + 1) * 16, PER_T = (CHUNKS + 127) / 128;
+      uint4 wsc[PER_T];
+      __half asc[PER_T];
+#pragma unroll
+      for (int i = 0; i < PER_T; ++i) {
+        const int c = t + 128 * i, s = c >> 4, col = c & 15;
+        wsc[i] = make_uint4(0, 0, 0, 0);
+        if (c < CHUNKS && (s < n4 || (s == C::PACK && has_keeper)) && n0 + 8 * col < args.N)
+          wsc[i] = ld_cg_v4((s == C::PACK ? args.b_keeper_scale : args.b_scale + (size_t)(g_begin + s) * args.ldb_scale) + n0 + 8 * col);
+      }
+      griddep_wait();                       // from here on the preceding kernel's output (the activations) may be read
+      if (t == 0) trace_stamp(args, 5);
+      // Every dynamic input in one burst of L2 loads, all in flight together.  The token tiles do not take the TMA queue:
+      // there they wait behind the weight requests of the next launch's CTA on this SM and land one by one.
+      // Thread t: 16-B chunk t % 64 (token row r, quarter qq) of the packed tiles of groups s = t / 64 + 2i, and 16-B chunk
+      // t of the keeper's INT8 token tile (row t / 8).  Rows past M read as zero, as the TMA box would.
+      const int r = (t & 63) >> 2, qq = t & 3, rk = t >> 3, ck = t & 7;
+      const size_t pitch4 = (size_t)args.G * 64;
+      uint4 tok[C::PACK / 2], ktok = make_uint4(0, 0, 0, 0);
+#pragma unroll
+      for (int i = 0; i < C::PACK / 2; ++i) {
+        const int s = (t >> 6) + 2 * i;
+        tok[i] = make_uint4(0, 0, 0, 0);
+        if (s < n4 && m0 + r < args.M) tok[i] = ld_cg_v4(args.a4 + (size_t)(m0 + r) * pitch4 + (size_t)(g_begin + s) * 64 + qq * 16);
+      }
+      if (has_keeper && m0 + rk < args.M) ktok = ld_cg_v4(args.a8 + (size_t)(m0 + rk) * 128 + ck * 16);
+#pragma unroll
+      for (int i = 0; i < PER_T; ++i) {
+        const int c = t + 128 * i, s = c >> 4, tk = c & 15;
+        asc[i] = __ushort_as_half(0);
+        if (c < CHUNKS && (s < n4 || (s == C::PACK && has_keeper)) && m0 + tk < args.M)
+          asc[i] = __ushort_as_half(ld_cg_u16((s == C::PACK ? args.a_keeper_scale : args.a_scale + (size_t)(g_begin + s) * args.lda_scale) +
+                                              scale_index(m0 + tk)));
+      }
+      // widen into the SWIZZLE_128B INT8 operands, as the ring's widening does; the keeper tile as its TMA box would land
+#pragma unroll
+      for (int i = 0; i < C::PACK / 2; ++i) {
+        const int s = (t >> 6) + 2 * i;
+        if (s < n4) {
+          const uint32_t ww[4] = {tok[i].x, tok[i].y, tok[i].z, tok[i].w};
+          uint8_t* row = smem + C::OFF_EXP + s * C::EXP_Q + (r >> 3) * 1024 + (r & 7) * 128 + 4 * qq;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            *reinterpret_cast<uint32_t*>(row + (((2 * j) ^ (r & 7)) << 4)) = (ww[j] << 4) & 0xF0F0F0F0u;
+            *reinterpret_cast<uint32_t*>(row + (((2 * j + 1) ^ (r & 7)) << 4)) = ww[j] & 0xF0F0F0F0u;
+          }
+        }
+      }
+      if (has_keeper) *reinterpret_cast<uint4*>(smem + C::OFF_KEEP_Q + (rk >> 3) * 1024 + (rk & 7) * 128 + ((ck ^ (rk & 7)) << 4)) = ktok;
+#pragma unroll
+      for (int i = 0; i < PER_T; ++i) {
+        const int c = t + 128 * i, s = c >> 4, col = c & 15;
+        if (c < CHUNKS && (s < n4 || (s == C::PACK && has_keeper))) {
+          uint8_t* slot = smem + C::OFF_SCALE + s * C::SCALE_BYTES;
+          reinterpret_cast<uint4*>(slot)[col] = wsc[i];
+          reinterpret_cast<__half*>(slot + C::ROWS * 2)[col] = asc[i];
+        }
+      }
+      // the weight tiles landed long ago; observing them here lets the consumers' single wait below cover them
+      for (int s = 0; s < n4; ++s) mbar_wait(&pack_full[s], 0);
+      fence_proxy_async_smem();             // generic-proxy stores -> visible to the wgmma operand fetch
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&exp_full[0]);
+      if (t == 0) trace_group(args, 3, 0);
+      if constexpr (kSplit > 1) cluster_wait();
+      if (t == 0) trace_stamp(args, 4);
+      return;
+    }
     if (t == 0) {
       const int first = min(C::PACK, n4);
       for (int s = 0; s < first; ++s) issue_stage(s, 1);
@@ -368,9 +477,14 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
       }
     };
 
+    if constexpr (C::RESIDENT) {
+      // the producers passed every group's pack_full before they arrived: the weight tiles are in place too
+      mbar_wait(&exp_full[0], 0);
+      if (cw == 0 && lane == 0) trace_group(args, 5, 0);
+    }
     for (int s = 0; s < n4; ++s) {
       const int ps = s % C::PACK, es = s % C::EXP;
-      mbar_wait(&pack_full[ps], (s / C::PACK) & 1);
+      if constexpr (!C::RESIDENT) mbar_wait(&pack_full[ps], (s / C::PACK) & 1);
       if (cw == 0 && lane == 0) trace_group(args, 4, s);
       uint4 wa[C::MT], wb[C::MT];
 #pragma unroll
@@ -379,10 +493,12 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
         wa[t] = *reinterpret_cast<const uint4*>(p);
         wb[t] = *reinterpret_cast<const uint4*>(p + 8 * 64);
       }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&pack_empty[ps]);
-      mbar_wait(&exp_full[es], (s / C::EXP) & 1);
-      if (cw == 0 && lane == 0) trace_group(args, 5, s);
+      if constexpr (!C::RESIDENT) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&pack_empty[ps]);
+        mbar_wait(&exp_full[es], (s / C::EXP) & 1);
+        if (cw == 0 && lane == 0) trace_group(args, 5, s);
+      }
       const uint64_t db = wgmma_desc_k_sw128(smem_u32(smem + C::OFF_EXP + es * C::EXP_Q));
       const __half* sb = reinterpret_cast<const __half*>(smem + C::OFF_SCALE + es * C::SCALE_BYTES);
       const __half* sa = sb + C::ROWS;
@@ -402,8 +518,10 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
         const int ch = (wg * C::MT + t) * 64 + wq * 16 + g8;
         dequant(acc[t], d, sa, sb, ch, false);
       }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&exp_empty[es]);
+      if constexpr (!C::RESIDENT) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&exp_empty[es]);
+      }
       if (cw == 0 && lane == 0) trace_group(args, 6, s);
     }
     if (has_keeper) {
@@ -437,24 +555,51 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
     }
     if (cw == 0 && lane == 0) trace_stamp(args, 2);
 
-    // ------------------------------------------------------------ stage the FP32 tile as [token][channel]
-    asm volatile("bar.sync 1, 256;" ::: "memory");     // both consumer warpgroups have left the operand rings
     float* tile = reinterpret_cast<float*>(smem);
+    // resident receive slots: [rank][row tk / kSplit][ROWS floats], channel c at (c & ~15) + 2 (c & 7) + ((c >> 3) & 1), so
+    // that a thread's channel pair (ch, ch + 8) is one 8-byte push
+    const float* recv = reinterpret_cast<const float*>(smem + C::OFF_PACK_Q);
+    if constexpr (C::RESIDENT) {
+      // ------------------------------------------------------------ push row tk of the partial tile to rank tk % kSplit
+      cluster_wait();                                  // every rank has initialised and armed its recv_bar
+      if (cw == 0 && lane == 0) trace_stamp(args, 3);
+      const uint32_t rbase = smem_u32(recv), rbar = smem_u32(recv_bar);
 #pragma unroll
-    for (int t = 0; t < C::MT; ++t) {
-      const int ch = (wg * C::MT + t) * 64 + wq * 16 + g8;
+      for (int t = 0; t < C::MT; ++t) {
+        const int ch = (wg * C::MT + t) * 64 + wq * 16 + g8;
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int tk = 8 * j + 2 * q;
-        tile[tk * C::TILE_PITCH + ch] = acc[t][4 * j + 0];
-        tile[(tk + 1) * C::TILE_PITCH + ch] = acc[t][4 * j + 1];
-        tile[tk * C::TILE_PITCH + ch + 8] = acc[t][4 * j + 2];
-        tile[(tk + 1) * C::TILE_PITCH + ch + 8] = acc[t][4 * j + 3];
+        for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int tk = 8 * j + 2 * q + e, dst = tk % kSplit;
+            const uint32_t at = rbase + (((int)krank * (BN / kSplit) + tk / kSplit) * C::ROWS + ch + g8) * 4;
+            st_async_v2(mapa_shared(at, dst), acc[t][4 * j + e], acc[t][4 * j + 2 + e], mapa_shared(rbar, dst));
+          }
       }
+      // Every consumer warp waits, so that the CTA stays alive until the last push into it has landed.  The st.async
+      // write and its complete-tx on this mbarrier are one operation (PTX ISA, st.async), so once the phase completes no
+      // other CTA touches this CTA's shared memory again, and the senders read registers only: no cluster barrier
+      // before exit is needed (a CTA's shared memory may be accessed remotely only while that CTA is running).
+      mbar_wait<true>(recv_bar, 0);
+    } else {
+      // ------------------------------------------------------------ stage the FP32 tile as [token][channel]
+      asm volatile("bar.sync 1, 256;" ::: "memory");     // both consumer warpgroups have left the operand rings
+#pragma unroll
+      for (int t = 0; t < C::MT; ++t) {
+        const int ch = (wg * C::MT + t) * 64 + wq * 16 + g8;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int tk = 8 * j + 2 * q;
+          tile[tk * C::TILE_PITCH + ch] = acc[t][4 * j + 0];
+          tile[(tk + 1) * C::TILE_PITCH + ch] = acc[t][4 * j + 1];
+          tile[tk * C::TILE_PITCH + ch + 8] = acc[t][4 * j + 2];
+          tile[(tk + 1) * C::TILE_PITCH + ch + 8] = acc[t][4 * j + 3];
+        }
+      }
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      if constexpr (kSplit > 1) { cluster_wait(); cluster_arrive(); cluster_wait(); }   // every rank's tile is staged
+      if (cw == 0 && lane == 0) trace_stamp(args, 3);
     }
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    if constexpr (kSplit > 1) { cluster_wait(); cluster_arrive(); cluster_wait(); }   // every rank's tile is staged
-    if (cw == 0 && lane == 0) trace_stamp(args, 3);
 
     // ------------------------------------------------------------ output: one warp per token row, 4 channels per lane
     constexpr float kInv = 1.0f / 256.0f;   // exact: removes the 16 * 16 operand factor
@@ -470,11 +615,20 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
       if (m >= (kGrouped ? gtile.y + gtile.z : args.M)) break;
       if (kSplit > 1 && (tk % kSplit) != (int)krank) continue;  // split-K: rank r reduces + stores the token rows r mod kSplit
       float v[4];
-      {
+      if constexpr (C::RESIDENT) {
+        // channels 4 lane .. 4 lane + 3 of every rank's slot, summed in rank order as below
+        const float* r0 = recv + (tk / kSplit) * C::ROWS + 16 * (lane >> 2) + 8 * (lane & 1) + ((lane >> 1) & 1);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) v[e] = r0[2 * e];
+#pragma unroll
+        for (int rk = 1; rk < kSplit; ++rk)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) v[e] += r0[rk * (BN / kSplit) * C::ROWS + 2 * e];
+      } else {
         const float4 f = *reinterpret_cast<const float4*>(tile + tk * C::TILE_PITCH + lane * 4);
         v[0] = f.x; v[1] = f.y; v[2] = f.z; v[3] = f.w;
       }
-      if constexpr (kSplit > 1) {
+      if constexpr (kSplit > 1 && !C::RESIDENT) {
         // every remote rank's 4 channels in one 16-B load, all in flight together (one at a time, the remote-load latency
         // stacked up 4 (kSplit - 1) deep per token row), then the rank-order sums
         const uint32_t local = smem_u32(tile + tk * C::TILE_PITCH + lane * 4);
@@ -575,8 +729,8 @@ gemm_i4_kernel(const __grid_constant__ CUtensorMap tm_w4,   // packed INT4 weigh
       }
     }
     if (cw == 0 && lane == 0) trace_stamp(args, 6);
-    // split-K: no CTA of the cluster leaves while its tile may still be read
-    if constexpr (kSplit > 1) { cluster_arrive(); cluster_wait(); }
+    // split-K: no CTA of the cluster leaves while its tile may still be read (resident: nothing is read remotely)
+    if constexpr (kSplit > 1 && !C::RESIDENT) { cluster_arrive(); cluster_wait(); }
     if (cw == 0 && lane == 0) trace_stamp(args, 7);
   }
   if (threadIdx.x == 0) trace_stamp(args, 4);

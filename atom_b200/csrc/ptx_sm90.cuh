@@ -23,16 +23,28 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
 // try_wait with a suspend-time hint: the thread sleeps in hardware until the phase completes (or ~the hint elapses)
-// instead of burning issue slots in a software spin loop.
+// instead of burning issue slots in a software spin loop.  kCluster: acquire at cluster scope, for a phase completed by
+// other CTAs of the cluster (st.async into this CTA's shared memory).
+template <bool kCluster = false>
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity), "r"(20000u)
-      : "memory");
+  if constexpr (kCluster) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2, %3;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(ok)
+        : "r"(smem_u32(bar)), "r"(parity), "r"(20000u)
+        : "memory");
+  } else {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(ok)
+        : "r"(smem_u32(bar)), "r"(parity), "r"(20000u)
+        : "memory");
+  }
   return ok != 0;
 }
 // A pipeline bug must not hang the GPU: after ~4 s the waiting thread traps, turning a deadlock into a launch error.  The
@@ -49,11 +61,12 @@ __device__ __noinline__ void mbar_timeout(uint64_t* bar, uint32_t parity) {
 #else
 __device__ __forceinline__ void mbar_timeout(uint64_t*, uint32_t) { asm volatile("trap;"); }
 #endif
+template <bool kCluster = false>
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;
+  if (mbar_try_wait<kCluster>(bar, parity)) return;
   long long t0 = 0;
   uint32_t spins = 0;
-  while (!mbar_try_wait(bar, parity)) {
+  while (!mbar_try_wait<kCluster>(bar, parity)) {
     if ((++spins & 63u) == 0) {
       const long long now = clock64();
       if (t0 == 0) t0 = now;
@@ -150,6 +163,12 @@ __device__ __forceinline__ float4 ld_dsmem_v4(uint32_t addr) {
   float4 v;
   asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
   return v;
+}
+// 8 bytes from registers into a cluster CTA's shared memory at `addr`; the write completes 8 bytes of transaction count on
+// that CTA's mbarrier `bar` (both addresses from mapa_shared).  Nothing of the sender's shared memory is read.
+__device__ __forceinline__ void st_async_v2(uint32_t addr, float x, float y, uint32_t bar) {
+  asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v2.f32 [%0], {%1, %2}, [%3];"
+               ::"r"(addr), "f"(x), "f"(y), "r"(bar) : "memory");
 }
 __device__ __forceinline__ float2 ld_dsmem_v2(uint32_t addr) {
   float2 v;

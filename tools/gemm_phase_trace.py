@@ -131,8 +131,11 @@ def main():
             own = [c for c in ctas if tr[c, 5] and tr[c, 8 + 6 * TRACE_GROUPS + g]]
             if not own:
                 break
-            cols = [np.median([tr[c, 8 + kind * TRACE_GROUPS + g] - tr[c, 5] for c in own]) for kind in range(len(GROUP_KINDS))]
-            print(f"{g:5d} " + " ".join(f"{v:15.0f}" for v in cols))
+            cols = []
+            for kind in range(len(GROUP_KINDS)):
+                v = [tr[c, 8 + kind * TRACE_GROUPS + g] - tr[c, 5] for c in own if tr[c, 8 + kind * TRACE_GROUPS + g]]
+                cols.append(f"{np.median(v):15.0f}" if v else f"{'-':>15s}")   # the resident variant writes fewer kinds
+            print(f"{g:5d} " + " ".join(cols))
 
 
 if __name__ == "__main__":
