@@ -53,6 +53,8 @@ _SIGNATURES = {
     "atom_sample_f16": (_I, [_P, _I64, _I, _I] + [_P] * 7),
     "atom_sample_ex_f16": (_I, [_P, _I64, _I, _I] + [_P] * 11 + [_I64, _P, _P, _I, _P, _P, _P]),
     "atom_sample_slot_init": (_I, [_P, _I64, _I, _I, _P, _I, _P]),
+    "atom_sample_draft_f16": (_I, [_P, _I64, _I, _I] + [_P] * 8 + [_I, _P, _P, _P, _P]),
+    "atom_spec_commit_propose": (_I, [_P] * 4 + [_I, _P, _P] + [_I] * 5 + [_P, _P]),
 }
 
 _lib = None

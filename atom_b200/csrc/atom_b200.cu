@@ -29,6 +29,7 @@
 #include "quant_kernels.cuh"
 #include "moe_kernels.cuh"
 #include "sample_kernels.cuh"
+#include "spec_kernels.cuh"
 
 namespace {
 
@@ -1053,14 +1054,16 @@ int atom_moe_combine_f16(const void* y, const void* topk_ids, const void* topk_w
 
 namespace {
 
-template <bool PEN, bool EXT>
-int sample_launch(const atom::SampleArgs& args, const atom::SampleExArgs& x, int batch, cudaStream_t stream) {
+template <bool PEN, bool EXT, bool DRAFT = false>
+int sample_launch(const atom::SampleArgs& args, const atom::SampleExArgs& x, int batch, cudaStream_t stream,
+                  const int32_t* drafts = nullptr) {
   const int C = atom::sample_cluster(args.V);
   const size_t fixed = EXT ? atom::sample_ex_offset(args.slice) + sizeof(atom::SampleExShared)
                            : atom::SAMPLE_SMEM_FIXED + (size_t)args.slice * sizeof(uint16_t);
   const int most = (int)(EXT ? atom::sample_ex_offset(atom::SAMPLE_SLICE_MAX) + sizeof(atom::SampleExShared)
                              : atom::SAMPLE_SMEM_FIXED + atom::SAMPLE_SLICE_MAX * sizeof(uint16_t));
-  int rc = ensure_dynamic_smem(atom::sample_kernel<PEN, EXT>, most, "sample_f16");
+  int rc = DRAFT ? ensure_dynamic_smem(atom::sample_draft_kernel, most, "sample_draft_f16")
+                 : ensure_dynamic_smem(atom::sample_kernel<PEN, EXT>, most, "sample_f16");
   if (rc) return rc;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3((unsigned)(C * batch)); cfg.blockDim = dim3(atom::SAMPLE_THREADS); cfg.dynamicSmemBytes = fixed;
@@ -1075,7 +1078,8 @@ int sample_launch(const atom::SampleArgs& args, const atom::SampleExArgs& x, int
     attr[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.numAttrs = 2;
   }
-  cudaError_t e = cudaLaunchKernelEx(&cfg, atom::sample_kernel<PEN, EXT>, args, pdl, x);
+  cudaError_t e = DRAFT ? cudaLaunchKernelEx(&cfg, atom::sample_draft_kernel, args, pdl, x, drafts)
+                        : cudaLaunchKernelEx(&cfg, atom::sample_kernel<PEN, EXT>, args, pdl, x);
   if (e != cudaSuccess) return fail(ATOM_E_CUDA, "sample_f16 launch (cluster %d): %s", C, cudaGetErrorString(e));
   return check_launch("sample_f16");
 }
@@ -1139,6 +1143,40 @@ int atom_sample_ex_f16(const void* logits, int64_t ld, int batch, int vocab, con
   const cudaStream_t st = (cudaStream_t)stream;
   if (pen) return ext ? sample_launch<true, true>(args, x, batch, st) : sample_launch<true, false>(args, x, batch, st);
   return ext ? sample_launch<false, true>(args, x, batch, st) : sample_launch<false, false>(args, x, batch, st);
+}
+
+int atom_sample_draft_f16(const void* logits, int64_t ld, int batch, int vocab, const void* temperature, const void* top_k,
+                          const void* top_p, const void* key, const void* counter, const void* min_p, void* out, void* logprob_out,
+                          int top_n, void* top_ids, void* top_logprobs, const void* drafts, void* stream) {
+  int rc = sample_check(logits, ld, batch, vocab, temperature, top_k, top_p, key, counter, out);
+  if (rc) return rc;
+  ATOM_REQUIRE(drafts && aligned4(drafts), "sample_draft_f16: drafts must be a 4-byte aligned i32 [batch]");
+  ATOM_REQUIRE(top_n >= 0 && top_n <= atom::SAMPLE_TOP_N_MAX && (top_n == 0 || (top_ids && top_logprobs)),
+               "sample_draft_f16: top_n=%d must be in [0, %d], with top_ids and top_logprobs", top_n, atom::SAMPLE_TOP_N_MAX);
+  ATOM_REQUIRE(aligned4(min_p) && aligned4(logprob_out) && aligned4(top_ids) && aligned4(top_logprobs),
+               "sample_draft_f16: misaligned pointer (4 bytes)");
+  atom::SampleExArgs x{};
+  x.min_p = (const float*)min_p; x.logprob = (float*)logprob_out; x.top_n = top_n;
+  x.top_ids = (int32_t*)top_ids; x.top_logprobs = (float*)top_logprobs;
+  return sample_launch<false, true, true>(sample_args(logits, ld, vocab, temperature, top_k, top_p, key, counter, out), x, batch,
+                                          (cudaStream_t)stream, (const int32_t*)drafts);
+}
+
+int atom_spec_commit_propose(const void* tokens, const void* cands, const void* row_indptr, const void* slots, int batch, void* history,
+                             void* history_len, int num_slots, int cap, int num_draft, int ngram_min, int ngram_max, void* out,
+                             void* stream) {
+  ATOM_REQUIRE(tokens && cands && row_indptr && slots && history && history_len && out, "spec_commit_propose: null pointer argument");
+  ATOM_REQUIRE(aligned4(tokens) && aligned4(cands) && aligned4(row_indptr) && aligned4(slots) && aligned4(history) &&
+               aligned4(history_len) && aligned4(out), "spec_commit_propose: misaligned pointer (4 bytes)");
+  ATOM_REQUIRE(batch > 0 && num_slots > 0 && cap > 0, "spec_commit_propose: batch=%d, num_slots=%d and cap=%d must be positive",
+               batch, num_slots, cap);
+  ATOM_REQUIRE(num_draft >= 1 && num_draft <= atom::SPEC_MAX_DRAFT && ngram_min >= 1 && ngram_min <= ngram_max &&
+               ngram_max <= atom::SPEC_MAX_NGRAM, "spec_commit_propose: need 1 <= num_draft=%d <= %d and 1 <= ngram_min=%d <= "
+               "ngram_max=%d <= %d", num_draft, atom::SPEC_MAX_DRAFT, ngram_min, ngram_max, atom::SPEC_MAX_NGRAM);
+  atom::SpecArgs a{(const int32_t*)tokens, (const int32_t*)cands, (const int32_t*)row_indptr, (const int32_t*)slots, (int32_t*)history,
+                   (int32_t*)history_len, num_slots, cap, num_draft, ngram_min, ngram_max, (int32_t*)out};
+  return launch_k("spec_commit_propose", atom::spec_commit_propose_kernel, dim3(batch), dim3(atom::SPEC_THREADS), 0,
+                  (cudaStream_t)stream, a);
 }
 
 int atom_sample_slot_init(void* table, int64_t table_ld, int vocab, int slot, const void* prompt, int prompt_len, void* stream) {

@@ -112,6 +112,18 @@ __device__ __forceinline__ unsigned long long philox4x64_w0(unsigned long long k
   }
   return c0;
 }
+// words 0 and 1 of the same block (the draft rule's acceptance uses word 1)
+__device__ __forceinline__ ulonglong2 philox4x64_w01(unsigned long long k0, unsigned long long k1, unsigned long long n) {
+  const unsigned long long M0 = 0xD2E7470EE14C6C93ull, M1 = 0xCA5A826395121157ull;
+  unsigned long long c0 = n, c1 = 0, c2 = 0, c3 = 0;
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    if (r) { k0 += 0x9E3779B97F4A7C15ull; k1 += 0xBB67AE8584CAA73Bull; }
+    const unsigned long long hi0 = __umul64hi(M0, c0), lo0 = M0 * c0, hi1 = __umul64hi(M1, c2), lo1 = M1 * c2;
+    c0 = hi1 ^ c1 ^ k0; c1 = lo1; c2 = hi0 ^ c3 ^ k1; c3 = lo0;
+  }
+  return make_ulonglong2(c0, c1);
+}
 
 __device__ __forceinline__ unsigned long long dsmem_u64(const void* p, uint32_t rank) {
   unsigned long long v;
@@ -364,9 +376,11 @@ __device__ __forceinline__ void sample_logprobs(SampleShared& s, const SampleArg
   }
 }
 
-// grid (C * B), cluster (C): CTA x is rank x % C of row x / C
-template <bool PEN, bool EXT>
-__global__ void __launch_bounds__(SAMPLE_THREADS, 1) sample_kernel(const SampleArgs a, int pdl, const SampleExArgs x) {
+// One row per cluster; sample_kernel and sample_draft_kernel are its instances.  DRAFT: the row has one candidate token
+// drafts[row] (-1: none), accepted or replaced by the rule of atom_sample_draft_f16 (DESIGN section 5.7); never with PEN.
+// (the drafts pointer is a pack, empty without DRAFT: an unused parameter changes how the other instances are scheduled)
+template <bool PEN, bool EXT, bool DRAFT, typename... Drafts>
+__device__ __forceinline__ void sample_row(const SampleArgs a, int pdl, const SampleExArgs x, Drafts... drafts) {
   extern __shared__ __align__(16) uint8_t smem_s[];
   SampleShared& s = *reinterpret_cast<SampleShared*>(smem_s);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -427,6 +441,11 @@ __global__ void __launch_bounds__(SAMPLE_THREADS, 1) sample_kernel(const SampleA
   const int K = a.top_k[row];
   bool bad_param = !(T >= 0.f) || isinf(T) || K < 0 || !(P > 0.f && P <= 1.f);
   if constexpr (PEN) bad_param = bad_param || !(rp > 0.f) || isinf(rp) || !isfinite(fp) || !isfinite(pp);
+  int d = -1;
+  if constexpr (DRAFT) {
+    d = (drafts[row], ...);
+    bad_param = bad_param || d < -1 || d >= a.V;
+  }
   float M = 0.f;
   if constexpr (EXT) {
     if (x.min_p) M = x.min_p[row];
@@ -513,15 +532,52 @@ __global__ void __launch_bounds__(SAMPLE_THREADS, 1) sample_kernel(const SampleA
     }
 
     // ---- the draw: inverse CDF over the kept tokens in ascending index, u = (w0 >> 11) * 2^-53, t = floor(u * Z)
-    const unsigned long long u53 = philox4x64_w0(a.key[2 * row], a.key[2 * row + 1], a.counter[row]) >> 11;
-    result = sample_find(
-        s, 7, len, lo, C, rank,
-        [&](int i) {
+    if constexpr (!DRAFT) {
+      const unsigned long long u53 = philox4x64_w0(a.key[2 * row], a.key[2 * row + 1], a.counter[row]) >> 11;
+      result = sample_find(
+          s, 7, len, lo, C, rank,
+          [&](int i) {
+            const uint32_t k = s.keys[i];
+            const bool keep = topk_keep(i, k) && (k > pth || (k == pth && lo + i <= pidx));
+            return keep ? weight(k, vmax) : 0ull;
+          },
+          [&](unsigned long long z) { return (__umul64hi(u53, z) << 11) | ((u53 * z) >> 53); });
+    } else {
+      // the candidate d: its kept weight W_d, published by the CTA that holds it (pub[12]); the draw runs over the kept set
+      // without d, so the find's total is Z' = Z - W_d.  Accept iff floor(a * Z * 2^-53) < W_d with a = (w1 >> 11); then
+      // no token is found.  Otherwise the draw is rule 5's with word 0 over that set (Z' > 0: a rejection needs W_d < Z).
+      const ulonglong2 w = philox4x64_w01(a.key[2 * row], a.key[2 * row + 1], a.counter[row]);
+      const unsigned long long u53 = w.x >> 11, a53 = w.y >> 11;
+      const uint32_t owner = d >= 0 ? (uint32_t)(d / a.slice) : C;
+      if (tid == 0) {
+        unsigned long long wd = 0;
+        if (rank == owner) {
+          const int i = d - lo;
           const uint32_t k = s.keys[i];
-          const bool keep = topk_keep(i, k) && (k > pth || (k == pth && lo + i <= pidx));
-          return keep ? weight(k, vmax) : 0ull;
-        },
-        [&](unsigned long long z) { return (__umul64hi(u53, z) << 11) | ((u53 * z) >> 53); });
+          if (topk_keep(i, k) && (k > pth || (k == pth && d <= pidx))) wd = weight(k, vmax);
+        }
+        s.pub[12] = wd;
+      }
+      result = sample_find(
+          s, 7, len, lo, C, rank,
+          [&](int i) {
+            const uint32_t k = s.keys[i];
+            const bool keep = topk_keep(i, k) && (k > pth || (k == pth && lo + i <= pidx)) && lo + i != d;
+            return keep ? weight(k, vmax) : 0ull;
+          },
+          [&](unsigned long long zr) {
+            if (owner < C) {
+              const unsigned long long wd = dsmem_u64(&s.pub[12], owner), z = zr + wd;
+              if (((__umul64hi(a53, z) << 11) | ((a53 * z) >> 53)) < wd) return ~0ull;    // accepted: nothing is found
+            }
+            return (__umul64hi(u53, zr) << 11) | ((u53 * zr) >> 53);
+          });
+      if (result < 0 && d >= 0) result = d;         // accepted (a rejection always finds a token)
+      if (d >= 0 && (x.logprob || x.top_n)) {       // pub[7] summed Z - W_d: make it Z for the log-probabilities' shortcut
+        if (rank == owner && tid == 0) s.pub[7] += s.pub[12];
+        sample_cluster_sync();
+      }
+    }
   }
   if constexpr (EXT) {
     if (x.logprob || x.top_n) sample_logprobs(s, a, x, row, len, lo, C, rank, result, best, T, K, P, mthr);
@@ -537,6 +593,18 @@ __global__ void __launch_bounds__(SAMPLE_THREADS, 1) sample_kernel(const SampleA
       }
     }
   }
+}
+
+// grid (C * B), cluster (C): CTA x is rank x % C of row x / C
+template <bool PEN, bool EXT>
+__global__ void __launch_bounds__(SAMPLE_THREADS, 1) sample_kernel(const SampleArgs a, int pdl, const SampleExArgs x) {
+  sample_row<PEN, EXT, false>(a, pdl, x);
+}
+
+// atom_sample_draft_f16: min-p and log-probabilities as sample_kernel<false, true>, and one candidate per row
+__global__ void __launch_bounds__(SAMPLE_THREADS, 1) sample_draft_kernel(const SampleArgs a, int pdl, const SampleExArgs x,
+                                                                         const int32_t* drafts) {
+  sample_row<false, true, true>(a, pdl, x, drafts);
 }
 
 // one table slot set up for a new request (atom_sample_slot_init): CTA j zeroes entries [j * chunk, (j + 1) * chunk) of the

@@ -761,7 +761,7 @@ def _sample_slots(slots, b, table, device):
 
 
 def sample_tokens(logits, temperature, top_k, top_p, keys, counters, *, min_p=0.0, repetition_penalty=1.0, frequency_penalty=0.0,
-                  presence_penalty=0.0, penalty_table=None, slots=None, logprobs=None):
+                  presence_penalty=0.0, penalty_table=None, slots=None, logprobs=None, drafts=None):
     """EXTENSION: one token id per row of f16 logits [B, V] (rows may have any pitch), int32 [B].  Per row: temperature
     (0 = argmax), top_k (0 = off, on the raw logits), top_p (1 = off), Philox key (key0, key1) and counter; the semantics are
     atom_sample_f16's (include/atom_b200.h, DESIGN section 5.6).  Each parameter is a CUDA tensor with one entry per row (keys:
@@ -776,7 +776,14 @@ def sample_tokens(logits, temperature, top_k, top_p, keys, counters, *, min_p=0.
       penalises each row's logits by its slot's history and records the drawn token in that slot;
       logprobs = n in [0, 20]: also return, per row, the log-probability of the chosen token (float32 [B]) and the first n
       tokens of the order on the penalised logits with theirs (int32 / float32 [B, n]), a log-softmax at temperature 1.
-    With logprobs the result is (tokens, logprob, top_ids, top_logprobs)."""
+    With logprobs the result is (tokens, logprob, top_ids, top_logprobs).
+
+    drafts (atom_sample_draft_f16; speculative decoding): one candidate token per row, an int32 CUDA tensor [B] or a host sequence
+    (-1 = none).  A row accepts its candidate d with probability W_d / Z (its kept weight over the kept total: rejection
+    sampling with a point-mass proposal) and otherwise draws from the kept set without d, so every token keeps the probability
+    the sampler gives it (DESIGN section 5.7).  Greedy rows return the argmax whatever d is; rows without a candidate are exactly
+    the call without drafts; a candidate outside [-1, V) in a device tensor gives -1.  Not with penalties.  None: exactly the
+    call above."""
     if not (isinstance(logits, torch.Tensor) and logits.is_cuda):
         raise RuntimeError("atom_b200.ops: all tensors must live on a CUDA device (there is no CPU path)")
     if logits.dtype != torch.float16 or logits.dim() != 2 or logits.stride(1) != 1:
@@ -795,6 +802,10 @@ def sample_tokens(logits, temperature, top_k, top_p, keys, counters, *, min_p=0.
         raise RuntimeError("atom_b200.ops.sample_tokens: penalties need a penalty_table and slots")
     if logprobs is not None and not (isinstance(logprobs, (int, np.integer)) and 0 <= int(logprobs) <= SAMPLE_TOP_N_MAX):
         raise RuntimeError(f"atom_b200.ops.sample_tokens: logprobs must be an integer in [0, {SAMPLE_TOP_N_MAX}], got {logprobs!r}")
+    if drafts is not None:
+        if pen or slots is not None:
+            raise RuntimeError("atom_b200.ops.sample_tokens: drafts cannot be combined with penalties")
+        return _sample_draft(logits, t, k, p, key, ctr, min_p, logprobs, drafts)
     if pen or logprobs is not None or not _neutral(min_p, 0):
         return _sample_ex(logits, t, k, p, key, ctr, min_p, repetition_penalty, frequency_penalty, presence_penalty, penalty_table,
                           slots, logprobs)
@@ -838,3 +849,94 @@ def _sample_ex(logits, t, k, p, key, ctr, min_p, rep, freq, pres, table, slots, 
                 ptr(sl) if pen else None, ptr(table) if pen else None, table.stride(0) if pen else 0, out.data_ptr(), ptr(lp), n,
                 top_ids.data_ptr() if n else None, top_lp.data_ptr() if n else None, _stream(logits)), "sample_tokens")
     return out if logprobs is None else (out, lp, top_ids, top_lp)
+
+
+def _sample_draft(logits, t, k, p, key, ctr, min_p, logprobs, drafts):
+    import numpy as np
+    b, v = logits.shape
+    dev = logits.device
+    if isinstance(drafts, torch.Tensor):
+        _req_cuda(drafts)
+        if drafts.dtype != torch.int32 or tuple(drafts.shape) != (b,) or drafts.device != dev:
+            raise RuntimeError(f"atom_b200.ops.sample_tokens: `drafts` must be int32 [{b}] on {dev}")
+        d = drafts
+    else:
+        a = np.asarray(drafts, dtype=np.int64).reshape(-1)
+        if a.shape != (b,) or (a < -1).any() or (a >= v).any():
+            raise RuntimeError(f"atom_b200.ops.sample_tokens: `drafts` must hold {b} entries in [-1, {v})")
+        d = torch.from_numpy(a.astype(np.int32)).to(dev)
+    m = None if _neutral(min_p, 0) else _sample_param("min_p", min_p, b, torch.float32, dev, lambda a: ~((a >= 0) & (a <= 1)))
+    n = 0 if logprobs is None else int(logprobs)
+    out = torch.empty((b,), dtype=torch.int32, device=dev)
+    lp = torch.empty((b,), dtype=torch.float32, device=dev) if logprobs is not None else None
+    top_ids = torch.empty((b, n), dtype=torch.int32, device=dev)
+    top_lp = torch.empty((b, n), dtype=torch.float32, device=dev)
+    if b:
+        ptr = lambda x: None if x is None else x.data_ptr()      # noqa: E731
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().atom_sample_draft_f16(
+                logits.data_ptr(), logits.stride(0) if b > 1 else v, b, v, t.data_ptr(), k.data_ptr(), p.data_ptr(), key.data_ptr(),
+                ctr.data_ptr(), ptr(m), out.data_ptr(), ptr(lp), n, top_ids.data_ptr() if n else None,
+                top_lp.data_ptr() if n else None, d.data_ptr(), _stream(logits)), "sample_tokens")
+    return out if logprobs is None else (out, lp, top_ids, top_lp)
+
+
+SPEC_MAX_DRAFT = 7
+SPEC_MAX_NGRAM = 16
+
+
+def spec_history(slots, cap, device):
+    """EXTENSION (speculative decoding): zeroed token histories for `slots` sequences of up to `cap` tokens each, for
+    spec_commit_propose: (history int32 [slots, cap], lengths int32 [slots])."""
+    if int(slots) < 1 or int(cap) < 1 or int(cap) >= 1 << 31:
+        raise RuntimeError(f"atom_b200.ops.spec_history: need slots >= 1 and cap in [1, 2^31), got {slots}, {cap}")
+    return (torch.zeros((int(slots), int(cap)), dtype=torch.int32, device=device),
+            torch.zeros((int(slots),), dtype=torch.int32, device=device))
+
+
+def spec_init_slot(history, lengths, slot, context):
+    """EXTENSION: set slot `slot` of a token history to `context` (a request's whole context: a shared system prompt, then its
+    own prompt), by a plain device copy."""
+    if not 0 <= int(slot) < history.size(0) or len(context) > history.size(1):
+        raise RuntimeError(f"atom_b200.ops.spec_init_slot: slot {slot} outside [0, {history.size(0)}) or a context of "
+                           f"{len(context)} tokens past cap {history.size(1)}")
+    n = len(context)
+    if n:
+        history[int(slot), :n].copy_(torch.tensor(list(context), dtype=torch.int32))
+    lengths[int(slot)].fill_(n)
+
+
+def spec_commit_propose(tokens, cands, row_indptr, slots, history, lengths, out, num_draft, ngram_min, ngram_max):
+    """EXTENSION (atom_spec_commit_propose; DESIGN section 5.8): after a (verify) sampling step, per sequence i owning rows
+    row_indptr[i] .. row_indptr[i+1] of `tokens` (the sampler's output) and `cands` (the candidates it was given, -1: none):
+    commit the accepted tokens to its history slot slots[i] and propose up to num_draft drafts by prompt lookup (the longest
+    n-gram in [ngram_min, ngram_max] whose latest earlier occurrence in the history matches its tail).  All int32 CUDA tensors;
+    tokens and cands [R], row_indptr [B+1], slots [B], history / lengths as spec_history makes them, out [B, 2 * num_draft + 3]
+    receives (emitted, draft_len, tokens [num_draft + 1], drafts [num_draft]), padded with -1.  Allocates nothing, so a CUDA
+    graph may capture it.  slots given as a host sequence are checked to lie in range and be distinct."""
+    k, nmin, nmax = int(num_draft), int(ngram_min), int(ngram_max)
+    if not (1 <= k <= SPEC_MAX_DRAFT and 1 <= nmin <= nmax <= SPEC_MAX_NGRAM):
+        raise RuntimeError(f"atom_b200.ops.spec_commit_propose: need 1 <= num_draft <= {SPEC_MAX_DRAFT} and "
+                           f"1 <= ngram_min <= ngram_max <= {SPEC_MAX_NGRAM}, got {k}, {nmin}, {nmax}")
+    _req_cuda(tokens, cands, row_indptr, history, lengths, out)
+    b = row_indptr.numel() - 1
+    nslots, cap = history.shape
+    if b < 1 or any(x.dtype != torch.int32 or not x.is_contiguous() for x in (tokens, cands, row_indptr, history, lengths, out)):
+        raise RuntimeError("atom_b200.ops.spec_commit_propose: all tensors must be contiguous int32, with at least one sequence")
+    if tokens.shape != cands.shape or tuple(lengths.shape) != (nslots,) or tuple(out.shape) != (b, 2 * k + 3):
+        raise RuntimeError(f"atom_b200.ops.spec_commit_propose: tokens and cands [R], lengths [{nslots}], out [{b}, {2 * k + 3}]")
+    if cap < k + 1:
+        raise RuntimeError(f"atom_b200.ops.spec_commit_propose: cap={cap} must hold at least num_draft + 1 tokens")
+    if not isinstance(slots, torch.Tensor):
+        import numpy as np
+        a = np.asarray(slots, dtype=np.int64).reshape(-1)
+        if a.shape != (b,) or (a < 0).any() or (a >= nslots).any() or len(np.unique(a)) != b:
+            raise RuntimeError(f"atom_b200.ops.spec_commit_propose: `slots` must hold {b} distinct entries in [0, {nslots})")
+        slots = torch.from_numpy(a.astype(np.int32)).to(history.device)
+    elif slots.dtype != torch.int32 or tuple(slots.shape) != (b,) or not slots.is_cuda:
+        raise RuntimeError(f"atom_b200.ops.spec_commit_propose: `slots` must be int32 [{b}]")
+    with torch.cuda.device(history.device):
+        _lib.check(_lib.lib().atom_spec_commit_propose(tokens.data_ptr(), cands.data_ptr(), row_indptr.data_ptr(), slots.data_ptr(), b,
+                                                       history.data_ptr(), lengths.data_ptr(), nslots, cap, k, nmin, nmax,
+                                                       out.data_ptr(), _stream(history)), "spec_commit_propose")
+    return out

@@ -135,6 +135,23 @@ class SamplingParams:
         return {k: v for k, v in d.items() if k not in self._EXTRAS or v != self._EXTRAS[k]}
 
 
+@dataclasses.dataclass(frozen=True)
+class SpeculativeParams:
+    """Speculative decoding with prompt-lookup drafts (DESIGN sections 5.7 and 5.8).  After every step the device commits each
+    sequence's accepted tokens to its token history (its whole context: the shared system prompt, its prompt and its generated
+    tokens) and proposes up to num_draft drafts: the tokens that followed the latest earlier occurrence of the history's last
+    n tokens, for the longest n in [ngram_min, ngram_max] that occurs.  The next step carries S = 1 + the longest draft of the
+    batch tokens per running sequence (S = 1: a plain decode step), and the sampler accepts or replaces each draft so that
+    greedy runs give the greedy tokens and sampled runs draw from exactly the sampler's distribution."""
+    num_draft: int = 4
+    ngram_max: int = 3
+    ngram_min: int = 1
+
+    def __post_init__(self):
+        if not (1 <= int(self.num_draft) <= 7 and 1 <= int(self.ngram_min) <= int(self.ngram_max) <= 16):
+            raise ValueError(f"need 1 <= num_draft <= 7 and 1 <= ngram_min <= ngram_max <= 16: {self}")
+
+
 @dataclasses.dataclass
 class TextGenConfig:
     batch_size: int
@@ -142,6 +159,7 @@ class TextGenConfig:
     shared_prefix: int = 0                  # tokens of one system prompt before every request's prompt, prefilled once and forked
     sampling: Optional[SamplingParams] = None   # None: greedy (argmax)
     stop_token_ids: Tuple[int, ...] = ()        # a request that emits one of these finishes on it (greedy or sampled)
+    speculate: Optional[SpeculativeParams] = None   # None: one token per running request and step
 
 
 @dataclasses.dataclass
@@ -156,6 +174,7 @@ class TextGenBenchResult:
     output_lens: Optional[np.ndarray] = None    # tokens each request generated (fewer than asked when it met a stop id)
     logprobs: Optional[List[List[float]]] = None    # with SamplingParams.logprobs and keep_tokens: each token's log-probability
     top_logprobs: Optional[List[List[Tuple[List[int], List[float]]]]] = None    # ... and each token's top-n (ids, logprobs)
+    speculative: Optional[dict] = None      # with speculation: TextGenScheduler.spec_stats
 
 
 @dataclasses.dataclass
@@ -169,6 +188,7 @@ class RequestContext:
     slot: int = -1                          # its penalty-table slot (-1: none)
     logprobs: List[float] = dataclasses.field(default_factory=list)
     top_logprobs: List[tuple] = dataclasses.field(default_factory=list)
+    drafts: List[int] = dataclasses.field(default_factory=list)     # with speculation: the next step's drafts
 
 
 @dataclasses.dataclass(eq=False)
@@ -210,10 +230,18 @@ class TextGenScheduler:
     penalty_slots=True: every admitted request takes a slot of a penalty table of batch_size slots (the smallest free one), to be
     set up with its whole prompt -- the system prompt and its own -- before its first token is drawn: `slot_inits` lists the
     (slot, prompt tokens) the driver must apply after each admit().  The slot is freed when the request finishes; the system
-    prompt's root sequence has none."""
+    prompt's root sequence has none.
+
+    num_draft=K (> 0, speculative decoding; needs slots, which then index the device token histories): a running request carries
+    the drafts the device proposed for it after the previous step.  A step carries S = 1 + the longest of them rows per running
+    request -- [last token, drafts, padding] -- after the prompt chunks; admit() grows each running sequence by S - 1 tokens for
+    them and keeps pages in reserve for every running request to grow by K + 1 tokens.  commit_spec() takes the device's per-
+    sequence result (tokens emitted, drafts), cuts the tokens at the output length and the first stop id, and truncates each
+    sequence to the tokens it kept."""
 
     def __init__(self, rs: RequestSet, batch_size: int, pool: KvPoolInt4, device, vocab_size: int = 32000,
-                 prefill_chunk: Optional[int] = None, shared_prefix: int = 0, stop_token_ids=(), penalty_slots: bool = False):
+                 prefill_chunk: Optional[int] = None, shared_prefix: int = 0, stop_token_ids=(), penalty_slots: bool = False,
+                 num_draft: int = 0):
         if prefill_chunk is not None and int(prefill_chunk) < 1:
             raise ValueError("prefill_chunk must be a positive number of tokens (or None)")
         if int(shared_prefix) < 0:
@@ -238,6 +266,12 @@ class TextGenScheduler:
         self.stop_token_ids = frozenset(int(t) for t in stop_token_ids)
         self._free_slots = list(range(batch_size)) if penalty_slots else None
         self.slot_inits: List[tuple] = []
+        self.num_draft = int(num_draft)
+        if self.num_draft and self._free_slots is None:
+            raise ValueError("speculation needs slots (penalty_slots=True): they index the token histories")
+        self.S = 1                                  # rows per running request in the admitted step
+        self.spec_stats = {"verify_steps": 0, "drafted_tokens": 0, "accepted_tokens": 0, "emitted_tokens": 0,
+                           "verify_sequence_steps": 0, "verify_emitted_tokens": 0}
 
     @property
     def finished(self) -> bool:
@@ -252,6 +286,10 @@ class TextGenScheduler:
         # the prompt's pages plus one spare: the first generated token may open a new page.  Behind a shared prefix of N tokens
         # a fork takes the pages from N // P on: a copy of the partly filled page, if any, and the pages its prompt adds
         n, bl = self.shared_prefix, self.pool.block_len
+        if self.num_draft:
+            # speculating, the spare is room for the first token and for its first step as a running request, which can grow
+            # the sequence by K + 1 more tokens
+            return -(-(n + prompt_len + 1 + self.num_draft + 1) // bl) - n // bl
         return (n + prompt_len + bl - 1) // bl - n // bl + 1
 
     def _outstanding(self, p: _Prefill) -> int:
@@ -268,6 +306,9 @@ class TextGenScheduler:
         # running requests may each need a fresh page this step, and the requests being prefilled the pages of the rest of
         # their prompt: keep those in reserve before admitting anyone, so that no admitted request ever waits for a page
         reserve = len(self.workset) + sum(self._outstanding(p) for p in self._prefilling)
+        if self.num_draft:                          # ... or, speculating, pages for K + 1 more tokens
+            bl = self.pool.block_len
+            reserve += sum(-(-(r.kvcache.seqlen + self.num_draft + 1) // bl) - len(r.kvcache.indicies) - 1 for r in self.workset)
         for p in self._prefilling:
             if budget is not None and budget == 0:
                 break
@@ -302,6 +343,9 @@ class TextGenScheduler:
             self._new.append((p, 0, n))
             reserve += self._outstanding(p)
             budget = None if budget is None else budget - n
+        self.S = 1 + max((len(r.drafts) for r in self.workset), default=0)
+        for r in self.workset:                      # the verify rows' K/V slots (from the reserve)
+            r.kvcache.acquire(self.S - 1)
         self._admitted = True
         return len(self._new)
 
@@ -313,8 +357,8 @@ class TextGenScheduler:
         input_ids: List[int] = []
         for p, s, n in self._new:
             input_ids.extend(p.prompt[s:s + n])
-        input_ids.extend(int(r.output[-1]) for r in self.workset)
-        self._blen = BatchLenInfo([n for _, _, n in self._new], len(self.workset), self.device)
+        input_ids.extend(self.decode_ids())
+        self._blen = BatchLenInfo([n for _, _, n in self._new], len(self.workset), self.device, decode_len=self.S)
         prefill_kv = BatchedKvCacheInt4([p.kvcache for p, _, _ in self._new]) if self._new else None
         decode_kv = BatchedKvCacheInt4([r.kvcache for r in self.workset]) if self.workset else None
         return StepBatch(input_ids, self._blen, prefill_kv, decode_kv, len(self._new))
@@ -327,21 +371,51 @@ class TextGenScheduler:
         chunks = getattr(self, "_new", None)        # None: a bare step description, whole prompts only
         if chunks is not None:
             rows = [r for r, (p, s, n) in zip(rows, chunks) if s + n == len(p.prompt) and p.req_idx >= 0]
-        return rows + list(range(blen.doff, blen.doff + blen.decode))
+        return rows + list(range(blen.doff, blen.doff + blen.decode * blen.decode_len))
+
+    def _first(self) -> list:
+        """The requests whose first token this step draws (prompts it completes, the system prompt's root excluded)."""
+        return [p for p, s, n in (getattr(self, "_new", None) or []) if s + n == len(p.prompt) and p.req_idx >= 0]
+
+    def decode_ids(self) -> List[int]:
+        """Input ids of the running requests' rows: the last token, then (speculating) the drafts and padding up to S rows."""
+        out: List[int] = []
+        for r in self.workset:
+            row = [int(r.output[-1])] + r.drafts
+            out.extend(row + [row[-1]] * (self.S - len(row)))
+        return out
+
+    def candidates(self) -> List[int]:
+        """Speculating: the candidate of every row of last_token_rows() (-1: none): row j of a running request proposes its
+        draft j, the token its input at row j + 1 assumed."""
+        out = [-1] * len(self._first())
+        for r in self.workset:
+            out.extend(r.drafts + [-1] * (self.S - len(r.drafts)))
+        return out
+
+    def sequence_rows(self) -> List[int]:
+        """Speculating: the rows of last_token_rows() of each sequence that draws (those of sequence_slots()), as an indptr."""
+        counts = [1] * len(self._first()) + [self.S] * len(self.workset)
+        return np.concatenate([[0], np.cumsum(counts, dtype=np.int64)]).astype(np.int32).tolist()
+
+    def sequence_slots(self) -> List[int]:
+        """Speculating: the token-history slot of each sequence that draws, first tokens first, then the running requests."""
+        return [p.slot for p in self._first()] + [r.slot for r in self.workset]
 
     def sample_slots(self) -> List[tuple]:
         """(request index, counter) of every row of last_token_rows(), in its order: the counter is the number of tokens the
         request has generated so far (0 for the row that completes its prompt)."""
         chunks = getattr(self, "_new", None) or []
         first = [(p.req_idx, 0) for p, s, n in chunks if s + n == len(p.prompt) and p.req_idx >= 0]
-        return first + [(r.req_idx, len(r.output)) for r in self.workset]
+        return first + [(r.req_idx, len(r.output) + j) for r in self.workset for j in range(self.S)]
 
     def row_slots(self) -> List[int]:
         """The penalty-table slot of every row of last_token_rows(), in its order (-1: none)."""
         chunks = getattr(self, "_new", None) or []
-        return [p.slot for p, s, n in chunks if s + n == len(p.prompt) and p.req_idx >= 0] + [r.slot for r in self.workset]
+        return [p.slot for p, s, n in chunks if s + n == len(p.prompt) and p.req_idx >= 0] + \
+            [r.slot for r in self.workset for _ in range(self.S)]
 
-    def commit(self, next_tokens, t1: float, t2: float, logprobs=None) -> int:
+    def commit(self, next_tokens, t1: float, t2: float, logprobs=None, _speculative=False) -> int:
         """next_tokens: one id per row of last_token_rows(); logprobs: None or (logprob [R], top_ids [R, n], top_logprobs [R, n])
         for the same rows.  Returns the number of tokens this step processed."""
         completes = [s + n == len(p.prompt) for p, s, n in self._new]
@@ -350,6 +424,7 @@ class TextGenScheduler:
         processed = sum(n for _, _, n in self._new) + len(self.workset)
         new_workset: List[RequestContext] = []
         b = 0
+        first = []
         for (p, _, n), c in zip(self._new, completes):
             p.done += n
             if p.start_at is None:
@@ -363,12 +438,57 @@ class TextGenScheduler:
                                  slot=p.slot)
             self._keep_logprobs(req, logprobs, b)
             b += 1
+            first.append(req)
             self._finish_or_continue(req, t2, new_workset)
+        if _speculative:                            # commit_spec() goes on with the running requests
+            self._first_committed, self._first_workset, self._running_committed = first, new_workset, self.workset
+            self._new, self._admitted = [], False
+            return processed
         for i, req in enumerate(self.workset):
             req.output.append(int(next_tokens[n_first + i]))
             self._keep_logprobs(req, logprobs, n_first + i)
             self._finish_or_continue(req, t2, new_workset)
         self.workset, self._new, self._admitted = new_workset, [], False
+        return processed
+
+    def commit_spec(self, out, t1: float, t2: float, logprobs=None) -> int:
+        """Speculating: out int32 [sequences, 2K + 3], one row per sequence of sequence_slots() (ops.spec_commit_propose: tokens
+        emitted, drafts proposed, the tokens, the drafts); logprobs as commit()'s, for the rows of last_token_rows().  Returns the
+        number of tokens this step processed."""
+        K, S = self.num_draft, self.S
+        out = np.asarray(out)
+        first, rows = len(self._first()), self.sequence_rows()
+        seq_drafts = [[int(t) for t in o[K + 3:K + 3 + int(o[1])]] for o in out]
+        tokens = [[int(t) for t in o[2:2 + int(o[0])]] for o in out]
+        processed = sum(n for _, _, n in self._new) + S * len(self.workset)
+        if S > 1:
+            st = self.spec_stats
+            st["verify_steps"] += 1
+            st["verify_sequence_steps"] += len(self.workset)
+        self.commit([t[0] for t in tokens[:first]] + [0] * len(self.workset), t1, t2, logprobs, _speculative=True)
+        for req, d in zip(self._first_committed, seq_drafts[:first]):
+            req.drafts = d
+        new_workset = self._first_workset
+        for i, req in enumerate(self._running_committed):
+            seq, drafted = first + i, len(req.drafts)
+            kept = 0
+            for j, t in enumerate(tokens[seq]):
+                req.output.append(t)
+                self._keep_logprobs(req, logprobs, rows[seq] + j)
+                kept += 1
+                if len(req.output) >= int(self.rs.output_lens[req.req_idx]) or t in self.stop_token_ids:
+                    break
+            st = self.spec_stats
+            st["emitted_tokens"] += kept
+            st["accepted_tokens"] += min(kept - 1, drafted) if kept else 0
+            if S > 1:
+                st["drafted_tokens"] += drafted
+                st["verify_emitted_tokens"] += kept
+            if not self._finishes(req):
+                req.kvcache.truncate(req.kvcache.seqlen - S + kept)
+            req.drafts = seq_drafts[seq]
+            self._finish_or_continue(req, t2, new_workset)
+        self.workset = new_workset
         return processed
 
     @staticmethod
@@ -378,8 +498,11 @@ class TextGenScheduler:
             req.logprobs.append(float(lp[row]))
             req.top_logprobs.append(([int(t) for t in ids[row]], [float(x) for x in lps[row]]))
 
+    def _finishes(self, req) -> bool:
+        return len(req.output) >= int(self.rs.output_lens[req.req_idx]) or req.output[-1] in self.stop_token_ids
+
     def _finish_or_continue(self, req, t2, new_workset):
-        if len(req.output) >= int(self.rs.output_lens[req.req_idx]) or req.output[-1] in self.stop_token_ids:
+        if self._finishes(req):
             req.decode_latency = t2 - req.decode_start_at
             req.kvcache.release()
             if req.slot >= 0:
@@ -437,10 +560,19 @@ class DecodeGraphRunner:
     freq(B) | pres(B)]  (FP32 bit patterns), the step also passes `penalty_table` (set by run_textgen) and, with logprobs, returns
     (tokens, logprob, top_ids, top_logprobs).  Otherwise the buffer and the step are exactly the above.
 
+    With `speculate` (SpeculativeParams) every step -- graphs keyed on (B, prefix groups, S) -- carries S rows per sequence and
+    ends with the draft sampler (`draft_sample_op`, ops.sample_tokens with drafts; at T = 0 when greedy) and the commit and
+    proposal (`propose_op`, ops.spec_commit_propose) on the token histories set by use_history().  Its buffer is
+    [ids(BS) | indptr(B+1) | last_page_offset(B) | indicies(B * max_pages) | groups (S = 1 only) | candidates(BS) |
+    row_indptr(B+1) | history slots(B) | keys(2BS x u64) | counters(BS x u64) | top_k(BS) | T(BS) | top_p(BS) | min_p(BS)], one
+    H2D copy; a verify step (S > 1) passes BatchLenInfo(decode_len=S, max_len=max_pages * page size) and no groups.  The step
+    returns the proposer's output [B, 2K + 3] (and, with logprobs, the sampler's per-row log-probabilities).
+
     capture=False runs the same buffers through the model eagerly (the CPU tests use it; it is also the warm-up path)."""
 
     def __init__(self, model: Callable, pool: KvPoolInt4, device, max_pages_per_seq: int, capture: bool = True,
-                 sampling: Optional[SamplingParams] = None, sample_op: Callable = None):
+                 sampling: Optional[SamplingParams] = None, sample_op: Callable = None,
+                 speculate: Optional[SpeculativeParams] = None, propose_op: Callable = None, draft_sample_op: Callable = None):
         self.model, self.pool, self.device = model, pool, torch.device(device)
         self.max_pages, self.capture = max_pages_per_seq, capture
         self.sampling = sampling
@@ -450,6 +582,22 @@ class DecodeGraphRunner:
         self.sample_op = sample_op
         self.penalty_table = None
         self._entries = {}
+        self.speculate = speculate
+        self.history = None
+        if speculate is not None:
+            if sampling is not None and sampling.penalties:
+                raise ValueError("speculative decoding cannot be combined with penalties")
+            if propose_op is None or draft_sample_op is None:
+                from . import ops
+            self.propose_op = propose_op or ops.spec_commit_propose
+            self.draft_sample_op = draft_sample_op or ops.sample_tokens
+
+    def use_history(self, history):
+        """The (token histories, lengths) the speculative step commits to and proposes from; graphs captured with others are
+        dropped."""
+        if self.history is None or history[0] is not self.history[0] or history[1] is not self.history[1]:
+            self.history = history
+            self._entries = {}
 
     def use_table(self, table):
         """The penalty table the sampling step reads and updates; graphs captured with another one are dropped."""
@@ -530,6 +678,20 @@ class DecodeGraphRunner:
         o_ids, o_indptr, o_last, o_ind, o_grp, _ = self._layout(b, ng)
         h = e["host"].numpy()
         h[o_ids:o_ids + b] = last_tokens
+        self._fill_pages(h, kvs, o_indptr, o_last, o_ind)
+        self._fill_groups(h, e, groups, b, o_grp)
+        if self.sampling is not None:
+            o_key, o_ctr, o_k, o_t, o_p, _ = self._sampling_layout(b, ng)
+            sp = self.sampling
+            self._fill_draw(h, sp, slots, o_key, o_ctr, o_k, o_t, o_p, b)
+            if sp.extended:
+                o_sl, o_m, o_r, o_f, o_q, _ = self._ext_layout(b, ng)
+                h[o_sl:o_m] = row_slots if sp.penalties else -1
+                for o, v in ((o_m, sp.min_p), (o_r, sp.repetition_penalty), (o_f, sp.frequency_penalty), (o_q, sp.presence_penalty)):
+                    h[o:o + b] = np.float32(v).view(np.int32)
+        return self._launch(e, self._step)
+
+    def _fill_pages(self, h, kvs, o_indptr, o_last, o_ind):
         n = 0
         h[o_indptr] = 0
         for i, c in enumerate(kvs):
@@ -540,6 +702,10 @@ class DecodeGraphRunner:
             n += len(pages)
             h[o_indptr + i + 1] = n
             h[o_last + i] = (c.seqlen - 1) % self.pool.block_len + 1
+
+    @staticmethod
+    def _fill_groups(h, e, groups, b, o_grp):
+        ng = len(groups)
         if ng:
             members = [r for rows, _ in groups for r in rows]
             h[o_grp:o_grp + ng + 1] = np.cumsum([0] + [len(rows) for rows, _ in groups])
@@ -549,40 +715,118 @@ class DecodeGraphRunner:
             for rows, n in groups:
                 shared[rows] = n
             e["kv"].groups = groups              # the host view: it decides, when the step is captured, which decode runs
-        if self.sampling is not None:
-            o_key, o_ctr, o_k, o_t, o_p, _ = self._sampling_layout(b, ng)
-            sp = self.sampling
-            words = np.array([w for r, _ in slots for w in (int(sp.seed), r)], dtype=np.uint64)
-            h[o_key:o_ctr] = words.view(np.int32)
-            h[o_ctr:o_k] = np.array([c for _, c in slots], dtype=np.uint64).view(np.int32)
-            h[o_k:o_t] = int(sp.top_k)
-            h[o_t:o_p] = np.float32(sp.temperature).view(np.int32)
-            h[o_p:o_p + b] = np.float32(sp.top_p).view(np.int32)
-            if sp.extended:
-                o_sl, o_m, o_r, o_f, o_q, _ = self._ext_layout(b, ng)
-                h[o_sl:o_m] = row_slots if sp.penalties else -1
-                for o, v in ((o_m, sp.min_p), (o_r, sp.repetition_penalty), (o_f, sp.frequency_penalty), (o_q, sp.presence_penalty)):
-                    h[o:o + b] = np.float32(v).view(np.int32)
+
+    @staticmethod
+    def _fill_draw(h, sp, slots, o_key, o_ctr, o_k, o_t, o_p, n):
+        words = np.array([w for r, _ in slots for w in (int(sp.seed), r)], dtype=np.uint64)
+        h[o_key:o_ctr] = words.view(np.int32)
+        h[o_ctr:o_k] = np.array([c for _, c in slots], dtype=np.uint64).view(np.int32)
+        h[o_k:o_t] = int(sp.top_k)
+        h[o_t:o_p] = np.float32(sp.temperature).view(np.int32)
+        h[o_p:o_p + n] = np.float32(sp.top_p).view(np.int32)
+
+    def _launch(self, e, step):
         e["dev"].copy_(e["host"], non_blocking=True)
         if not self.capture:
-            return _to_numpy(self._step(e))
+            return _to_numpy(step(e))
         if e["graph"] is None:
             side = torch.cuda.Stream(self.device)
             side.wait_stream(torch.cuda.current_stream(self.device))
             with torch.cuda.stream(side):
                 table = self.penalty_table if self.sampling is not None and self.sampling.penalties else None
-                saved = None if table is None else table.clone()
-                self._step(e)                       # warm-up on real data (lazy initialisations must not be captured)
-                if saved is not None:
-                    table.copy_(saved)              # the warm-up's draw was recorded: the replay below is the step's draw
+                state = ([table] if table is not None else []) + (list(self.history) if self.speculate is not None else [])
+                saved = [t.clone() for t in state]
+                step(e)                             # warm-up on real data (lazy initialisations must not be captured)
+                for t, v in zip(state, saved):
+                    t.copy_(v)                      # the warm-up's draw was recorded: the replay below is the step's draw
                 side.synchronize()
                 g = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(g, stream=side):
-                    e["out"] = self._step(e)
+                    e["out"] = step(e)
             torch.cuda.current_stream(self.device).wait_stream(side)
             e["graph"] = g
         e["graph"].replay()
         return _to_numpy(e["out"])                  # synchronises: the caller needs the tokens to go on
+
+    # ---- speculative steps
+    def _spec_layout(self, b, ng, S):
+        """int32 offsets: ids, indptr, last, indicies, groups, candidates, row_indptr, history slots, keys, counters, top_k, T,
+        top_p, min_p and the total."""
+        R = b * S
+        o_ind = R + 2 * b + 1
+        o_grp = o_ind + b * self.max_pages
+        o_cand = o_grp + (ng + 1 + 2 * b if ng else 0)
+        o_rip = o_cand + R
+        o_hs = o_rip + b + 1
+        o_key = (o_hs + b + 1) // 2 * 2
+        o_ctr = o_key + 4 * R
+        o_k = o_ctr + 2 * R
+        return {"ids": 0, "indptr": R, "last": R + b + 1, "ind": o_ind, "grp": o_grp, "cand": o_cand, "rip": o_rip, "hs": o_hs,
+                "key": o_key, "ctr": o_ctr, "k": o_k, "t": o_k + R, "p": o_k + 2 * R, "m": o_k + 3 * R, "total": o_k + 4 * R}
+
+    def _spec_entry(self, b, ng, S):
+        e = self._entries.get((b, ng, S))
+        if e is None:
+            o, R = self._spec_layout(b, ng, S), b * S
+            host = torch.zeros(o["total"], dtype=torch.int32)
+            if self.device.type == "cuda":
+                host = host.pin_memory()
+            dev = torch.zeros(o["total"], dtype=torch.int32, device=self.device)
+            kv = _StaticKv(self.pool, dev[o["indptr"]:o["indptr"] + b + 1], dev[o["ind"]:o["ind"] + b * self.max_pages],
+                           dev[o["last"]:o["last"] + b])
+            g = o["grp"]
+            if ng:
+                kv.group_indptr = dev[g:g + ng + 1]
+                kv.group_members = dev[g + ng + 1:g + ng + 1 + b]
+                kv.shared_pages = dev[g + ng + 1 + b:g + ng + 1 + 2 * b]
+                kv.group_bounds = (b, self.max_pages)
+            blen = BatchLenInfo([], b, self.device) if S == 1 else \
+                BatchLenInfo([], b, self.device, decode_len=S, max_len=self.max_pages * self.pool.block_len)
+            f32 = lambda x: dev[o[x]:o[x] + R].view(torch.float32)      # noqa: E731
+            sp = self.sampling
+            ext = {}
+            if sp is not None and sp.min_p != 0:
+                ext["min_p"] = f32("m")
+            if sp is not None and sp.logprobs is not None:
+                ext["logprobs"] = int(sp.logprobs)
+            K = self.speculate.num_draft
+            e = {"host": host, "dev": dev, "ids": dev[:R], "kv": kv, "blen": blen, "graph": None, "out": None, "ext": ext,
+                 "sample": (f32("t"), dev[o["k"]:o["k"] + R], f32("p"), dev[o["key"]:o["ctr"]].view(torch.int64).view(R, 2),
+                            dev[o["ctr"]:o["k"]].view(torch.int64)),
+                 "cands": dev[o["cand"]:o["cand"] + R], "rip": dev[o["rip"]:o["rip"] + b + 1], "hs": dev[o["hs"]:o["hs"] + b],
+                 "spec_out": torch.zeros((b, 2 * K + 3), dtype=torch.int32, device=self.device)}
+            self._entries[(b, ng, S)] = e
+        return e
+
+    def _spec_step(self, e):
+        logits, _ = self.model(e["ids"], e["blen"], None, e["kv"])
+        out = self.draft_sample_op(logits, *e["sample"], drafts=e["cands"], **e["ext"])
+        tokens = out[0] if isinstance(out, tuple) else out
+        sp = self.speculate
+        self.propose_op(tokens, e["cands"], e["rip"], e["hs"], self.history[0], self.history[1], e["spec_out"], sp.num_draft,
+                        sp.ngram_min, sp.ngram_max)
+        return (e["spec_out"],) + tuple(out[1:]) if isinstance(out, tuple) else e["spec_out"]
+
+    def run_spec(self, S: int, ids: List[int], cands: List[int], kvs: List[KvCacheInt4], slots: List[tuple], hist_slots: List[int]):
+        """A speculative step of S rows per sequence (TextGenScheduler: S, decode_ids, candidates, sample_slots, sequence_slots;
+        the sequences' pages already hold the S rows).  Returns the proposer's output [B, 2K + 3] (with logprobs, and then the
+        sampler's logprob, top_ids, top_logprobs per row), as numpy arrays."""
+        b = len(kvs)
+        groups = prefix_groups(kvs) if S == 1 else []
+        ng = len(groups)
+        e = self._spec_entry(b, ng, S)
+        o, R = self._spec_layout(b, ng, S), b * S
+        h = e["host"].numpy()
+        h[:R] = ids
+        self._fill_pages(h, kvs, o["indptr"], o["last"], o["ind"])
+        self._fill_groups(h, e, groups, b, o["grp"])
+        h[o["cand"]:o["cand"] + R] = cands
+        h[o["rip"]:o["rip"] + b + 1] = np.arange(0, R + 1, S)
+        h[o["hs"]:o["hs"] + b] = hist_slots
+        sp = self.sampling if self.sampling is not None else SamplingParams(0.0)
+        self._fill_draw(h, sp, slots, o["key"], o["ctr"], o["k"], o["t"], o["p"], R)
+        h[o["m"]:o["m"] + R] = np.float32(sp.min_p).view(np.int32)
+        return self._launch(e, self._spec_step)
 
 
 def _to_numpy(out):
@@ -598,15 +842,19 @@ def _vocab_size(model) -> int:
     return int(getattr(cfg, "vocab_size", 32000))
 
 
-def pool_capacity(batch_size: int, maxlen: int, block_len: int) -> int:
-    """Pages for `batch_size` sequences of up to `maxlen` tokens (+1 spare page each), bench_textgen.py:99."""
-    return batch_size * ((maxlen + block_len - 1) // block_len + 1)
+def pool_capacity(batch_size: int, maxlen: int, block_len: int, num_draft: int = 0) -> int:
+    """Pages for `batch_size` sequences of up to `maxlen` tokens (+1 spare page each), bench_textgen.py:99.  With num_draft = K
+    (speculative decoding) each sequence also gets the pages of K + 1 more tokens: a verify step grows a sequence by up to K
+    tokens past its length and the commit by one more, so every request can reach its full length without waiting for a page
+    in the middle of a step."""
+    return batch_size * ((maxlen + block_len - 1) // block_len + 1 + (-(-(num_draft + 1) // block_len) if num_draft else 0))
 
 
 @torch.inference_mode()
 def run_textgen(model: Callable, rs: RequestSet, cfg: TextGenConfig, pool: KvPoolInt4, device, sync: Callable = None,
                 keep_tokens: bool = False, progress: Callable = None, decode_runner: DecodeGraphRunner = None,
-                sample_op: Callable = None, slot_init_op: Callable = None) -> TextGenBenchResult:
+                sample_op: Callable = None, slot_init_op: Callable = None, propose_op: Callable = None,
+                draft_sample_op: Callable = None) -> TextGenBenchResult:
     """Drive `model(input_ids, blen, prefill_kv, decode_kv) -> (logits, hidden)` through the whole request set.
     Latencies are wall-clock around the step *including* the device->host read of the next tokens (which synchronises),
     as in the reference.  With a `decode_runner`, steps that carry no prompt tokens are replayed from its CUDA graphs.
@@ -615,13 +863,22 @@ def run_textgen(model: Callable, rs: RequestSet, cfg: TextGenConfig, pool: KvPoo
     must have been built with the same SamplingParams, samples in its graphs.  With penalties a penalty table of
     cfg.batch_size slots is made on `device` (ops.penalty_table) and each admitted request's slot is set up by `slot_init_op`
     (default ops.init_penalty_slot) before its first token; the runner is given the same table.  cfg.stop_token_ids: see
-    TextGenScheduler."""
+    TextGenScheduler.
+    cfg.speculate: token histories of cfg.batch_size slots (ops.spec_history) hold each request's context, set up at admission
+    (ops.spec_init_slot); every step samples with `draft_sample_op` (default ops.sample_tokens with drafts, at T = 0 when
+    greedy) and then commits and proposes with `propose_op` (default ops.spec_commit_propose); the runner must have been built
+    with the same SpeculativeParams and is given the same histories.  Not with penalties."""
     sp = cfg.sampling
     if sp is not None and sample_op is None:
         from . import ops
         sample_op = ops.sample_tokens
     if decode_runner is not None and decode_runner.sampling != sp:
         raise ValueError("decode_runner was built for other sampling parameters than cfg.sampling")
+    spec = cfg.speculate
+    if spec is not None and sp is not None and sp.penalties:
+        raise ValueError("speculative decoding cannot be combined with penalties")
+    if decode_runner is not None and decode_runner.speculate != spec:
+        raise ValueError("decode_runner was built for other speculative parameters than cfg.speculate")
     vocab = _vocab_size(model)
     table = None
     if sp is not None and sp.penalties:
@@ -634,19 +891,65 @@ def run_textgen(model: Callable, rs: RequestSet, cfg: TextGenConfig, pool: KvPoo
             slot_init_op = ops.init_penalty_slot
         if decode_runner is not None:
             decode_runner.use_table(table)
+    hist = None
+    if spec is not None:
+        from . import ops
+        propose_op = propose_op or ops.spec_commit_propose
+        draft_sample_op = draft_sample_op or ops.sample_tokens
+        # every token a request's history can hold: its context, its output and the drafts a last step may commit past it
+        cap = cfg.shared_prefix + int(rs.prompt_lens.max()) + int(rs.output_lens.max()) + spec.num_draft + 1
+        old = None if decode_runner is None else decode_runner.history
+        if old is not None and old[0].size(0) == cfg.batch_size and old[0].size(1) >= cap and \
+                old[0].device == torch.empty(0, device=device).device:
+            hist = old                      # its graphs stay valid; every slot is set up again at admission
+        else:
+            hist = ops.spec_history(cfg.batch_size, cap, device)
+        if decode_runner is not None:
+            decode_runner.use_history(hist)
+    gsp = sp if sp is not None else SamplingParams(0.0)     # speculating, greedy is the draft sampler at T = 0
     sched = TextGenScheduler(rs, cfg.batch_size, pool, device, vocab_size=vocab, prefill_chunk=cfg.prefill_chunk,
-                             shared_prefix=cfg.shared_prefix, stop_token_ids=cfg.stop_token_ids, penalty_slots=table is not None)
+                             shared_prefix=cfg.shared_prefix, stop_token_ids=cfg.stop_token_ids,
+                             penalty_slots=table is not None or spec is not None, num_draft=0 if spec is None else spec.num_draft)
     steps = graphed = peak = 0
     t_start = time.perf_counter()
     while not sched.finished:
         sched.admit()
         for slot, prompt in sched.slot_inits:
-            slot_init_op(table, slot, prompt)
+            if table is not None:
+                slot_init_op(table, slot, prompt)
+            if hist is not None:
+                ops.spec_init_slot(hist[0], hist[1], slot, prompt)
         sched.slot_inits.clear()
         peak = max(peak, pool.capacity - pool.num_free_blocks)
         t1 = time.perf_counter()
         logprobs = None
-        if decode_runner is not None and sched.prompt_tokens == 0:
+        if spec is not None and decode_runner is not None and sched.prompt_tokens == 0:
+            out = decode_runner.run_spec(sched.S, sched.decode_ids(), sched.candidates(), [r.kvcache for r in sched.workset],
+                                         sched.sample_slots(), sched.sequence_slots())
+            next_tokens, logprobs = (out[0], out[1:]) if isinstance(out, tuple) else (out, None)
+            graphed += 1
+        elif spec is not None:
+            batch = sched.next_batch()
+            ids = torch.tensor(batch.input_ids, dtype=torch.long, device=device)
+            logits, _ = model(ids, batch.blen, batch.prefill_kv, batch.decode_kv)
+            rows = torch.tensor(sched.last_token_rows(), dtype=torch.long, device=logits.device)
+            slots = sched.sample_slots()
+            n = len(slots)
+            i32 = lambda x: torch.tensor(x, dtype=torch.int32, device=logits.device)      # noqa: E731
+            cands = i32(sched.candidates())
+            opts = {} if gsp.min_p == 0 else {"min_p": [gsp.min_p] * n}
+            if gsp.logprobs is not None:
+                opts["logprobs"] = int(gsp.logprobs)
+            out = draft_sample_op(logits.index_select(0, rows), [gsp.temperature] * n, [gsp.top_k] * n, [gsp.top_p] * n,
+                                  [(int(gsp.seed), r) for r, _ in slots], [c for _, c in slots], drafts=cands, **opts)
+            res_out = torch.empty((len(sched.sequence_slots()), 2 * spec.num_draft + 3), dtype=torch.int32, device=logits.device)
+            if len(res_out):                        # (a step of prompt chunks alone draws nothing)
+                propose_op(out[0] if isinstance(out, tuple) else out, cands, i32(sched.sequence_rows()), i32(sched.sequence_slots()),
+                           hist[0], hist[1], res_out, spec.num_draft, spec.ngram_min, spec.ngram_max)
+            next_tokens = res_out.cpu().numpy()
+            if isinstance(out, tuple):
+                logprobs = _to_numpy(out[1:])
+        elif decode_runner is not None and sched.prompt_tokens == 0:
             next_tokens = decode_runner.run([int(r.output[-1]) for r in sched.workset], [r.kvcache for r in sched.workset],
                                             sched.sample_slots() if sp is not None else None,
                                             sched.row_slots() if table is not None else None)
@@ -673,13 +976,18 @@ def run_textgen(model: Callable, rs: RequestSet, cfg: TextGenConfig, pool: KvPoo
         if sync is not None:
             sync()
         t2 = time.perf_counter()
-        n = sched.commit(next_tokens, t1, t2) if logprobs is None else sched.commit(next_tokens, t1, t2, logprobs)
+        if spec is not None:
+            n = sched.commit_spec(next_tokens, t1, t2, logprobs)
+        else:
+            n = sched.commit(next_tokens, t1, t2) if logprobs is None else sched.commit(next_tokens, t1, t2, logprobs)
         steps += 1
         if progress is not None:
             progress(n)
     res = sched.result(time.perf_counter() - t_start, steps, keep_tokens)
     res.graphed_steps = graphed
     res.peak_pages = peak
+    if spec is not None:
+        res.speculative = dict(sched.spec_stats)
     return res
 
 
@@ -703,4 +1011,14 @@ def report(rs: RequestSet, cfg: TextGenConfig, res: TextGenBenchResult) -> dict:
     }
     if cfg.stop_token_ids:
         out["stop_token_ids"] = [int(t) for t in cfg.stop_token_ids]
+    if cfg.speculate is not None and res.speculative is not None:
+        st, sp = res.speculative, cfg.speculate
+        out["speculative"] = {
+            "num_draft": sp.num_draft, "ngram_min": sp.ngram_min, "ngram_max": sp.ngram_max,
+            "verify_steps": st["verify_steps"], "drafted_tokens": st["drafted_tokens"], "accepted_tokens": st["accepted_tokens"],
+            "acceptance_rate": st["accepted_tokens"] / st["drafted_tokens"] if st["drafted_tokens"] else 0.0,
+            "emitted_tokens": st["emitted_tokens"],
+            "tokens_per_sequence_per_verify_step":
+                st["verify_emitted_tokens"] / st["verify_sequence_steps"] if st["verify_sequence_steps"] else 0.0,
+        }
     return out

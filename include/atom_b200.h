@@ -388,6 +388,37 @@ ATOM_API int atom_sample_ex_f16(const void* logits, int64_t ld, int batch, int v
                                 const void* freq, const void* pres, const void* slots, void* table, int64_t table_ld, void* out,
                                 void* logprob_out, int top_n, void* top_ids, void* top_logprobs, void* stream);
 
+/* atom_sample_draft_f16: sampling with one candidate token per row, for speculative decoding (new; DESIGN section 5.7).
+ * The arguments of atom_sample_ex_f16 without the penalty ones (rep, freq, pres, slots, table, table_ld), plus drafts i32 [batch],
+ * read on the device after the preceding kernel has completed.  Rules 1-4, min-p and the log-probabilities are atom_sample_ex_f16's
+ * and give the kept weights W (Z = sum of W).  Per row, d = drafts[b]:
+ *   - d = -1 (no candidate): rule 5; token, logprob and top-n are bit-identical to atom_sample_ex_f16's for the same row.
+ *   - d in [0, vocab): W_d = d's kept weight (0 if d is not kept); a = w1 >> 11, w1 = word 1 of rule 5's Philox block.  The row
+ *     accepts d iff floor(a * Z * 2^-53) < W_d (the exact 128-bit product of rule 5); then the token is d.  Otherwise the token
+ *     is rule 5's draw with word 0 over the kept set without d, whose total Z - W_d is then > 0.  So P(token = t) = W_t / Z up
+ *     to the 2^-53 discretisation of a and u, for every t.  T = 0 or top_k = 1: the first index of the maximum, whatever d.
+ *   - d < -1 or d >= vocab: -1, as any parameter out of range.
+ * logprob_out is the emitted token's; the top-n list does not depend on d or the draw. */
+ATOM_API int atom_sample_draft_f16(const void* logits, int64_t ld, int batch, int vocab, const void* temperature, const void* top_k,
+                                   const void* top_p, const void* key, const void* counter, const void* min_p, void* out,
+                                   void* logprob_out, int top_n, void* top_ids, void* top_logprobs, const void* drafts, void* stream);
+
+/* atom_spec_commit_propose: one launch per speculative step, one CTA per sequence (new; DESIGN section 5.8).  Token histories:
+ * history i32 [num_slots][cap], history_len i32 [num_slots].  Sequence i owns rows row_indptr[i] .. row_indptr[i+1] of tokens
+ * (the sampler's output) and cands (the candidates it was given, -1: none), and history slot slots[i].  The kernel
+ *   1. commits: m = the first j with cands[j] < 0 or tokens[j] != cands[j] (rows past num_draft + 1 are ignored); tokens 0 .. m
+ *      are emitted and appended to the slot, never past cap;
+ *   2. proposes by prompt lookup over the slot's history h[0, L): for n = ngram_max down to ngram_min, the latest p with
+ *      p + n <= L - 1 and h[p, p + n) == h[L - n, L); the drafts are h[p + n, min(p + n + num_draft, L)), and the first n that
+ *      matches wins; no match: no drafts;
+ *   3. writes out i32 [batch][2 * num_draft + 3]: emitted (m + 1), draft_len, the emitted tokens [num_draft + 1] and the drafts
+ *      [num_draft], both padded with -1.
+ * A slot outside [0, num_slots) gives emitted = draft_len = 0 and touches no history.  Needs 1 <= num_draft <= 7 and
+ * 1 <= ngram_min <= ngram_max <= 16.  Allocates nothing; all inputs are read after the preceding kernel has completed. */
+ATOM_API int atom_spec_commit_propose(const void* tokens, const void* cands, const void* row_indptr, const void* slots, int batch,
+                                      void* history, void* history_len, int num_slots, int cap, int num_draft, int ngram_min,
+                                      int ngram_max, void* out, void* stream);
+
 /* atom_sample_slot_init: set up slot `slot` of a penalty table u16 [*][table_ld] (16-byte aligned, table_ld >= vocab a multiple
  * of 8) for a new request in one launch: zero the row, then set bit 15 of every token in prompt i32 [prompt_len] (ids outside
  * [0, vocab) are ignored). */

@@ -64,6 +64,10 @@ def main():
                     help="with sampling: each token's log-probability and the top N (0 to 20)")
     ap.add_argument("--stop-token", type=int, action="append", default=[], metavar="ID",
                     help="a request that emits this id finishes on it (repeatable)")
+    ap.add_argument("--speculate", type=int, default=0, metavar="K",
+                    help="speculative decoding with up to K prompt-lookup drafts per sequence and step (0 = off; 1 to 7)")
+    ap.add_argument("--ngram-max", type=int, default=3, help="with --speculate: the longest n-gram the proposer matches")
+    ap.add_argument("--ngram-min", type=int, default=1, help="with --speculate: the shortest n-gram the proposer matches")
     ap.add_argument("--warmup-batches", type=int, default=1,
                     help="untimed request batches served first (first-use costs: lazy kernel loading, attribute calls, graph "
                          "capture); 0 = time the cold process like the reference's script")
@@ -84,15 +88,19 @@ def main():
     if args.temperature is None and tg.SamplingParams(1.0, **extra).extended:
         ap.error("--min-p, the penalties and --logprobs need --temperature")
     sampling = None if args.temperature is None else tg.SamplingParams(args.temperature, args.top_k, args.top_p, args.seed, **extra)
+    spec = tg.SpeculativeParams(args.speculate, args.ngram_max, args.ngram_min) if args.speculate else None
     cfg = tg.TextGenConfig(args.batch_size, prefill_chunk=args.prefill_chunk, shared_prefix=args.shared_prefix, sampling=sampling,
-                           stop_token_ids=tuple(args.stop_token))
+                           stop_token_ids=tuple(args.stop_token), speculate=spec)
+    # speculating, a sequence grows by up to K + 1 tokens past its length within a step: those pages too, per sequence
+    spec_pages = -(-(args.speculate + 1) // args.block_len) if spec else 0
     shared_pages = -(-args.shared_prefix // args.block_len)           # the system prompt's pages, held once
     pool = KvPoolInt4(layers, mc.kv_heads, mc.hidden_size // mc.num_heads,     # the cache holds KV heads (grouped-query: fewer)
-                      tg.pool_capacity(args.batch_size, args.maxlen, args.block_len) + shared_pages + args.batch_size * (shared_pages > 0),
+                      tg.pool_capacity(args.batch_size, args.maxlen, args.block_len) + shared_pages + args.batch_size * (shared_pages > 0)
+                      + args.batch_size * spec_pages,
                       args.block_len, device)
     runner = None if args.no_cuda_graphs else tg.DecodeGraphRunner(
-        model, pool, device, max_pages_per_seq=(args.maxlen + args.block_len - 1) // args.block_len + 1 + shared_pages,
-        sampling=sampling)
+        model, pool, device, max_pages_per_seq=(args.maxlen + args.block_len - 1) // args.block_len + 1 + shared_pages + spec_pages,
+        sampling=sampling, speculate=spec)
     if args.warmup_batches > 0:
         wrs = tg.generate_request_set(args.batch_size * args.warmup_batches, args.maxlen)
         tg.run_textgen(model, wrs, cfg, pool, device, sync=torch.cuda.synchronize, decode_runner=runner)
@@ -111,6 +119,10 @@ def main():
     print("duration:", f"{rep['duration_s']:.3f}s")
     print("throughput ((prompt+new)/duration):", f"{rep['throughput_tokens_per_s']:.3f} token/s")
     print("peak KV pages in use:", rep["peak_kv_pages_in_use"], f"of {pool.capacity}")
+    if spec is not None:
+        s = rep["speculative"]
+        print("speculative:", f"{s['verify_steps']} verify steps, {s['accepted_tokens']} of {s['drafted_tokens']} drafts accepted "
+              f"({s['acceptance_rate']:.3f}), {s['tokens_per_sequence_per_verify_step']:.3f} tokens per sequence per verify step")
     rep.update({"model": args.model, "layers": layers, "maxlen": args.maxlen, "kv_pool_pages": pool.buf.size(0),
                 "kv_pool_GB": round((pool.buf.numel() + 2 * pool.param.numel()) / 1e9, 2)})
     print(json.dumps(rep))
