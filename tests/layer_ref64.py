@@ -14,21 +14,33 @@ step:
   * its output must match the reference's own result for those inputs: quantisers bit exact (rmsnorm: +-1 code, 2e-3 on the scale,
     the kernel's rsqrtf is approximate; activate: +-1 code, expf), residual sums exact, GEMMs bit exact against the oracle at the
     K split the dispatcher picks for the call's M (and FP16 GEMMs and the INT4 K/V quantiser within gemm_ref64's float64
-    bounds), attention within attn_ref64's bound on a cache assembled from the reference's OWN history of K/V bytes (it never
-    reads the pool to compute attention).
+    bounds), attention within the float64 bound of its kind (attn_ref64: prompts, decode; attn_ctx_ref64: prompts over a
+    cached prefix; attn_verify_ref64: verify steps; attn_cascade_ref64: the shared-prefix cascade) on the reference's OWN
+    shadow of the pool (it never reads the pool to compute attention).
 Quantisation is discontinuous, so after checking a stage the reference continues from the kernel's value ("borrows" it): a rounding
 flip upstream cannot spread, and a wiring fault shows at the stage where it happens, named in the error.
-After the step, the pool is audited: every sequence's slots, in every layer, hold the bytes of the reference's history; every
-other byte is what it was before the step.
+The shadow is what the reference says each physical slot holds: (page, layer, K|V, entry) -> the K/V codes and (scale, zero),
+written by the stages it checked and by the fork hook (ModelRef.fork: a fork copies its partly filled page outside the recorded
+operators).  Pages shared by forks carry one history.  Sequences are known by where their history ends: the (page, entry) of a
+sequence's last cached token, its length and its pages.  A row of a step must continue a history the reference knows, at the
+length it expects -- after a verify step that is the length the kept tokens leave (ModelRef.keep, or check_spec from the emitted
+tokens) -- and may write only into pages no other holder has.
+Before the step, every history slot the step reads must hold the shadow's bytes; after it, the pool is audited: the slots the
+step wrote, in every layer, hold the shadow's bytes, and every other byte (slots past a sequence's length included) is what it
+was before the step.
 """
 import inspect
+from collections import Counter
 from dataclasses import dataclass, field
 
 import numpy as np
 
 from oracle import oracle as O
 from tests import attn_ref64 as A
+from tests import attn_verify_ref64 as VR
 from tests import gemm_ref64 as G
+from tests.attn_cascade_ref64 import cascade_bound
+from tests.attn_ctx_ref64 import prefill_ctx_bound
 from tests import moe_ref as ME
 
 U16 = 2.0 ** -11
@@ -44,7 +56,7 @@ GEMM_ARGS = {      # the operand names of each GEMM entry point: a, b, a_scale, 
                                        "b_keeper_scale_gu"),
 }
 RECORDED_OPS = ("rmsnorm_fp16_i4", "add_rmsnorm_fp16_i4", "dense_layer_gemm_i4_qkv", "init_kv_i4", "prefill_attention_i4",
-                "append_kv_i4", "batch_decode_i4", "reorder_fp16_i4", "dense_layer_gemm_i4_fp16", "dense_layer_gemm_i4_o4",
+                "append_kv_i4", "batch_decode_i4", "batch_verify_i4", "reorder_fp16_i4", "dense_layer_gemm_i4_fp16", "dense_layer_gemm_i4_o4",
                 "dense_layer_gemm_i4_gateup_act", "activate_fp16_i4", "moe_route_f16", "moe_plan", "moe_gather_i4",
                 "dense_layer_gemm_i4_gateup_act_grouped", "dense_layer_gemm_i4_fp16_grouped", "moe_combine_f16")
 
@@ -58,7 +70,10 @@ def host(x):
     if hasattr(x, "detach"):
         return x.detach().cpu().numpy().copy()
     if hasattr(x, "indptr") and hasattr(x, "last_page_offset"):
-        return {"indptr": host(x.indptr), "indices": host(x.indicies), "last": host(x.last_page_offset)}
+        tab = {"indptr": host(x.indptr), "indices": host(x.indicies), "last": host(x.last_page_offset)}
+        if getattr(x, "shared_pages", None) is not None:          # prefix groups (forked rows) and their shared page counts
+            tab.update(shared=host(x.shared_pages), groups=[(list(r), int(n)) for r, n in x.groups])
+        return tab
     if isinstance(x, (tuple, list)) and any(hasattr(t, "detach") for t in x):
         return tuple(host(t) for t in x)
     return x
@@ -209,20 +224,27 @@ class Step:
     x: np.ndarray = None
     out: tuple = None
     rows: list = None                      # the rows whose logits the caller reads (serving loop), None = not checked
+    decode_len: int = 1                    # S: rows of each running sequence (S > 1: a verify step)
+    refs: list = None                      # holders of every pool page before the step (None: not known)
     info: dict = field(default_factory=dict)
 
 
 class ModelRef:
     """The reference of a stack of LlamaDecoderLayers (or MixtralDecoderLayers) on one KV pool (page size P), optionally with the embedding, the final
-    LlamaRMSNorm and lm_head of LlamaForCausalLM (numpy copies: embed [V, H], norm (w, eps), lm_head [V, H])."""
+    LlamaRMSNorm and lm_head of LlamaForCausalLM (numpy copies: embed [V, H], norm (w, eps), lm_head [V, H]).  sm_count: the SMs
+    of the device the steps run on, for ops.decode_cascade's choice (None: the plain decode kernel is expected)."""
 
-    def __init__(self, layers, P, embed=None, norm=None, lm_head=None, row_cap=1 << 27, prefill_rows=None):
+    def __init__(self, layers, P, embed=None, norm=None, lm_head=None, row_cap=1 << 27, prefill_rows=None, sm_count=None):
         self.layers, self.P = layers, P
         self.embed, self.norm, self.lm_head = embed, norm, lm_head
         self.row_cap = row_cap              # an oracle GEMM above this many multiply-adds is checked on a row subset
         self.prefill_rows = prefill_rows    # rows of each prompt where attn_ref64 evaluates the exact spread term (None: all)
-        self.seqs = {}                      # key (first page) -> (pages, length)
-        self.hist = {}                      # (key, layer) -> [k u8 [n, Hkv, 64], k (s, z) [n, Hkv, 2], v, v (s, z)]
+        self.sm_count = sm_count
+        self.sd = self.sp = self.known = None   # shadow: K/V codes [pages, L, 2, Hkv, P, 64], (s, z) [.., 2], written [pages, L, P]
+        self.ends = {}                      # (page, entry) of a sequence's last cached token -> [length, its pages, holders]
+        self.worst = {}                     # attention kind -> largest |kernel - float64| / bound seen
+        self.calls = Counter()              # attention kind -> checked calls
+        self._rows_step, self._S = [], 1
 
     # ---------------------------------------------------------------------------------------------------------- checks
     def _where(self, st):
@@ -273,7 +295,6 @@ class ModelRef:
         for j in range(1, 4):
             if not (same(np.asarray(s8)[idx + 2 * j], np.asarray(s8)[idx]) and same(np.asarray(s4)[:, idx + 2 * j], np.asarray(s4)[:, idx])):
                 self._fail(st, "scale replicas differ")
-
     def _gemm_call(self, st, c, act, lin, flags=None):
         want = (act[1], lin.raw[0], act[3], lin.raw[1], act[0], lin.raw[2], act[2], lin.raw[3])
         for name, w in zip(GEMM_ARGS[c.name], want):
@@ -308,10 +329,12 @@ class ModelRef:
         except AssertionError as e:                                  # names the stage, (row, head) and element
             raise WiringError(str(e)) from None
 
-    def _attn_bound(self, st, got, ref, bnd):
+    def _attn_bound(self, st, got, ref, bnd, kind="attention"):
         ratio = np.abs(np.asarray(got, np.float64).reshape(ref.shape) - ref) / bnd
+        w = np.unravel_index(np.argmax(np.nan_to_num(ratio, nan=np.inf)), ratio.shape)
+        self.worst[kind] = max(self.worst.get(kind, 0.0), float(ratio[w]))
+        self.calls[kind] += 1
         if not (ratio <= 1).all():
-            w = np.unravel_index(np.argmax(np.nan_to_num(ratio, nan=np.inf)), ratio.shape)
             self._fail(st, f"attention output outside the float64 bound (x{ratio[w]:.3g} at {tuple(int(i) for i in w)})")
 
     def _table(self, st, got, want):
@@ -319,45 +342,150 @@ class ModelRef:
             if not same(np.asarray(got[k], np.int32), np.asarray(want[k], np.int32)):
                 self._fail(st, f"page table `{k}` {np.asarray(got[k]).tolist()} is not the step's {np.asarray(want[k]).tolist()}")
 
+    # ---------------------------------------------------------------------------------------------------------- shadow
+    def _ensure(self, pages):
+        """Grow the shadow to hold `pages`."""
+        n = max(pages, default=-1) + 1
+        if self.sd is None:
+            L, hkv = len(self.layers), self.layers[0].hkv
+            self.sd = np.zeros((0, L, 2, hkv, self.P, 64), np.uint8)
+            self.sp = np.zeros((0, L, 2, hkv, self.P, 2), np.float16)
+            self.known = np.zeros((0, L, self.P), bool)
+        if n > len(self.sd):
+            more = n - len(self.sd) + 8
+            self.sd = np.concatenate([self.sd, np.zeros((more,) + self.sd.shape[1:], np.uint8)])
+            self.sp = np.concatenate([self.sp, np.zeros((more,) + self.sp.shape[1:], np.float16)])
+            self.known = np.concatenate([self.known, np.zeros((more,) + self.known.shape[1:], bool)])
+
+    def _slots(self, pages, pos):
+        """(page, entry) index arrays of the positions `pos` of a sequence on `pages`."""
+        pos = np.asarray(pos)
+        return np.asarray(pages, np.int64)[pos // self.P], pos % self.P
+
+    def _write(self, l, pages, pos, k4, ks, v4, vs, hkv):
+        """The shadow takes what a checked cache write of layer l stores at positions `pos` (rows of k4 / ks / v4 / vs)."""
+        pg, e = self._slots(pages, pos)
+        self.sd[pg, l, 0, :, e], self.sp[pg, l, 0, :, e] = k4.reshape(-1, hkv, 64), ks.reshape(-1, hkv, 2)
+        self.sd[pg, l, 1, :, e], self.sp[pg, l, 1, :, e] = v4.reshape(-1, hkv, 64), vs.reshape(-1, hkv, 2)
+        self.known[pg, l, e] = True
+        if l == 0:
+            self._written.append((pg, e))
+
+    def _end(self, pages, n):
+        """The key of a sequence of n tokens on `pages`: the (page, entry) of its last token."""
+        return int(pages[(n - 1) // self.P]), (n - 1) % self.P
+
+    def _register(self, pages, n, holders=1):
+        key = self._end(pages, n)
+        e = self.ends.get(key)
+        if e is not None and e[0] == n and e[1] == tuple(pages[:-(-n // self.P)]):
+            e[2] += holders
+        else:
+            self.ends[key] = [n, tuple(int(x) for x in pages[:-(-n // self.P)]), holders]
+
+    def fork(self, parent_pages, n, child_pages):
+        """A fork (KvCacheInt4.fork) of the first n tokens of the sequence on `parent_pages` onto `child_pages`: the child shares
+        the parent's full pages among them and holds a copy of the partly filled one, if any, in a page of its own."""
+        P, full = self.P, n // self.P
+        parent_pages, child_pages = [int(x) for x in parent_pages], [int(x) for x in child_pages]
+        self._ensure(parent_pages + child_pages)
+        if child_pages[:full] != parent_pages[:full] or len(child_pages) != -(-n // P):
+            self._fail("fork", f"the child's pages {child_pages} are not the parent's full pages {parent_pages[:full]} + one copy")
+        t = np.arange(n)
+        pg, e = self._slots(parent_pages, t)
+        if not self.known[pg, :, e].all():
+            self._fail("fork", f"the parent's first {n} tokens are not all a history the reference saw written")
+        if n % P:
+            src, dst = parent_pages[full], child_pages[full]
+            if dst in parent_pages:
+                self._fail("fork", f"the partly filled page {src} is shared with the child (page {dst}), not copied")
+            self.sd[dst], self.sp[dst] = self.sd[src], self.sp[src]
+            self.known[dst] = False
+            self.known[dst, :, :n % P] = self.known[src, :, :n % P]
+        if n:
+            self._register(child_pages, n)
+
+    def keep(self, kept):
+        """After a verify step: running sequence j keeps kept[j] of its S rows (KvCacheInt4.truncate to its length - S + kept[j]);
+        the next step must continue it at that length."""
+        for (pages, n, _, _), c in zip([r for r in self._rows_step if r[3]], kept):
+            if not 1 <= int(c) <= self._S:
+                raise ValueError(f"kept {c} outside [1, {self._S}]")
+            key = self._end(pages, n)
+            e = self.ends.get(key)
+            if e is not None and e[0] == n:
+                del self.ends[key]
+            self._register(pages, n - self._S + int(c))
+
     # ---------------------------------------------------------------------------------------------------------- page tables
     def _admit(self, step):
-        """Check the step's page tables against the reference's sequences: prompts have their length, running sequences grew by one
-        token on the pages they held.  Returns the keys of the prompts and of the running sequences, in batch order."""
-        pkeys, dkeys = [], []
-        if step.prefills:
-            for i, (pages, n) in enumerate(sequences(step.ptab, self.P)):
-                if n != step.prefills[i]:
-                    self._fail("page table", f"prompt {i} holds {n} positions for a prompt of {step.prefills[i]} tokens")
-                if pages[0] in pkeys:
-                    self._fail("page table", f"prompt {i} shares page {pages[0]} with another prompt")
-                pkeys.append(pages[0])
-        if step.decode:
-            for j, (pages, n) in enumerate(sequences(step.dtab, self.P)):
-                key = pages[0]
-                if key not in self.seqs or key in pkeys:
-                    self._fail("page table", f"decode row {j}: page {key} does not start a running sequence")
-                old_pages, old_n = self.seqs[key]
-                if n != old_n + 1 or pages[:len(old_pages)] != old_pages:
-                    self._fail("page table", f"decode row {j}: {n} positions on pages {pages}; the sequence held {old_n} on {old_pages}")
-                dkeys.append(key)
-        for key, (pages, n) in zip(pkeys, sequences(step.ptab, self.P) if step.prefills else []):
-            self.seqs[key] = (pages, n)
-            for l in range(len(self.layers)):
-                self.hist.pop((key, l), None)
-        for key, (pages, n) in zip(dkeys, sequences(step.dtab, self.P) if step.decode else []):
-            self.seqs[key] = (pages, n)
-        return pkeys, dkeys
+        """Check the step's page tables against the sequences the reference knows: every row continues a history that ends
+        where it says, at the length the reference expects (prompts: none, or the earlier chunks / the forked prefix of their
+        sequence; running sequences: what their last step kept), and writes its new positions into pages it alone holds.
+        Returns the rows of the prompts and of the running sequences, in batch order: (pages, length, new tokens, running)."""
+        P, S = self.P, int(step.decode_len)
+        self._written, self._S = [], S
+        prows = [(p, n, k, False) for (p, n), k in zip(sequences(step.ptab, P), step.prefills)] if step.prefills else []
+        if step.prefills and len(prows) != len(step.prefills):
+            self._fail("page table", f"{len(prows)} prompt rows for {len(step.prefills)} prompts")
+        drows = [(p, n, S, True) for p, n in sequences(step.dtab, P)] if step.decode else []
+        if step.decode and len(drows) != step.decode:
+            self._fail("page table", f"{len(drows)} decode rows for {step.decode} running sequences")
+        rows = prows + drows
+        self._ensure([x for r in rows for x in r[0]])
+        held = Counter(x for r in rows for x in set(r[0]))
+        for i, (pages, n, k, running) in enumerate(rows):
+            what = f"decode row {i - len(prows)}" if running else f"prompt {i}"
+            h = n - k
+            if h < 0 or (running and h == 0):
+                self._fail("page table", f"{what} holds {n} positions for {k} new tokens" + (" and no history" if h == 0 else ""))
+            if h:
+                key = self._end(pages, h)
+                e = self.ends.get(key)
+                if e is None or e[0] != h or e[1] != tuple(pages[:-(-h // P)]):
+                    self._fail("page table", f"{what}: {n} positions on pages {pages} continue a history of {h} tokens that no "
+                                             f"sequence the reference knows ends with" +
+                                             (f" (the one ending there holds {e[0]} on {list(e[1])})" if e else ""))
+                e[2] -= 1
+                if not e[2]:
+                    del self.ends[key]
+            for pg in set(pages[h // P:]):
+                refs = None if step.refs is None else step.refs[pg]
+                if held[pg] > 1 or (refs is not None and refs != 1):
+                    self._fail("page table", f"{what} writes into page {pg}, which {refs or held[pg]} sequences hold")
+        self._rows_step = rows
+        return prows, drows
 
-    # ---------------------------------------------------------------------------------------------------------- one step
+    def _check_history(self, before, rows):
+        """Every slot of history a step reads holds, in every layer, the bytes of the reference's shadow."""
+        L = len(self.layers)
+        for i, (pages, n, k, running) in enumerate(rows):
+            if n == k:
+                continue
+            pg, e = self._slots(pages, np.arange(n - k))
+            if not self.known[pg, :, e].all():
+                self._fail("history", f"row {i} reads slots the reference never saw written")
+            if not (same(before[0][pg, :L, :, :, e], self.sd[pg, :, :, :, e]) and
+                    same(before[1][pg, :L, :, :, e], self.sp[pg, :, :, :, e])):
+                self._fail("pool before the step", f"row {i}: its history in the pool is not what the reference saw written")
+
+    def _settle(self):
+        """After the step: every row's sequence ends at its whole length."""
+        for pages, n, k, running in self._rows_step:
+            self._register(pages, n)
+
     def check_step(self, calls, step, pool_before=None, pool_after=None):
         """Walk the trace `calls` of one step; raises WiringError naming the first stage that differs.  pool_before / pool_after:
         (data, param) host copies for the audit.  Returns step.info: the float64 logits and their bound when the model has a head."""
         self._calls, self._pos = calls, 0
-        pf, nd = list(step.prefills), int(step.decode)
+        pf, nd, S = list(step.prefills), int(step.decode), int(step.decode_len)
         doff = sum(pf)
         self._doff = doff
-        m = doff + nd
-        pkeys, dkeys = self._admit(step)
+        m = doff + nd * S
+        prows, drows = self._admit(step)
+        if pool_before is not None:
+            self._check_history(pool_before, prows + drows)
+        ctx = any(n > k for _, n, k, _ in prows)               # a prompt over a cached prefix (a chunk, a continuation)
         cum = np.concatenate([[0], np.cumsum(pf)]).astype(np.int32)
         if step.x is not None:
             residual = step.x
@@ -388,7 +516,7 @@ class ModelRef:
             self._quant(st, x, ref, m, exact=False)
             q, k4, ks, v4, vs = self._qkv(L, p, x, m)
             stack = []
-            # ---- prompts: cache write and causal attention over their own K/V
+            # ---- prompts: cache write at the tail of each sequence, causal attention over its cached prefix and itself
             if pf:
                 st = f"{L} init_kv"
                 c = self._next(st, ["init_kv_i4"])
@@ -398,10 +526,9 @@ class ModelRef:
                 self._eq(st, "seqlen_indptr", np.asarray(c.args["seqlen_indptr"], np.int32), cum)
                 if c.args["layer_idx"] != l:
                     self._fail(st, f"layer_idx {c.args['layer_idx']}, the layer is {l}")
-                for i, key in enumerate(pkeys):
+                for i, (pages, n, k, _) in enumerate(prows):
                     r = slice(cum[i], cum[i + 1])
-                    self.hist[(key, l)] = [k4[r].reshape(pf[i], p.hkv, 64), ks[r].reshape(pf[i], p.hkv, 2),
-                                           v4[r].reshape(pf[i], p.hkv, 64), vs[r].reshape(pf[i], p.hkv, 2)]
+                    self._write(l, pages, np.arange(n - k, n), k4[r], ks[r], v4[r], vs[r], p.hkv)
                 st = f"{L} prefill_attention"
                 c = self._next(st, ["prefill_attention_i4"])
                 for name, t in (("q", q[:doff]), ("k", k4[:doff]), ("k_param", ks[:doff]), ("v", v4[:doff]), ("v_param", vs[:doff])):
@@ -409,17 +536,27 @@ class ModelRef:
                 self._eq(st, "seqlen_indptr", np.asarray(c.args["seqlen_indptr"], np.int32), cum)
                 if list(c.args["seqlens"]) != pf or c.args["rope_theta"] != p.theta:
                     self._fail(st, f"seqlens {c.args['seqlens']} / rope_theta {c.args['rope_theta']}, expected {pf} / {p.theta}")
-                # the reference's K/V of each prompt: its history (= what init_kv was given, checked above)
-                kk = np.concatenate([self.hist[(key, l)][0].reshape(-1, p.hkv * 64) for key in pkeys])
-                kp = np.concatenate([self.hist[(key, l)][1].reshape(-1, p.hkv * 2) for key in pkeys])
-                vv = np.concatenate([self.hist[(key, l)][2].reshape(-1, p.hkv * 64) for key in pkeys])
-                vp = np.concatenate([self.hist[(key, l)][3].reshape(-1, p.hkv * 2) for key in pkeys])
-                ref, bnd = A.prefill_bound(q[:doff], kk, kp, vv, vp, pf, p.hq, p.theta, rows=self.prefill_rows)
-                self._attn_bound(st, c.out, ref, bnd)
+                if ctx:
+                    if c.args.get("kv") is None:
+                        self._fail(st, "prompts over a cached prefix, called without `kv`")
+                    self._table(st, c.args["kv"], step.ptab)
+                    if c.args["layer_idx"] != l:
+                        self._fail(st, f"layer_idx {c.args['layer_idx']}, the layer is {l}")
+                    pt = step.ptab
+                    ref, bnd = prefill_ctx_bound(q[:doff], k4[:doff], ks[:doff], v4[:doff], vs[:doff], pf, p.hq, p.theta, self.sd,
+                                                 self.sp, pt["indptr"], pt["indices"], pt["last"], l, rows=self.prefill_rows)
+                    self._attn_bound(st, c.out, ref, bnd, "prefill over a cached prefix")
+                else:
+                    if c.args.get("kv") is not None:
+                        self._fail(st, "whole prompts, called with `kv`")
+                    ref, bnd = A.prefill_bound(q[:doff], k4[:doff], ks[:doff], v4[:doff], vs[:doff], pf, p.hq, p.theta, rows=self.prefill_rows)
+                    self._attn_bound(st, c.out, ref, bnd, "prefill")
                 stack.append(c.out)
-            # ---- running sequences: one appended position, decode attention over the whole history
-            if nd:
-                stack.append(self._decode(L, l, p, q, k4, ks, v4, vs, doff, nd, dkeys, step.dtab))
+            # ---- running sequences: one appended position and decode attention, or S positions and verify attention
+            if nd and S > 1:
+                stack.append(self._verify(L, l, p, q, k4, ks, v4, vs, doff, drows, step.dtab, S))
+            elif nd:
+                stack.append(self._decode(L, l, p, q, k4, ks, v4, vs, doff, nd, drows, step.dtab))
             attn = np.concatenate(stack) if len(stack) > 1 else stack[0]
             # ---- o_proj
             xo = self._reorder(L, p, attn, m)
@@ -450,7 +587,8 @@ class ModelRef:
         else:
             self._head(step, h)
         if pool_before is not None:
-            self._audit(pool_before, pool_after, pkeys + dkeys)
+            self._audit(pool_before, pool_after)
+        self._settle()
         return step.info
 
     # ---------------------------------------------------------------------------------------------------------- stages
@@ -490,9 +628,9 @@ class ModelRef:
         self._o4(st + " (v)", x, p.qkv.rows(nq + nkv, nq + 2 * nkv), (v4, vs), rows)
         return q, k4, ks, v4, vs
 
-    def _decode(self, L, l, p, q, k4, ks, v4, vs, doff, nd, dkeys, dtab):
-        """append_kv of the rows [doff, doff + nd) and decode attention over each running sequence's history; returns the
-        attention output [nd, heads * 128]."""
+    def _decode(self, L, l, p, q, k4, ks, v4, vs, doff, nd, drows, dtab):
+        """append_kv of the rows [doff, doff + nd) and decode attention over each running sequence's history (the cascade's
+        bound when the table has prefix groups and ops.decode_cascade picks it); returns the attention output [nd, heads * 128]."""
         st = f"{L} append_kv"
         c = self._next(st, ["append_kv_i4"])
         for name, t in (("k", k4), ("v", v4), ("k_param", ks), ("v_param", vs)):
@@ -500,26 +638,64 @@ class ModelRef:
         self._table(st, c.args["kv"], dtab)
         if c.args["layer_idx"] != l:
             self._fail(st, f"layer_idx {c.args['layer_idx']}, the layer is {l}")
-        seqs = []
-        for j, key in enumerate(dkeys):
-            h = self.hist.get((key, l))
-            if h is None or len(h[0]) != self.seqs[key][1] - 1:
-                self._fail(st, f"decode row {j}: the reference holds no history of {self.seqs[key][1] - 1} positions")
-            r = doff + j
-            new = (k4[r].reshape(1, p.hkv, 64), ks[r].reshape(1, p.hkv, 2), v4[r].reshape(1, p.hkv, 64), vs[r].reshape(1, p.hkv, 2))
-            h = self.hist[(key, l)] = [np.concatenate([a, b]) for a, b in zip(h, new)]
-            un = lambda b: A.unpack(b.transpose(1, 0, 2))                               # noqa: E731  [Hkv, n, 128]
-            seqs.append((un(h[0]), h[1].transpose(1, 0, 2), un(h[2]), h[3].transpose(1, 0, 2)))
+        for j, (pages, n, _, _) in enumerate(drows):
+            r = slice(doff + j, doff + j + 1)
+            self._write(l, pages, [n - 1], k4[r], ks[r], v4[r], vs[r], p.hkv)
         st = f"{L} batch_decode"
         c = self._next(st, ["batch_decode_i4"])
         self._eq(st, "q", c.args["q"], q[doff:])
         self._table(st, c.args["kv"], dtab)
         if c.args["layer_idx"] != l or c.args["rope_theta"] != p.theta:
             self._fail(st, f"layer_idx {c.args['layer_idx']} / rope_theta {c.args['rope_theta']}, expected {l} / {p.theta}")
-        data, param, ip, ind, last = A.make_pool(seqs, self.P, p.hkv)                     # private: from the history alone
-        ref, bnd = A.decode_bound(q[doff:].reshape(nd, p.hq, 128), data, param, ip, ind, last, 0, p.hq, p.theta)
-        self._attn_bound(st, c.out, ref, bnd)
+        qd = q[doff:].reshape(nd, p.hq, 128)
+        tab = (dtab["indptr"], dtab["indices"], dtab["last"])
+        if c.args.get("kv_split", 0) == 0 and self._cascade(dtab, nd, p):
+            ref, bnd = cascade_bound(qd, self.sd, self.sp, *tab, l, p.hq, p.theta, dtab["shared"])
+            self._attn_bound(st + " (cascade)", c.out, ref, bnd, "cascade decode")
+        else:
+            ref, bnd = A.decode_bound(qd, self.sd, self.sp, *tab, l, p.hq, p.theta)
+            self._attn_bound(st, c.out, ref, bnd, "decode")
         return c.out.reshape(nd, p.hq * 128)
+
+    def _cascade(self, dtab, nd, p):
+        """Whether batch_decode_i4 runs the shared-prefix cascade on this table (ops.decode_cascade, on sm_count SMs)."""
+        if not dtab.get("groups") or self.sm_count is None:
+            return False
+        from atom_b200 import ops
+        return ops.decode_cascade(dtab["groups"], nd, self.P, p.hkv, p.hq // p.hkv, self.sm_count)
+
+    def _verify(self, L, l, p, q, k4, ks, v4, vs, doff, drows, dtab, S):
+        """A verify step: init_kv of each running sequence's S rows at stride S to its last S positions, and verify attention
+        of those rows over the sequence's history and, causally, each other; returns the attention output [nd * S, heads * 128].
+        The verify kernel does not use prefix groups: its output is held to verify_bound whatever groups the table has."""
+        nd = len(drows)
+        n = nd * S
+        st = f"{L} init_kv (verify)"
+        c = self._next(st, ["init_kv_i4"])
+        for name, t in (("k", k4), ("v", v4), ("k_param", ks), ("v_param", vs)):
+            self._eq(st, name, c.args[name], t[doff:])
+        self._table(st, c.args["kv"], dtab)
+        self._eq(st, "seqlen_indptr", np.asarray(c.args["seqlen_indptr"], np.int32), np.arange(0, n + 1, S, dtype=np.int32))
+        if c.args["layer_idx"] != l:
+            self._fail(st, f"layer_idx {c.args['layer_idx']}, the layer is {l}")
+        for j, (pages, ln, _, _) in enumerate(drows):
+            r = slice(doff + j * S, doff + (j + 1) * S)
+            self._write(l, pages, np.arange(ln - S, ln), k4[r], ks[r], v4[r], vs[r], p.hkv)
+        st = f"{L} batch_verify"
+        c = self._next(st, ["batch_verify_i4"])
+        self._eq(st, "q", c.args["q"], q[doff:])
+        self._table(st, c.args["kv"], dtab)
+        a = c.args
+        if a["tokens_per_seq"] != S or a["layer_idx"] != l or a["rope_theta"] != p.theta:
+            self._fail(st, f"tokens_per_seq {a['tokens_per_seq']} / layer_idx {a['layer_idx']} / rope_theta {a['rope_theta']}, expected "
+                           f"{S} / {l} / {p.theta}")
+        longest = max(ln for _, ln, _, _ in drows)
+        if a["max_len"] is not None and a["max_len"] < longest:
+            self._fail(st, f"max_len {a['max_len']} below the longest sequence's {longest} tokens")
+        ref, bnd = VR.verify_bound(q[doff:].reshape(n, p.hq, 128), self.sd, self.sp, dtab["indptr"], dtab["indices"], dtab["last"], l,
+                                   p.hq, p.theta, S)
+        self._attn_bound(st, c.out, ref, bnd, "verify")
+        return c.out.reshape(n, p.hq * 128)
 
     def _reorder(self, L, p, attn, m):
         st = f"{L} o_proj reorder"
@@ -689,38 +865,80 @@ class ModelRef:
             self._fail("lm_head", "logits outside gamma_K sum|x w| + half an ulp of the float64 product")
         step.info.update(logits64=S, bound=b)
         if step.rows is not None:
-            want = (cum_last(step.prefills) + list(range(sum(step.prefills), sum(step.prefills) + step.decode)))
-            if list(step.rows) != want:
-                self._fail("last_token_rows", f"logits read at rows {list(step.rows)}, the last token of each prompt and every decode row "
-                                              f"are {want}")
+            dec = list(range(sum(step.prefills), sum(step.prefills) + step.decode * step.decode_len))
+            rows, last = [int(r) for r in step.rows], cum_last(step.prefills)
+            first = rows[:len(rows) - len(dec)]
+            if rows[len(first):] != dec or any(r not in last for r in first) or first != sorted(set(first)):
+                self._fail("last_token_rows", f"logits read at rows {rows}: the last token of prompts it completes (of {last}) and every "
+                                              f"decode row ({dec}) are expected")
 
-    def _audit(self, before, after, keys):
+    def _audit(self, before, after):
+        """The slots the step wrote hold the shadow's bytes in every layer; every other byte is as it was before the step."""
         data, param = before[0].copy(), before[1].copy()
-        P = self.P
-        for key in keys:
-            pages, n = self.seqs[key]
-            t = np.arange(n)
-            pg, e = np.asarray(pages)[t // P], t % P
-            for l in range(len(self.layers)):
-                k4, kp, v4, vp = self.hist[(key, l)]
-                data[pg, l, 0, :, e], param[pg, l, 0, :, e] = k4, kp
-                data[pg, l, 1, :, e], param[pg, l, 1, :, e] = v4, vp
+        L = len(self.layers)
+        for pg, e in self._written:
+            data[pg, :L, :, :, e], param[pg, :L, :, :, e] = self.sd[pg, :, :, :, e], self.sp[pg, :, :, :, e]
         bad_d = np.argwhere(data != after[0])
         bad_p = np.argwhere(param.view(np.uint16) != after[1].view(np.uint16))
         if len(bad_d) or len(bad_p):
             where = (bad_d if len(bad_d) else bad_p)[0].tolist()
-            self._fail(f"layer {where[1]} pool audit", f"{len(bad_d)} data bytes and {len(bad_p)} parameters differ from the reference's history "
-                                     f"(owned slots) or from the pool before the step (all others); first at "
+            self._fail(f"layer {where[1]} pool audit", f"{len(bad_d)} data bytes and {len(bad_p)} parameters differ from the reference's shadow "
+                                     f"(slots the step wrote) or from the pool before the step (all others); first at "
                                      f"[page, layer, k|v, head, entry] = {where[:5]}")
 
-    def check_tokens(self, step, tokens):
-        """Greedy tokens of a step (one per row of step.rows): the argmax of the float64 logits wherever the top-2 gap exceeds
-        twice the logits' bound."""
+    def _argmax(self, step, st, r, token):
+        """token is the float64 argmax of logits row r wherever the top-2 gap exceeds twice the logits' bound."""
         S, b = step.info["logits64"], step.info["bound"]
-        for i, r in enumerate(cum_last(step.prefills) + list(range(sum(step.prefills), sum(step.prefills) + step.decode))):
-            top = np.argsort(S[r])[::-1][:2]
-            if S[r, top[0]] - S[r, top[1]] > 2 * (b[r, top[0]] + b[r, top[1]]) and int(tokens[i]) != int(top[0]):
-                self._fail("greedy token", f"row {r}: token {int(tokens[i])}, the float64 argmax is {int(top[0])}")
+        top = np.argsort(S[r])[::-1][:2]
+        if S[r, top[0]] - S[r, top[1]] > 2 * (b[r, top[0]] + b[r, top[1]]) and int(token) != int(top[0]):
+            self._fail(st, f"row {r}: token {int(token)}, the float64 argmax is {int(top[0])}")
+
+    def check_tokens(self, step, tokens):
+        """Greedy tokens of a step (one per row of step.rows, or of the last row of each prompt and every decode row): the argmax
+        of the float64 logits wherever the top-2 gap exceeds twice the logits' bound."""
+        rows = step.rows if step.rows is not None else \
+            cum_last(step.prefills) + list(range(sum(step.prefills), sum(step.prefills) + step.decode * step.decode_len))
+        for r, t in zip(rows, tokens):
+            self._argmax(step, "greedy token", int(r), t)
+
+    def check_spec(self, step, drafts, emitted, room=None, stop_ids=()):
+        """Greedy speculative tokens of a step (its rows: step.rows, as the scheduler reads them).  emitted: the tokens each
+        sequence emitted -- one for each prompt the step completes, then every running sequence's; drafts: each running
+        sequence's drafts (the inputs of its rows 1, 2, ..).  Row by row, emitted token j is the float64 argmax of row j, and draft
+        j + 1 is accepted exactly when it equals that token: a sequence emits its accepted prefix + 1 tokens.  room: tokens each
+        running sequence may still emit (its output length), stop_ids: ids that end a request.  The tokens a sequence keeps --
+        emitted, cut at the room and at the first stop id -- set the length the next step must continue it at (keep).  Returns
+        the kept counts."""
+        st = "speculative commit"
+        S, nd, doff = int(step.decode_len), int(step.decode), sum(step.prefills)
+        rows = [int(r) for r in step.rows]
+        first = len(rows) - nd * S
+        if len(emitted) != first + nd or len(drafts) != nd:
+            self._fail(st, f"{len(emitted)} sequences emitted and {len(drafts)} drafted, the step has {first} prompts it completes and "
+                           f"{nd} running sequences")
+        for i in range(first):
+            if len(emitted[i]) != 1:
+                self._fail(st, f"prompt {i}: {len(emitted[i])} tokens emitted for its first")
+            self._argmax(step, st, rows[i], emitted[i][0])
+        kept = []
+        for i in range(nd):
+            em, dr = [int(t) for t in emitted[first + i]], [int(t) for t in drafts[i]]
+            j = 0
+            while True:
+                if j >= len(em):
+                    self._fail(st, f"sequence {i}: {len(em)} tokens emitted, its accepted drafts call for {j + 1}")
+                self._argmax(step, st, doff + i * S + j, em[j])
+                if j + 1 < S and j < len(dr) and dr[j] == em[j]:
+                    j += 1
+                    continue
+                break
+            if len(em) != j + 1:
+                self._fail(st, f"sequence {i}: {len(em)} tokens emitted ({em}); its drafts {dr} against the emitted tokens accept {j}")
+            c = j + 1 if room is None else min(j + 1, int(room[i]))
+            c = next((t + 1 for t in range(c) if em[t] in stop_ids), c)
+            kept.append(c)
+        self.keep(kept)
+        return kept
 
 
 def cum_last(prefills):
@@ -739,7 +957,8 @@ def run_step(rec, pool, fn, inp, blen, prefill_kv, decode_kv, ids=True):
     """fn(inp, blen, prefill_kv, decode_kv) with the kernels recorded.  inp: token ids (ids=True) or the FP16 hidden states.
     Returns (out, Step, calls, pool before, pool after) for ModelRef.check_step (set Step.rows first where tokens are read)."""
     step = Step(list(blen.prefills), blen.decode, host(prefill_kv) if prefill_kv is not None else None,
-                host(decode_kv) if decode_kv is not None else None)
+                host(decode_kv) if decode_kv is not None else None, decode_len=getattr(blen, "decode_len", 1),
+                refs=list(pool._refs) if hasattr(pool, "_refs") else None)
     if ids:
         step.ids = host(inp)
     else:

@@ -1,6 +1,8 @@
 """CPU self-test of tests/layer_ref64.py.  The real LlamaForCausalLM code runs on the CPU with every kernel replaced by its oracle
-(oracle/atom_oracle.c, attn_ref64 for attention), which gives a recorded trace of a two-layer prefill step and a mixed prefill +
-decode step.  The reference must (a) accept that trace and (b) reject each seeded wiring fault, naming the stage."""
+(oracle/atom_oracle.c; attn_ref64, attn_ctx_ref64 and attn_verify_ref64 for attention), which gives a recorded trace of a
+two-layer prefill step and a mixed prefill + decode step, and of a serving sequence with chunked prompts, forks, continuations and
+verify steps truncated to several kept counts.  The reference must (a) accept those traces and (b) reject each seeded wiring
+fault, naming the stage."""
 import types
 
 import numpy as np
@@ -9,7 +11,9 @@ import torch
 
 from oracle import oracle as O
 from tests import attn_ref64 as A
+from tests import attn_verify_ref64 as VR
 from tests import gemm_ref64 as G
+from tests.attn_ctx_ref64 import prefill_ctx_ref
 from tests import layer_ref64 as R
 
 P = 8
@@ -90,13 +94,23 @@ def append_kv_i4(kv, k, v, k_param, v_param, layer_idx):
     O.append_kv_i4(_np(kv.data), _np(kv.param), *_table(kv), _np(k), _np(v), _np(k_param), _np(v_param), layer_idx)
 
 
-def prefill_attention_i4(q, k, k_param, v, v_param, seqlen_indptr, seqlens=None, rope_theta=10000.0):
-    o = A.prefill_ref(_np(q), _np(k), _np(k_param), _np(v), _np(v_param), seqlens, q.shape[1] // 128, rope_theta)
+def prefill_attention_i4(q, k, k_param, v, v_param, seqlen_indptr, seqlens=None, rope_theta=10000.0, *, kv=None, layer_idx=None):
+    if kv is None:
+        o = A.prefill_ref(_np(q), _np(k), _np(k_param), _np(v), _np(v_param), seqlens, q.shape[1] // 128, rope_theta)
+    else:
+        o = prefill_ctx_ref(_np(q), _np(k), _np(k_param), _np(v), _np(v_param), seqlens, q.shape[1] // 128, rope_theta, _np(kv.data),
+                            _np(kv.param), *_table(kv), layer_idx)
     return torch.from_numpy(o.astype(np.float16))
 
 
 def batch_decode_i4(q, kv, layer_idx, rope_theta=10000.0):
+    """decode_ref on the pool: over forked rows too (shared pages hold the same bytes for every holder)."""
     o = A.decode_ref(_np(q), _np(kv.data), _np(kv.param), *_table(kv), layer_idx, q.shape[1], rope_theta)
+    return torch.from_numpy(o.astype(np.float16))
+
+
+def batch_verify_i4(q, kv, layer_idx, tokens_per_seq, rope_theta=10000.0, max_len=None, nchunks=0, **defect):
+    o = VR.verify_variant(_np(q), _np(kv.data), _np(kv.param), *_table(kv), layer_idx, q.shape[1], rope_theta, tokens_per_seq, **defect)
     return torch.from_numpy(o.astype(np.float16))
 
 
@@ -115,8 +129,35 @@ def _init_kv_into_layer0_in_kernel(kv, k, v, k_param, v_param, seqlen_indptr, la
     init_kv_i4(kv, k, v, k_param, v_param, seqlen_indptr, 0)
 
 
+def _ctx_positions_from_zero_in_kernel(q, k, k_param, v, v_param, seqlen_indptr, seqlens=None, rope_theta=10000.0, *, kv=None,
+                                       layer_idx=None):
+    """The chunk's queries rotated at positions 0 .. n - 1 instead of ctx .. ctx + n - 1 (its keys where they are): q turned
+    back by ctx positions in float64 before the exact reference."""
+    if kv is None:
+        return prefill_attention_i4(q, k, k_param, v, v_param, seqlen_indptr, seqlens, rope_theta)
+    qq = _np(q).astype(np.float64).reshape(len(_np(q)), -1, 2, 64)
+    f = A.freqs(rope_theta)
+    off = 0
+    for n, total in zip(seqlens, kv.seqlens):
+        z = (qq[off:off + n, :, 0] + 1j * qq[off:off + n, :, 1]) * np.exp(-1j * (total - n) * f)
+        qq[off:off + n, :, 0], qq[off:off + n, :, 1] = z.real, z.imag
+        off += n
+    o = prefill_ctx_ref(qq.reshape(len(qq), -1), _np(k), _np(k_param), _np(v), _np(v_param), seqlens, q.shape[1] // 128, rope_theta,
+                        _np(kv.data), _np(kv.param), *_table(kv), layer_idx)
+    return torch.from_numpy(o.astype(np.float16))
+
+
+def _verify_defect(**defect):
+    return lambda q, kv, layer_idx, tokens_per_seq, rope_theta=10000.0, max_len=None, nchunks=0: \
+        batch_verify_i4(q, kv, layer_idx, tokens_per_seq, rope_theta, max_len, nchunks, **defect)
+
+
 KERNEL_FAULTS = {"append_late_in_kernel": ("append_kv_i4", _append_late_in_kernel),
-                 "init_kv_into_layer0_in_kernel": ("init_kv_i4", _init_kv_into_layer0_in_kernel)}
+                 "init_kv_into_layer0_in_kernel": ("init_kv_i4", _init_kv_into_layer0_in_kernel),
+                 "ctx_positions_from_zero_in_kernel": ("prefill_attention_i4", _ctx_positions_from_zero_in_kernel),
+                 "verify_limit_off_by_one_in_kernel": ("batch_verify_i4", _verify_defect(limit_shift=1)),
+                 "verify_rotated_at_last_in_kernel": ("batch_verify_i4", _verify_defect(rotate_at_last=True)),
+                 "verify_kv_head_mod_in_kernel": ("batch_verify_i4", _verify_defect(head_mod=True))}
 
 
 # ---- the seeded faults: each wraps an operator (a wiring mistake between the layer and the kernel) or a model method
@@ -153,12 +194,12 @@ def _fault(monkeypatch, name, state):
         raise ValueError(name)
 
 
-def _model():
+def _model(hidden=256, heads=2, kv_heads=1):
     from atom_b200.llama import LinearInt4, LlamaConfig, LlamaForCausalLM
     torch.manual_seed(3)
     torch.set_default_dtype(torch.float16)
     try:
-        model = LlamaForCausalLM(LlamaConfig(hidden_size=256, intermediate_size=384, num_attention_heads=2, num_key_value_heads=1,
+        model = LlamaForCausalLM(LlamaConfig(hidden_size=hidden, intermediate_size=384, num_attention_heads=heads, num_key_value_heads=kv_heads,
                                              num_hidden_layers=2, vocab_size=64, rope_theta=5e5)).eval()
     finally:
         torch.set_default_dtype(torch.float32)
@@ -215,7 +256,7 @@ def _run(monkeypatch, fault=None):
 
 def test_reference_accepts_the_oracle_trace(monkeypatch):
     ref = _run(monkeypatch)
-    assert len(ref.seqs) == 3 and all(len(h[0]) == ref.seqs[key][1] for (key, _), h in ref.hist.items())
+    assert sorted(e[0] for e in ref.ends.values()) == [6, 7, 12]
 
 
 @pytest.mark.parametrize("fault,stage", [
@@ -238,3 +279,227 @@ def test_reference_rejects_a_seeded_wiring_fault(monkeypatch, fault, stage):
 def test_reference_rejects_a_kernel_that_stores_to_the_wrong_slot(monkeypatch, fault, stage):
     with pytest.raises(R.WiringError, match=stage):
         _run(monkeypatch, fault)
+
+
+# ---- serving sequences: chunked prompts, forks, continuations and verify steps
+class Driver:
+    """Steps of a model (token ids in, logits out) or of a layer stack (ids=False: hidden states in) as the serving scheduler
+    forms them, every one checked by `ref`.  Sequences are named; a prompt chunk of a sequence is the tail of its cached tokens;
+    `fork` starts a sequence on another's first n tokens (the reference is told through a wrapper of KvCacheInt4.fork).  A step's
+    running sequences carry S rows each -- their last token and drafts -- and, for S > 1, keep either the counts the test gives
+    (ModelRef.keep) or what greedy acceptance of the drafts emits (ModelRef.check_spec, models only)."""
+
+    def __init__(self, monkeypatch, fn, pool, ref, impl=None, fault=None, ids=True, vocab=64, setup=None):
+        from atom_b200 import textgen
+        from atom_b200.kvcache import KvCacheInt4
+        self.rec = R.Recorder(impl).install(monkeypatch)
+        if setup is not None:               # (seeded faults: around the recorded operators, under the fork hook)
+            setup()
+        self.fn, self.pool, self.ref, self.fault, self.ids, self.vocab = fn, pool, ref, fault, ids, vocab
+        real = KvCacheInt4.fork
+
+        def fork(kv, n=None):
+            child = real(kv, n)
+            ref.fork(list(kv.indicies), child.seqlen, list(child.indicies))
+            return child
+        monkeypatch.setattr(KvCacheInt4, "fork", fork)
+        self.rows_of = textgen.TextGenScheduler.last_token_rows
+        self.kv, self.total, self.done, self.last = {}, {}, {}, {}
+        self.rng = np.random.default_rng(1)
+        self.kept = []
+
+    def fork(self, name, parent, n=None, total=0):
+        self.kv[name] = self.kv[parent].fork(n)
+        self.total[name], self.done[name] = total, 0
+
+    def step(self, chunks=(), running=(), S=1, kept=None):
+        """chunks: [(name, tokens, prompt length)] (a new name starts a sequence; prompt length None = the root of forks, which
+        draws no token); running: names of running sequences."""
+        from atom_b200.cat_tensor import BatchLenInfo
+        from atom_b200.kvcache import BatchedKvCacheInt4, KvCacheInt4
+        dev = self.pool.device
+        new = []
+        for name, n, total in chunks:
+            if name not in self.kv:
+                self.kv[name], self.total[name], self.done[name] = KvCacheInt4(self.pool, 0), total, 0
+            elif total is not None:
+                self.total[name] = total
+            self.kv[name].acquire(n)
+            new.append((types.SimpleNamespace(prompt=[0] * (self.total[name] or 0), req_idx=-1 if self.total[name] is None else 0),
+                        self.done[name], n))
+            self.done[name] += n
+        drafts = {r: self.rng.integers(0, self.vocab, S - 1).tolist() for r in running}
+        for r in running:
+            self.kv[r].acquire(S - 1)
+        m = sum(n for _, n, _ in chunks) + S * len(running)
+        if self.ids:
+            inp = torch.tensor(sum((self.rng.integers(0, self.vocab, n).tolist() for _, n, _ in chunks), []) +
+                               sum(([self.last[r]] + drafts[r] for r in running), []), device=dev)
+        else:
+            inp = torch.from_numpy((self.rng.standard_normal((m, self.ref.layers[0].hidden)) * 0.5).astype(np.float16)).to(dev)
+        blen = BatchLenInfo([n for _, n, _ in chunks], len(running), dev, decode_len=S)
+        with torch.inference_mode():
+            out, step, calls, before, after = R.run_step(
+                self.rec, self.pool, self.fn, inp, blen, BatchedKvCacheInt4([self.kv[c] for c, _, _ in chunks]) if chunks else None,
+                BatchedKvCacheInt4([self.kv[r] for r in running]) if running else None, ids=self.ids)
+        firsts = [c for (c, _, _), (p, s, k) in zip(chunks, new) if self.total[c] is not None and s + k == self.total[c]]
+        if self.ref.lm_head is not None:
+            step.rows = self.rows_of(types.SimpleNamespace(_blen=blen, _new=new))
+        self.ref.check_step(calls, step, before, after)
+        emitted = self._emit(step, out, blen, firsts, running, drafts, S, kept)
+        self.kept.append([len(e) for e in emitted[len(firsts):]])
+        for name, em in zip(firsts + list(running), emitted):
+            if name in running:
+                self.kv[name].truncate(self.kv[name].seqlen - S + len(em))
+            self.last[name] = em[-1]
+            self.kv[name].acquire_one()
+        return step
+
+    def _emit(self, step, out, blen, firsts, running, drafts, S, kept):
+        """The tokens each sequence emits, checked: one per completed prompt, then the running sequences' (kept[i] of them, or
+        greedy acceptance of the drafts)."""
+        if self.ref.lm_head is None:
+            assert S == 1 or kept is not None
+            if S > 1:
+                self.ref.keep(kept)
+            return [[0]] * len(firsts) + [[0] * (1 if kept is None else kept[i]) for i in range(len(running))]
+        logits = out[0].float()
+        arg = lambda r: int(torch.argmax(logits[r]))                                                   # noqa: E731
+        emitted = [[arg(r)] for r in step.rows[:len(firsts)]]
+        for i, r in enumerate(running):
+            base = blen.doff + i * S
+            if kept is not None:
+                emitted.append([arg(base + j) for j in range(kept[i])])
+                continue
+            em, j = [], 0                           # greedy acceptance, row by row
+            while True:
+                t = arg(base + j)
+                if self.fault == "commit_accepts_non_argmax" and j < S - 1 and drafts[r][j] != t:
+                    t = drafts[r][j]
+                em.append(t)
+                if j + 1 < S and drafts[r][j] == t:
+                    j += 1
+                    continue
+                break
+            emitted.append(em)
+        if S > 1 and kept is not None:
+            self.ref.check_tokens(step, [e[0] for e in emitted[:len(firsts)]])
+            self.ref.keep(kept)
+        else:
+            self.ref.check_spec(step, [drafts[r] for r in running], emitted)
+        return emitted
+
+
+def _serving_fault(monkeypatch, name, P):
+    from atom_b200 import ops
+    from atom_b200 import textgen
+    from atom_b200.cat_tensor import BatchLenInfo
+    from atom_b200.kvcache import KvCacheInt4
+    if name == "continuation_without_kv":             # the layer drops the cache from a prompt over a cached prefix
+        f = ops.prefill_attention_i4
+        monkeypatch.setattr(ops, "prefill_attention_i4", lambda *a, kv=None, layer_idx=None, **k: f(*a, **k))
+    elif name == "verify_kv_at_stride_1":             # a verify step's K/V rows written one per sequence
+        monkeypatch.setattr(BatchLenInfo, "decode_indptr", property(
+            lambda self: None if self.decode_len == 1 else torch.arange(0, self.decode + 1, dtype=torch.int32)))
+    elif name in ("truncate_keeps_one_more", "truncate_keeps_one_less"):
+        f, d = KvCacheInt4.truncate, 1 if name.endswith("more") else -1
+        monkeypatch.setattr(KvCacheInt4, "truncate", lambda self, n: f(self, min(n + d, self.seqlen)))
+    elif name == "fork_shares_partial_page":          # the partly filled page shared instead of copied
+        def fork(self, n=None):
+            n = self.seqlen if n is None else n
+            child = KvCacheInt4(self.pool, 0)
+            for page in self.indicies[:-(-n // P)]:
+                self.pool.share_block(page)
+                child._pages.append(page)
+            child._seqlen = n
+            return child
+        monkeypatch.setattr(KvCacheInt4, "fork", fork)
+    elif name == "verify_rows_one_per_sequence":     # the logits of a verify step read at each sequence's first row only
+        f = textgen.TextGenScheduler.last_token_rows
+
+        def rows(self):
+            b = self._blen
+            r = f(self)
+            return r[:len(r) - b.decode * b.decode_len] + [b.doff + i * b.decode_len for i in range(b.decode)]
+        monkeypatch.setattr(textgen.TextGenScheduler, "last_token_rows", rows)
+    elif name != "commit_accepts_non_argmax":        # (the driver's own acceptance)
+        raise ValueError(name)
+
+
+def _serve(monkeypatch, fault=None):
+    """A root R of 13 tokens and the first chunk of X (30 tokens); X's second chunk (from position 11, off a 16-row boundary) with
+    forks of R at 8 (aligned, pages shared) and 13 (its partly filled page copied) and their continuation prompts; a verify step
+    (S = 4) with a new prompt Y, kept 4 / 1 (back across a page boundary) / 2 (inside a page); a verify step with greedy
+    acceptance; a decode step; a verify step (S = 2) and a last decode step."""
+    from atom_b200.kvcache import KvPoolInt4
+    monkeypatch.setattr(torch.cuda.nvtx, "range_push", lambda *a: None)
+    monkeypatch.setattr(torch.cuda.nvtx, "range_pop", lambda *a: None)
+    model = _model(hidden=512, heads=4, kv_heads=2)
+    impl = dict(ORACLE_OPS)
+    if fault in KERNEL_FAULTS:
+        impl.update([KERNEL_FAULTS[fault]])
+    pool = KvPoolInt4(2, 2, 128, 40, P, torch.device("cpu"))
+    pool.buf.random_(0, 256)
+    pool.param.view(torch.int16).random_(-32768, 32767)
+    d = Driver(monkeypatch, model, pool, R.model_ref(model, P), impl, fault,
+               setup=lambda: fault and fault not in KERNEL_FAULTS and _serving_fault(monkeypatch, fault, P))
+    d.step([("R", 13, None), ("X", 11, 30)])
+    d.fork("F1", "R", 8, total=5)
+    d.fork("F2", "R", total=6)
+    d.step([("X", 19, None), ("F1", 5, None), ("F2", 6, None)])
+    d.lens = [[d.kv[n].seqlen for n in ("X", "F1", "F2")]]
+    d.step([("Y", 7, 7)], ["X", "F1", "F2"], S=4, kept=[4, 1, 2])
+    d.lens.append([d.kv[n].seqlen for n in ("X", "F1", "F2", "Y")])
+    d.step([], ["X", "F1", "F2", "Y"], S=3)
+    d.step([("Z", 9, 9)], ["X", "F1", "F2", "Y"])
+    d.step([], ["X", "F1", "F2", "Y", "Z"], S=2, kept=[2, 1, 2, 1, 2])
+    d.step([], ["X", "F1", "F2", "Y", "Z"])
+    return d
+
+
+def test_reference_accepts_chunks_forks_and_verify_steps(monkeypatch):
+    d = _serve(monkeypatch)
+    ref = d.ref
+    assert d.lens == [[31, 14, 20], [35, 15, 22, 8]]           # (+ the next token's slot)
+    assert dict(ref.calls) == {"prefill": 3 * 2, "prefill over a cached prefix": 2, "verify": 3 * 2, "decode": 2 * 2}
+    assert all(ref.ends[ref._end(kv.indicies, kv.seqlen - 1)][0] == kv.seqlen - 1 for n, kv in d.kv.items() if n != "R")
+
+
+@pytest.mark.parametrize("fault,stage", [
+    ("continuation_without_kv", r"layer 0 prefill_attention: prompts over a cached prefix, called without `kv`"),
+    ("ctx_positions_from_zero_in_kernel", r"layer 0 prefill_attention: attention output outside the float64 bound"),
+    ("verify_limit_off_by_one_in_kernel", r"layer 0 batch_verify: attention output outside the float64 bound"),
+    ("verify_rotated_at_last_in_kernel", r"layer 0 batch_verify: attention output outside the float64 bound"),
+    ("verify_kv_head_mod_in_kernel", r"layer 0 batch_verify: attention output outside the float64 bound"),
+    ("verify_kv_at_stride_1", r"layer 0 init_kv \(verify\): `seqlen_indptr`"),
+    ("truncate_keeps_one_more", r"page table: decode row 1: 18 positions .* continue a history of 15 tokens"),
+    ("truncate_keeps_one_less", r"page table: decode row 0: 36 positions .* continue a history of 33 tokens"),
+    ("fork_shares_partial_page", r"fork: the partly filled page \d+ is shared"),
+    ("commit_accepts_non_argmax", r"speculative commit: row \d+: token \d+, the float64 argmax is"),
+    ("verify_rows_one_per_sequence", r"last_token_rows"),
+])
+def test_reference_rejects_a_seeded_serving_fault(monkeypatch, fault, stage):
+    with pytest.raises(R.WiringError, match=stage):
+        _serve(monkeypatch, fault)
+
+
+def test_check_spec_follows_the_greedy_acceptance_rule():
+    """check_spec on synthetic float64 logits: two running sequences of S = 4 rows whose argmaxes are known; drafts accepted while
+    they equal the argmax, the emitted count, the cut at the output length and at a stop id, and the lengths it keeps."""
+    ref = R.ModelRef([types.SimpleNamespace(hkv=1)], 8)
+    V, S = 16, 4
+    want = [3, 5, 7, 9, 2, 4, 6, 8]                              # the argmax of rows 0 .. 7
+    logits = np.zeros((8, V))
+    logits[np.arange(8), want] = 10.0
+    step = R.Step([], 2, decode_len=S, rows=list(range(8)), info={"logits64": logits, "bound": np.full((8, V), 1e-3)})
+    ref._rows_step, ref._S = [([0, 1], 12, S, True), ([2], 6, S, True)], S
+    kept = ref.check_spec(step, [[3, 5, 1], [4]], [[3, 5, 7], [2]])
+    assert kept == [3, 1] and ref.ends[(1, 2)][0] == 11 and ref.ends[(2, 2)][0] == 3
+    ref._rows_step = [([0, 1], 12, S, True), ([2], 6, S, True)]
+    assert ref.check_spec(step, [[3, 5, 7], [2, 4]], [[3, 5, 7, 9], [2, 4, 6]], room=[2, 5], stop_ids={4}) == [2, 2]
+    for drafts, emitted, msg in (([[3, 5, 1], [4]], [[3, 5], [2]], r"sequence 0: 2 tokens emitted, its accepted drafts call for 3"),
+                                 ([[3, 5, 1], [4]], [[3, 5, 7, 9], [2]], r"sequence 0: 4 tokens emitted"),
+                                 ([[3, 1, 1], [4]], [[3, 1, 1, 9], [2]], r"row 1: token 1, the float64 argmax is 5")):
+        ref._rows_step = [([0, 1], 12, S, True), ([2], 6, S, True)]
+        with pytest.raises(R.WiringError, match=msg):
+            ref.check_spec(step, drafts, emitted)

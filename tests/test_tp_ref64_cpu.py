@@ -174,7 +174,7 @@ def test_reference_accepts_the_oracle_trace(monkeypatch, world, heads, kv_heads)
     assert n.count("dense_layer_gemm_i4_qkv") == 2 and names[1].count("dense_layer_gemm_i4_o4") == 4
     assert h.ranks[0][0].inter_sizes == ([768, 640] if world == 2 else [384, 384, 384, 256])
     rk = h.ref.ranks[world - 1]
-    assert all(len(hist[0]) == rk.seqs[key][1] for (key, _), hist in rk.hist.items())
+    assert all(rk.ends[rk._end(c.indicies, c.seqlen)][0] == c.seqlen for c in h.seqs[world - 1][:70])
 
 
 @pytest.mark.parametrize("fault,world,batch,stage", [

@@ -385,93 +385,36 @@ def test_decode_graph_runner_replays_the_cascade_as_members_join_and_leave(monke
     assert crossed
 
 
-# ------------------------------------------------------------------------------------------------ 7. a decoder-layer step
-class ForkedRef:
-    """tests/layer_ref64.ModelRef for one decode step over rows forked from common pages.  Every stage is checked as layer_ref64
-    checks it; the rows' histories are the pool's own bytes (shared pages included), so the attention call is held to
-    attn_cascade_ref64.cascade_bound over the pool the step left, the appended slots must hold the step's K/V, and no other byte
-    of the pool may change."""
-
-    @staticmethod
-    def make(layers, P, shared):
-        from tests import layer_ref64 as LR
-
-        class _Ref(LR.ModelRef):
-            def _admit(self, step):
-                return [], list(range(step.decode))
-
-            def _decode(self, L, l, p, q, k4, ks, v4, vs, doff, nd, dkeys, dtab):
-                st = f"{L} append_kv"
-                c = self._next(st, ["append_kv_i4"])
-                for name, t in (("k", k4), ("v", v4), ("k_param", ks), ("v_param", vs)):
-                    self._eq(st, name, c.args[name], t[doff:])
-                self._table(st, c.args["kv"], dtab)
-                data, param = self.after
-                for j, (pages, n) in enumerate(LR.sequences(dtab, self.P)):
-                    pg, e, r = pages[(n - 1) // self.P], (n - 1) % self.P, doff + j
-                    for which, (b, s) in enumerate(((k4, ks), (v4, vs))):
-                        if not (LR.same(data[pg, l, which, :, e], b[r].reshape(p.hkv, 64))
-                                and LR.same(param[pg, l, which, :, e], s[r].reshape(p.hkv, 2))):
-                            self._fail(st, f"decode row {j}: the appended slot does not hold the step's {'kv'[which]}")
-                st = f"{L} batch_decode"
-                c = self._next(st, ["batch_decode_i4"])
-                self._eq(st, "q", c.args["q"], q[doff:])
-                self._table(st, c.args["kv"], dtab)
-                if c.args["layer_idx"] != l or c.args["rope_theta"] != p.theta:
-                    self._fail(st, f"layer_idx {c.args['layer_idx']} / rope_theta {c.args['rope_theta']}")
-                ref, bnd = cascade_bound(q[doff:].reshape(nd, p.hq, 128), data, param, dtab["indptr"], dtab["indices"], dtab["last"],
-                                         l, p.hq, p.theta, self.shared)
-                self._attn_bound(st, c.out, ref, bnd)
-                return c.out.reshape(nd, p.hq * 128)
-
-            def _audit(self, before, after, keys):
-                want_d, want_p = before[0].copy(), before[1].copy()
-                for pages, n in LR.sequences(self.dtab, self.P):
-                    pg, e = pages[(n - 1) // self.P], (n - 1) % self.P
-                    want_d[pg, :, :, :, e], want_p[pg, :, :, :, e] = after[0][pg, :, :, :, e], after[1][pg, :, :, :, e]
-                if not (np.array_equal(want_d, after[0]) and np.array_equal(want_p.view(np.uint16), after[1].view(np.uint16))):
-                    self._fail("pool audit", "the step changed pool bytes outside the appended slots")
-
-        ref = _Ref(layers, P)
-        ref.shared = shared
-        return ref
-
-
-@pytest.mark.timeout(600)
+# ------------------------------------------------------------------------------------------------ 7. decoder-layer steps
+@pytest.mark.timeout(900)
 def test_decoder_layer_decode_step_on_forked_rows_runs_the_cascade(monkeypatch):
-    """A LlamaDecoderLayer decode step (8 query heads, 2 KV heads) over 8 rows forked from a 3072-token root and 2 lone rows:
-    ops.decode_cascade picks the cascade, which runs inside LlamaAttention; layer_ref64 checks every stage of the step and the
-    attention call is held to cascade_bound."""
+    """LlamaDecoderLayer steps (8 query heads, 2 KV heads, P = 32), each checked stage by stage by tests/layer_ref64.ModelRef with
+    pool audits: a 3072-token root prefilled, 8 forks of it with continuation prompts beside 2 lone prompts, then two decode steps
+    in which ops.decode_cascade picks the cascade, which runs inside LlamaAttention and is held to cascade_bound over the
+    reference's shadow of the pool."""
     from atom_b200 import ops
-    from atom_b200.cat_tensor import BatchLenInfo
-    from atom_b200.kvcache import BatchedKvCacheInt4, KvCacheInt4, KvPoolInt4
+    from atom_b200.kvcache import KvPoolInt4
     from tests import layer_ref64 as LR
+    from tests.test_layer_ref64_cpu import Driver
     from tests.test_z_layer_ref64_gpu import _layer
     P, theta = 32, 5e5
     layer = _layer(1024, 1024, 8, 2, theta=theta)
     pool = KvPoolInt4(1, 2, 128, 140, P, torch.device(DEV))
     pool.buf.random_(0, 256)
-    pool.param[..., 0].uniform_(0.01, 0.05)
-    pool.param[..., 1].uniform_(0.0, 0.4)
-    root = KvCacheInt4(pool, 3072)
-    rows = [root.fork() for _ in range(8)]
-    for i, r in enumerate(rows):
-        r.acquire(1 + 9 * i)
-    rows.insert(3, KvCacheInt4(pool, 45))
-    rows.append(KvCacheInt4(pool, 300))
-    for r in rows:
-        r.acquire_one()                                            # the step's token
-    kv = BatchedKvCacheInt4(rows)
+    pool.param.view(torch.int16).random_(-32768, 32767)
     sms = torch.cuda.get_device_properties(DEV).multi_processor_count
-    assert ops.decode_cascade(kv.groups, len(rows), P, 2, 4, sms)
     calls = []
     real = ops._batch_decode_shared
     monkeypatch.setattr(ops, "_batch_decode_shared", lambda *a, **k: calls.append(1) or real(*a, **k))
-    rec = LR.Recorder().install(monkeypatch)
-    ref = ForkedRef.make([LR.LayerParams(layer, 0)], P, kv.shared_pages.cpu().numpy())
-    x = torch.from_numpy((np.random.default_rng(4).standard_normal((len(rows), 1024)) * 0.5).astype(np.float16)).to(DEV)
-    with torch.inference_mode():
-        out, step, rcalls, before, after = LR.run_step(rec, pool, layer, x, BatchLenInfo([], len(rows), DEV), None, kv, ids=False)
-    assert len(calls) == 1                                         # the attention call ran the cascade
-    ref.after, ref.dtab = after, step.dtab
-    ref.check_step(rcalls, step, before, after)
+    ref = LR.ModelRef([LR.LayerParams(layer, 0)], P, prefill_rows={0: [0, 1, 31, 32, 33, 1500, 3071]}, sm_count=sms)
+    d = Driver(monkeypatch, layer, pool, ref, ids=False)
+    d.step([("R", 3072, None)])
+    ref.prefill_rows = None
+    for i in range(8):
+        d.fork(f"F{i}", "R", total=1 + 9 * i)
+    d.step([(f"F{i}", 1 + 9 * i, 1 + 9 * i) for i in range(8)] + [("L0", 45, 45), ("L1", 300, 300)])
+    rows = [f"F{i}" for i in range(3)] + ["L0"] + [f"F{i}" for i in range(3, 8)] + ["L1"]
+    d.step([], rows)
+    d.step([], rows)
+    assert len(calls) == 2 and ref.calls["cascade decode"] == 2 and "decode" not in ref.calls     # the cascade ran, twice
+    print({k: round(v, 4) for k, v in sorted(ref.worst.items())})

@@ -1,6 +1,7 @@
 """GPU suite (-m gpu): decoder-layer and model steps checked tensor by tensor against tests/layer_ref64.py -- prefill, mixed
-prefill + decode and decode steps on multi-layer pools, both MLP paths on either side of the M = 64 switch, the Llama-7B shapes, and
-the serving loop's tokens.  Every kernel call of a step is recorded; the reference checks which call comes, what it was given and
+prefill + decode and decode steps on multi-layer pools, both MLP paths on either side of the M = 64 switch, the Llama-7B shapes,
+chunked prompts and continuations on forks, verify steps truncated and continued, and the serving loop's tokens with chunked
+prefill, a shared prefix and speculative decoding.  Every kernel call of a step is recorded; the reference checks which call comes, what it was given and
 what it returned, then audits the whole KV pool."""
 import numpy as np
 import pytest
@@ -207,42 +208,8 @@ def test_serving_loop_tokens_follow_the_float64_logits(monkeypatch):
     the scheduler forms them), the logits are read at the scheduler's last_token_rows, and every emitted token is the argmax of
     the float64 logits wherever the top-2 gap exceeds twice the bound."""
     from atom_b200 import textgen as tg
-    from atom_b200.kvcache import KvPoolInt4
-    model = _model(2, 512, 1024, 4, None, 1e4)
-    pool = KvPoolInt4(2, 4, 128, tg.pool_capacity(3, 72, 16), 16, DEV)
-    ref = R.model_ref(model, 16)
-    rec = R.Recorder().install(monkeypatch)
-    pending = {}
-
-    class Wrapped:
-        lm_head = model.lm_head             # the scheduler draws prompt ids below lm_head.out_features
-
-        def __call__(self, ids, blen, prefill_kv, decode_kv):
-            out, pending["step"], pending["calls"], pending["before"], pending["after"] = R.run_step(rec, pool, model, ids, blen,
-                                                                                                    prefill_kv, decode_kv)
-            return out
-
-    rows_of, commit = tg.TextGenScheduler.last_token_rows, tg.TextGenScheduler.commit
-
-    def last_token_rows(self):
-        pending["step"].rows = rows_of(self)
-        return pending["step"].rows
-
-    steps = []
-
-    def checked_commit(self, next_tokens, t1, t2):
-        s = pending.pop("step")
-        ref.check_step(pending["calls"], s, pending["before"], pending["after"])
-        ref.check_tokens(s, next_tokens)
-        steps.append((s.prefills, s.decode))
-        return commit(self, next_tokens, t1, t2)
-
-    monkeypatch.setattr(tg.TextGenScheduler, "last_token_rows", last_token_rows)
-    monkeypatch.setattr(tg.TextGenScheduler, "commit", checked_commit)
-    rs = tg.generate_request_set(7, 72)
-    res = tg.run_textgen(Wrapped(), rs, tg.TextGenConfig(3), pool, DEV, sync=torch.cuda.synchronize, keep_tokens=True)
-    assert [len(t) for t in res.tokens] == rs.output_lens.tolist()
-    assert any(p and d for p, d in steps), "the loop made no mixed step"
+    _, steps, _ = _serving_run(monkeypatch, tg.TextGenConfig(3))
+    assert any(p and d for p, d, _ in steps), "the loop made no mixed step"
 
 
 @pytest.mark.timeout(300)
@@ -277,3 +244,166 @@ def test_graphed_decode_step_equals_its_eager_replay():
         eager, _ = model(torch.tensor(toks, device=DEV), BatchLenInfo([], 3, DEV), None, BatchedKvCacheInt4(seqs))
     assert torch.equal(graphed, eager)
     assert torch.equal(graphed_pool[0], pool.buf) and torch.equal(graphed_pool[1].view(torch.int16), pool.param.view(torch.int16))
+
+
+# ------------------------------------------------------------------------------------------------ chunks, forks, verify steps
+def _driver(monkeypatch, fn, pool, ref, ids=True):
+    from tests.test_layer_ref64_cpu import Driver
+    return Driver(monkeypatch, fn, pool, ref, ids=ids, vocab=128)
+
+
+def _pool(layers, kv_heads, pages, P):
+    from atom_b200.kvcache import KvPoolInt4
+    pool = KvPoolInt4(layers, kv_heads, 128, pages, P, DEV)
+    pool.buf.random_(0, 256)
+    pool.param.view(torch.int16).random_(-32768, 32767)
+    return pool
+
+
+def _worst(ref):
+    """The largest error-to-bound ratio of each attention kind the reference checked (printed for the record, -s)."""
+    print({k: round(v, 4) for k, v in sorted(ref.worst.items())}, dict(ref.calls))
+
+
+@pytest.mark.timeout(900)
+@pytest.mark.parametrize("kv_heads,P", [(1, 16), (2, 32), (4, 16), (4, 32)])
+def test_chunked_prefill_and_continuations_on_forks(monkeypatch, kv_heads, P):
+    """Two-layer model: a root prefilled in two chunks (the second from position 21), a prompt chunked beside decode rows, forks of
+    the root at an aligned and an unaligned length with continuation prompts, then decode steps over the forks' shared pages."""
+    model = _model(2, 512, 1024, 4, kv_heads, 5e5 if P == 32 else 1e4)
+    pool = _pool(2, kv_heads, 40, P)
+    d = _driver(monkeypatch, model, pool, R.model_ref(model, P))
+    d.step([("R", 21, None), ("A", 16, 16)])
+    d.step([("R", 29, None), ("B", 19, 60)], ["A"])          # R from 21, B's first chunk: mixed with a decode row
+    d.fork("F1", "R", P, total=9)                             # aligned: shares the first page
+    d.fork("F2", "R", total=P + 3)                            # at 50: its partly filled page copied
+    d.step([("B", 41, None), ("F1", 9, 9), ("F2", P + 3, P + 3)], ["A"])
+    for _ in range(P // 2 + 2):
+        d.step([], ["A", "B", "F1", "F2"])
+    assert d.ref.calls["prefill over a cached prefix"] == 2 * 2 and d.ref.calls["decode"] == 2 * (P // 2 + 4)
+    _worst(d.ref)
+
+
+@pytest.mark.timeout(900)
+@pytest.mark.parametrize("kv_heads", [2, 4])
+def test_verify_steps_with_prompt_chunks_truncated_and_continued(monkeypatch, kv_heads):
+    """Two-layer model, GQA (2 KV heads) or MHA (4): verify steps of S = 4, 8 and 2 rows per sequence beside prompt chunks,
+    truncated to kept counts from 1 to S (back across page boundaries and inside pages), a verify step with greedy acceptance
+    of the drafts, and decode steps between them."""
+    model = _model(2, 512, 1024, 4, kv_heads, 5e5)
+    P = 16
+    pool = _pool(2, kv_heads, 48, P)
+    d = _driver(monkeypatch, model, pool, R.model_ref(model, P))
+    d.step([("A", 13, 13), ("B", 30, 30), ("C", 17, 40)])
+    d.step([("C", 23, None)], ["A", "B"], S=4, kept=[4, 1])
+    d.step([("D", 5, 5)], ["A", "B", "C"], S=8, kept=[3, 8, 1])
+    d.step([], ["A", "B", "C", "D"], S=2, kept=[2, 1, 2, 1])
+    d.step([], ["A", "B", "C", "D"])
+    d.step([], ["A", "B", "C", "D"], S=4)
+    d.step([("E", 9, 9)], ["A", "B", "C", "D"], S=8, kept=[8, 5, 2, 7])
+    d.step([], ["A", "B", "C", "D", "E"])
+    assert d.ref.calls["verify"] == 2 * 5
+    _worst(d.ref)
+
+
+@pytest.mark.timeout(900)
+def test_mixtral_layer_verify_steps(monkeypatch):
+    """Toy Mixtral layer (512 / 1024, 4 experts, top-2, 4 query and 2 KV heads): the MoE block on batches of S-row verify steps
+    beside prompt chunks, truncated and continued."""
+    from atom_b200.mixtral import MixtralConfig
+    cfg = MixtralConfig(hidden_size=512, intermediate_size=1024, num_attention_heads=4, num_key_value_heads=2, num_hidden_layers=1,
+                        num_local_experts=4, num_experts_per_tok=2, rope_theta=1e6)
+    layer = _mixtral_layer(cfg)
+    P = 16
+    pool = _pool(1, 2, 24, P)
+    d = _driver(monkeypatch, layer, pool, R.ModelRef([R.LayerParams(layer, 0)], P), ids=False)
+    d.step([("A", 5, 5), ("B", 20, 37)])
+    d.step([("B", 17, None)], ["A"], S=4, kept=[2])
+    d.step([("C", 9, 9)], ["A", "B"], S=8, kept=[8, 3])
+    d.step([], ["A", "B", "C"], S=2, kept=[1, 2, 2])
+    d.step([], ["A", "B", "C"])
+    assert d.ref.calls["verify"] == 3
+    _worst(d.ref)
+
+
+def _serving_run(monkeypatch, cfg, maxlen=72):
+    """run_textgen, eager, on the model of test_z_textgen_gpu.py with every step checked and every emitted token held to the
+    float64 logits (check_tokens, or check_spec under speculation, which also sets the lengths the truncations must leave)."""
+    from atom_b200 import textgen as tg
+    from atom_b200.kvcache import KvCacheInt4, KvPoolInt4
+    model = _model(2, 512, 1024, 4, None, 1e4)
+    P = 16
+    K = 0 if cfg.speculate is None else cfg.speculate.num_draft
+    pool = KvPoolInt4(2, 4, 128, tg.pool_capacity(3, maxlen + cfg.shared_prefix, P, K) + 8, P, DEV)
+    ref = R.model_ref(model, P, sm_count=torch.cuda.get_device_properties(DEV).multi_processor_count)
+    rec = R.Recorder().install(monkeypatch)
+    pending, steps = {}, []
+    fork = KvCacheInt4.fork
+
+    def forked(kv, n=None):
+        child = fork(kv, n)
+        ref.fork(list(kv.indicies), child.seqlen, list(child.indicies))
+        return child
+    monkeypatch.setattr(KvCacheInt4, "fork", forked)
+
+    class Wrapped:
+        lm_head = model.lm_head             # the scheduler draws prompt ids below lm_head.out_features
+
+        def __call__(self, ids, blen, prefill_kv, decode_kv):
+            out, pending["step"], pending["calls"], pending["before"], pending["after"] = R.run_step(rec, pool, model, ids, blen,
+                                                                                                    prefill_kv, decode_kv)
+            return out
+
+    rows_of, commit, commit_spec = tg.TextGenScheduler.last_token_rows, tg.TextGenScheduler.commit, tg.TextGenScheduler.commit_spec
+
+    def last_token_rows(self):
+        pending["step"].rows = rows_of(self)
+        return pending["step"].rows
+
+    def checked(self):
+        s = pending.pop("step")
+        ref.check_step(pending["calls"], s, pending["before"], pending["after"])
+        steps.append((s.prefills, s.decode, s.decode_len))
+        return s
+
+    def checked_commit(self, next_tokens, t1, t2, *a, **k):
+        if k.get("_speculative"):
+            return commit(self, next_tokens, t1, t2, *a, **k)
+        ref.check_tokens(checked(self), next_tokens)
+        return commit(self, next_tokens, t1, t2, *a, **k)
+
+    def checked_commit_spec(self, out, t1, t2, logprobs=None):
+        s = checked(self)
+        out = np.asarray(out)
+        room = [int(self.rs.output_lens[r.req_idx]) - len(r.output) for r in self.workset]
+        ref.check_spec(s, [list(r.drafts) for r in self.workset], [o[2:2 + int(o[0])].tolist() for o in out], room, self.stop_token_ids)
+        return commit_spec(self, out, t1, t2, logprobs)
+
+    monkeypatch.setattr(tg.TextGenScheduler, "last_token_rows", last_token_rows)
+    monkeypatch.setattr(tg.TextGenScheduler, "commit", checked_commit)
+    monkeypatch.setattr(tg.TextGenScheduler, "commit_spec", checked_commit_spec)
+    rs = tg.generate_request_set(7, maxlen)
+    res = tg.run_textgen(Wrapped(), rs, cfg, pool, DEV, sync=torch.cuda.synchronize, keep_tokens=True)
+    assert [len(t) for t in res.tokens] == rs.output_lens.tolist()
+    assert pool.num_free_blocks == pool.capacity                # every page given back, truncations included
+    _worst(ref)
+    return res, steps, ref
+
+
+@pytest.mark.timeout(1200)
+@pytest.mark.parametrize("kind", ["chunked", "shared_prefix", "speculative", "all"])
+def test_serving_loop_variants_follow_the_float64_logits(monkeypatch, kind):
+    """The serving loop with chunked prefill (16 tokens a step), a 70-token shared prefix forked for every request (24-token
+    chunks), speculative decoding (4 drafts of 1- to 3-grams), and all three together: every step checked, every emitted token
+    the float64 argmax wherever the top-2 gap is clear, and under speculation the drafts accepted exactly when they are it."""
+    from atom_b200 import textgen as tg
+    spec = tg.SpeculativeParams(4, 3, 1) if kind in ("speculative", "all") else None
+    chunk = {"chunked": 16, "shared_prefix": 24, "all": 16}.get(kind)
+    shared = 70 if kind in ("shared_prefix", "all") else 0
+    res, steps, ref = _serving_run(monkeypatch, tg.TextGenConfig(3, prefill_chunk=chunk, shared_prefix=shared, speculate=spec))
+    if chunk:
+        assert ref.calls["prefill over a cached prefix"] > 0
+    if spec is not None:
+        st = res.speculative
+        assert any(S > 1 for _, _, S in steps) and ref.calls["verify"] > 0
+        assert 0 < st["accepted_tokens"] < st["drafted_tokens"], st          # drafts both accepted and rejected

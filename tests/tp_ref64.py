@@ -127,7 +127,7 @@ class RankRef(R.ModelRef):
         """Walk this rank's trace of one decode step (generator, see TPRef.check_step).  Returns (residual sums, layer output)."""
         self._calls, self._pos, self._doff = calls, 0, 0
         m = int(step.decode)
-        _, dkeys = self._admit(step)
+        _, drows = self._admit(step)
         residual, pend, sums = step.x, None, []
         push = self.tp.can_push(m)
         for l, p in enumerate(self.layers):
@@ -146,7 +146,7 @@ class RankRef(R.ModelRef):
             sums.append(residual)
             # ---- attention
             q, k4, ks, v4, vs = self._qkv(L, p, x, m, fused=m <= 64)
-            attn = self._decode(L, l, p, q, k4, ks, v4, vs, 0, m, dkeys, step.dtab)
+            attn = self._decode(L, l, p, q, k4, ks, v4, vs, 0, m, drows, step.dtab)
             xo = self._reorder(L, p, attn, m)
             kind, rows, o = yield from self._row_parallel(f"{L} o_proj", p.o, xo, m, push)
             # ---- post-attention norm (+ o_proj's all-reduce)
@@ -179,21 +179,28 @@ class RankRef(R.ModelRef):
             self._fail(f"layer {len(self.layers) - 1} output", "residual + down_proj is not the exact FP16 sum")
         return sums, residual
 
+    def settle(self, before=None, after=None):
+        """After the step: the pool audit (before / after: this rank's pool) and the sequences' new ends."""
+        if after is not None:
+            self._audit(before, after)
+        self._settle()
+
 
 def seed_history(ref, dtab, pool):
     """Give the ModelRef `ref` the sequences of the decode page table `dtab` that it does not know yet (each one position longer
     than before the step) and their history, in every layer, from `pool` = (data, param) as it was before that step.
     TPRef.check_step does this with its `before` pools: a sequence's history is read from the pool once, before its first step."""
     data, param = pool
+    L = len(ref.layers)
     for pages, n in R.sequences(dtab, ref.P):
-        if pages[0] in ref.seqs:
-            continue
         n0 = n - 1
-        ref.seqs[pages[0]] = (pages[:-(-n0 // ref.P)], n0)
-        t = np.arange(n0)
-        pg, e = np.asarray(pages)[t // ref.P], t % ref.P
-        for l in range(len(ref.layers)):
-            ref.hist[(pages[0], l)] = [data[pg, l, 0, :, e], param[pg, l, 0, :, e], data[pg, l, 1, :, e], param[pg, l, 1, :, e]]
+        ref._ensure(pages)
+        if n0 == 0 or ref.ends.get(ref._end(pages, n0), [None])[0] == n0:
+            continue
+        pg, e = ref._slots(pages, np.arange(n0))
+        ref.sd[pg, :, :, :, e], ref.sp[pg, :, :, :, e] = data[pg, :L, :, :, e], param[pg, :L, :, :, e]
+        ref.known[pg, :, e] = True
+        ref._register(pages, n0)
 
 
 class TPRef:
@@ -257,10 +264,8 @@ class TPRef:
                     self.ranks[r]._fail(f"layer {i // 2} {stage}", "the residual stream differs from rank 0's")
             if not R.same(out, out0):
                 self.ranks[r]._fail(f"layer {len(self.ranks[r].layers) - 1} output", "the layer output differs from rank 0's")
-        if after is not None:
-            for rk, b, a in zip(self.ranks, before, after):
-                keys = [pages[0] for pages, _ in R.sequences(dtab, rk.P)]
-                rk._audit(b, a, keys)
+        for r, rk in enumerate(self.ranks):
+            rk.settle(None if before is None else before[r], None if after is None else after[r])
 
     @staticmethod
     def _advance(g, value, r, results):
