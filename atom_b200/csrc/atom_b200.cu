@@ -512,17 +512,16 @@ static int prefill_attention(const char* what, const void* q, const void* k, con
   int rc = check_launch("prefill_attention_i4 (dequant + RoPE)");
   if (rc) return rc;
   const unsigned q_tiles = (unsigned)((max_len + atom::PF_BQ - 1) / atom::PF_BQ);
-  const float scale_log2 = 0.08838834764831845f * 1.4426950408889634f;
   if (ctx == nullptr) {
     const dim3 grid(q_tiles, (unsigned)batch_size, (unsigned)num_heads);
     atom::prefill_attn_kernel<false><<<grid, atom::PF_THREADS, 0, (cudaStream_t)stream>>>(
         (const __half*)q, (const __half*)k_f16, (const __half*)v_f16, (const int32_t*)seqlen_indptr, (const float2*)rope_table,
-        (__half*)out, num_heads, num_kv_heads, scale_log2);
+        (__half*)out, num_heads, num_kv_heads);
   } else {
     const dim3 grid(q_tiles * (unsigned)(num_heads / num_kv_heads), (unsigned)num_kv_heads, (unsigned)batch_size);
     atom::prefill_attn_kernel<true, atom::KvArgs><<<grid, atom::PF_THREADS, 0, (cudaStream_t)stream>>>(
         (const __half*)q, (const __half*)k_f16, (const __half*)v_f16, (const int32_t*)seqlen_indptr, (const float2*)rope_table,
-        (__half*)out, num_heads, num_kv_heads, scale_log2, *ctx);
+        (__half*)out, num_heads, num_kv_heads, *ctx);
   }
   return check_launch(what);
 }
@@ -556,11 +555,38 @@ int atom_allreduce_push_f16(const void* in, void* out, const void* peer_buffers,
 
 int atom_allreduce_state_words(void) { return atom::AR_STATE_WORDS; }
 
-static int kv_check(const char* what, const void* data, const void* param, const void* indptr, const void* indices,
-                    const void* last, int L, int layer, int H, int P, int B) {
+// the checks of every call on the INT4 page pool, and the KvArgs it launches with
+static int kv_args(const char* what, const void* data, const void* param, const void* indptr, const void* indices, const void* last,
+                   int L, int layer, int H, int P, int B, atom::KvArgs* kv) {
   ATOM_REQUIRE(data && param && indptr && indices && last, "%s: null pointer argument", what);
   ATOM_REQUIRE(L > 0 && layer >= 0 && layer < L, "%s: layer_idx=%d out of range [0,%d)", what, layer, L);
   ATOM_REQUIRE(H > 0 && P > 0 && B > 0, "%s: num_heads=%d page_size=%d batch_size=%d must be positive", what, H, P, B);
+  *kv = atom::KvArgs{(uint8_t*)data, (__half2*)param, (const int32_t*)indptr, (const int32_t*)indices, (const int32_t*)last, L, layer, H, P,
+                     B};
+  return ATOM_OK;
+}
+
+// The checks every paged-attention entry point makes, and the KvArgs and group size (query heads per KV head) it launches with.
+// rope_theta: nullptr for an entry whose rotation comes from a table alone.  rope_table / workspace: the entry's pointers that must
+// be 16-byte aligned with the pool (nullptr: none), named in the message by `aligned`.
+static int paged_attn_args(const char* what, const void* kv_data, const void* kv_param, const void* kv_indptr, const void* kv_indices,
+                           const void* last_page_offset, int num_layers, int layer_idx, int num_q_heads, int num_kv_heads, int page_size,
+                           int batch_size, const float* rope_theta, const void* rope_table, const void* workspace, const char* aligned,
+                           atom::KvArgs* kv, int* group) {
+  int rc = kv_args(what, kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx, num_kv_heads, page_size,
+                   batch_size, kv);
+  if (rc) return rc;
+  ATOM_REQUIRE(num_q_heads > 0 && num_q_heads % num_kv_heads == 0,
+               "%s: num_q_heads=%d must be a positive multiple of num_kv_heads=%d", what, num_q_heads, num_kv_heads);
+  if (rope_theta)
+    ATOM_REQUIRE(*rope_theta > 1.f && *rope_theta < 1e30f, "%s: rope_theta=%g must be a finite base above 1", what, (double)*rope_theta);
+  *group = num_q_heads / num_kv_heads;
+  if (*group != 1 && *group != 2 && *group != 4 && *group != 8)
+    return fail(ATOM_E_UNSUPPORTED, "%s: %d query heads per KV head (num_q_heads=%d, num_kv_heads=%d); supported group sizes are 1, 2, "
+                                    "4 and 8", what, *group, num_q_heads, num_kv_heads);
+  ATOM_REQUIRE(page_size % 8 == 0 && page_size <= 64, "%s: page_size=%d must be a multiple of 8, at most 64", what, page_size);
+  ATOM_REQUIRE(aligned16(kv_data) && aligned16(kv_param) && aligned16(rope_table) && aligned16(workspace),
+               "%s: %s must be 16-byte aligned", what, aligned);
   return ATOM_OK;
 }
 
@@ -571,20 +597,11 @@ int atom_prefill_attention_ctx_gqa_i4(const void* q, const void* k, const void* 
                                       const void* kv_indices, const void* last_page_offset, int num_layers, int layer_idx,
                                       int page_size, void* stream) {
   const char* what = "prefill_attention_ctx_gqa_i4";
-  int rc = kv_check(what, kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx, num_kv_heads, page_size,
-                    batch_size);
+  atom::KvArgs kv;
+  int group;
+  int rc = paged_attn_args(what, kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx, num_q_heads,
+                           num_kv_heads, page_size, batch_size, nullptr, rope_table, nullptr, "KV pool and rope table", &kv, &group);
   if (rc) return rc;
-  ATOM_REQUIRE(num_q_heads > 0 && num_q_heads % num_kv_heads == 0,
-               "%s: num_q_heads=%d must be a positive multiple of num_kv_heads=%d", what, num_q_heads, num_kv_heads);
-  const int group = num_q_heads / num_kv_heads;
-  if (group != 1 && group != 2 && group != 4 && group != 8)
-    return fail(ATOM_E_UNSUPPORTED, "%s: %d query heads per KV head (num_q_heads=%d, num_kv_heads=%d); supported group sizes are 1, 2, "
-                                    "4 and 8", what, group, num_q_heads, num_kv_heads);
-  ATOM_REQUIRE(page_size % 8 == 0 && page_size <= 64, "%s: page_size=%d must be a multiple of 8, at most 64", what, page_size);
-  ATOM_REQUIRE(aligned16(kv_data) && aligned16(kv_param) && aligned16(rope_table), "%s: KV pool and rope table must be 16-byte aligned",
-               what);
-  const atom::KvArgs kv{(uint8_t*)kv_data, (__half2*)kv_param, (const int32_t*)kv_indptr, (const int32_t*)kv_indices,
-                        (const int32_t*)last_page_offset, num_layers, layer_idx, num_kv_heads, page_size, batch_size};
   return prefill_attention(what, q, k, k_param, v, v_param, seqlen_indptr, pos_of_token, rope_table, k_f16, v_f16, out, total_tokens,
                            batch_size, max_len, num_q_heads, num_kv_heads, stream, &kv);
 }
@@ -715,21 +732,12 @@ static int launch_decode_shared(const char* what, void* o, const void* q, const 
 static int batch_decode(const char* what, void* o, const void* q, const void* kv_data, const void* kv_param, const void* kv_indptr,
                         const void* kv_indices, const void* last_page_offset, int num_layers, int layer_idx, int num_q_heads,
                         int num_kv_heads, int page_size, int batch_size, float rope_theta, int kv_split, void* stream) {
-  int rc = kv_check(what, kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx, num_kv_heads, page_size,
-                    batch_size);
+  atom::KvArgs kv;
+  int group;
+  int rc = paged_attn_args(what, kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx, num_q_heads,
+                           num_kv_heads, page_size, batch_size, &rope_theta, nullptr, nullptr, "KV pool", &kv, &group);
   if (rc) return rc;
   ATOM_REQUIRE(o && q, "%s: null q/o", what);
-  ATOM_REQUIRE(num_q_heads > 0 && num_q_heads % num_kv_heads == 0,
-               "%s: num_q_heads=%d must be a positive multiple of num_kv_heads=%d", what, num_q_heads, num_kv_heads);
-  ATOM_REQUIRE(rope_theta > 1.f && rope_theta < 1e30f, "%s: rope_theta=%g must be a finite base above 1", what, (double)rope_theta);
-  const int group = num_q_heads / num_kv_heads;
-  if (group != 1 && group != 2 && group != 4 && group != 8)
-    return fail(ATOM_E_UNSUPPORTED, "%s: %d query heads per KV head (num_q_heads=%d, num_kv_heads=%d); supported group sizes are 1, 2, "
-                                    "4 and 8", what, group, num_q_heads, num_kv_heads);
-  ATOM_REQUIRE(page_size % 8 == 0 && page_size <= 64, "%s: page_size=%d must be a multiple of 8, at most 64", what, page_size);
-  ATOM_REQUIRE(aligned16(kv_data) && aligned16(kv_param), "%s: KV pool must be 16-byte aligned", what);
-  const atom::KvArgs kv{(uint8_t*)kv_data, (__half2*)kv_param, (const int32_t*)kv_indptr, (const int32_t*)kv_indices,
-                        (const int32_t*)last_page_offset, num_layers, layer_idx, num_kv_heads, page_size, batch_size};
   ATOM_REQUIRE(kv_split == 0 || kv_split == 1 || kv_split == 2 || kv_split == 4 || kv_split == 8,
                "%s: kv_split=%d must be 0 (automatic), 1 (no split), 2, 4 or 8", what, kv_split);
   int split = kv_split;
@@ -802,24 +810,15 @@ int atom_batch_decode_shared_gqa_i4(void* o, const void* q, const void* kv_data,
                                     const void* group_indptr, const void* group_members, const void* shared_pages, int num_groups,
                                     int max_group_size, const void* rope_table, float* workspace, int nchunks, void* stream) {
   const char* what = "batch_decode_shared_gqa_i4";
-  int rc = kv_check(what, kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx, num_kv_heads, page_size,
-                    batch_size);
+  atom::KvArgs kv;
+  int group;
+  int rc = paged_attn_args(what, kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx, num_q_heads,
+                           num_kv_heads, page_size, batch_size, &rope_theta, rope_table, workspace, "KV pool, rope table and workspace",
+                           &kv, &group);
   if (rc) return rc;
   ATOM_REQUIRE(o && q && group_indptr && group_members && shared_pages && rope_table && workspace, "%s: null pointer argument", what);
-  ATOM_REQUIRE(num_q_heads > 0 && num_q_heads % num_kv_heads == 0,
-               "%s: num_q_heads=%d must be a positive multiple of num_kv_heads=%d", what, num_q_heads, num_kv_heads);
-  ATOM_REQUIRE(rope_theta > 1.f && rope_theta < 1e30f, "%s: rope_theta=%g must be a finite base above 1", what, (double)rope_theta);
-  const int group = num_q_heads / num_kv_heads;
-  if (group != 1 && group != 2 && group != 4 && group != 8)
-    return fail(ATOM_E_UNSUPPORTED, "%s: %d query heads per KV head (num_q_heads=%d, num_kv_heads=%d); supported group sizes are 1, 2, "
-                                    "4 and 8", what, group, num_q_heads, num_kv_heads);
-  ATOM_REQUIRE(page_size % 8 == 0 && page_size <= 64, "%s: page_size=%d must be a multiple of 8, at most 64", what, page_size);
-  ATOM_REQUIRE(aligned16(kv_data) && aligned16(kv_param) && aligned16(rope_table) && aligned16(workspace),
-               "%s: KV pool, rope table and workspace must be 16-byte aligned", what);
   ATOM_REQUIRE(num_groups > 0 && max_group_size >= 2 && max_group_size <= batch_size && nchunks > 0,
                "%s: num_groups=%d max_group_size=%d nchunks=%d (batch %d)", what, num_groups, max_group_size, nchunks, batch_size);
-  const atom::KvArgs kv{(uint8_t*)kv_data, (__half2*)kv_param, (const int32_t*)kv_indptr, (const int32_t*)kv_indices,
-                        (const int32_t*)last_page_offset, num_layers, layer_idx, num_kv_heads, page_size, batch_size};
   const atom::DecPrefix px{(const int32_t*)group_indptr, (const int32_t*)group_members, (const int32_t*)shared_pages, workspace, nchunks};
   const float log2_theta = log2f(rope_theta);
   const cudaStream_t st = (cudaStream_t)stream;
@@ -848,25 +847,16 @@ int atom_batch_verify_gqa_i4(void* o, const void* q, const void* kv_data, const 
                              int num_kv_heads, int page_size, int batch_size, int tokens_per_seq, float rope_theta,
                              const void* rope_table, float* workspace, int nchunks, void* stream) {
   const char* what = "batch_verify_gqa_i4";
-  int rc = kv_check(what, kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx, num_kv_heads, page_size,
-                    batch_size);
+  atom::KvArgs kv;
+  int group;
+  int rc = paged_attn_args(what, kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx, num_q_heads,
+                           num_kv_heads, page_size, batch_size, &rope_theta, rope_table, workspace, "KV pool, rope table and workspace",
+                           &kv, &group);
   if (rc) return rc;
   ATOM_REQUIRE(o && q && rope_table, "%s: null pointer argument", what);
-  ATOM_REQUIRE(num_q_heads > 0 && num_q_heads % num_kv_heads == 0,
-               "%s: num_q_heads=%d must be a positive multiple of num_kv_heads=%d", what, num_q_heads, num_kv_heads);
-  ATOM_REQUIRE(rope_theta > 1.f && rope_theta < 1e30f, "%s: rope_theta=%g must be a finite base above 1", what, (double)rope_theta);
-  const int group = num_q_heads / num_kv_heads;
-  if (group != 1 && group != 2 && group != 4 && group != 8)
-    return fail(ATOM_E_UNSUPPORTED, "%s: %d query heads per KV head (num_q_heads=%d, num_kv_heads=%d); supported group sizes are 1, 2, "
-                                    "4 and 8", what, group, num_q_heads, num_kv_heads);
   ATOM_REQUIRE(tokens_per_seq >= 1 && tokens_per_seq <= 8, "%s: tokens_per_seq=%d must be in [1, 8]", what, tokens_per_seq);
-  ATOM_REQUIRE(page_size % 8 == 0 && page_size <= 64, "%s: page_size=%d must be a multiple of 8, at most 64", what, page_size);
   ATOM_REQUIRE(nchunks >= 1 && nchunks <= 64 && (nchunks == 1 || workspace), "%s: nchunks=%d must be in [1, 64], with a workspace above 1",
                what, nchunks);
-  ATOM_REQUIRE(aligned16(kv_data) && aligned16(kv_param) && aligned16(rope_table) && aligned16(workspace),
-               "%s: KV pool, rope table and workspace must be 16-byte aligned", what);
-  const atom::KvArgs kv{(uint8_t*)kv_data, (__half2*)kv_param, (const int32_t*)kv_indptr, (const int32_t*)kv_indices,
-                        (const int32_t*)last_page_offset, num_layers, layer_idx, num_kv_heads, page_size, batch_size};
   const cudaStream_t st = (cudaStream_t)stream;
   rc = launch_k(what, atom::verify_attn_kernel, dim3(nchunks, num_kv_heads, batch_size), dim3(atom::PF_THREADS), 0, st, (__half*)o,
                 (const __half*)q, kv, (const float2*)rope_table, log2f(rope_theta), tokens_per_seq, group, workspace, nchunks);
@@ -879,12 +869,11 @@ int atom_append_kv_i4(void* kv_data, void* kv_param, const void* kv_indptr, cons
                       const void* last_page_offset, const void* k, const void* v, const void* k_param,
                       const void* v_param, int num_layers, int layer_idx, int num_heads, int page_size, int batch_size,
                       void* stream) {
-  int rc = kv_check("append_kv_i4", kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx,
-                    num_heads, page_size, batch_size);
+  atom::KvArgs kv;
+  int rc = kv_args("append_kv_i4", kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx, num_heads,
+                   page_size, batch_size, &kv);
   if (rc) return rc;
   ATOM_REQUIRE(k && v && k_param && v_param, "append_kv_i4: null k/v");
-  atom::KvArgs kv{(uint8_t*)kv_data, (__half2*)kv_param, (const int32_t*)kv_indptr, (const int32_t*)kv_indices,
-                  (const int32_t*)last_page_offset, num_layers, layer_idx, num_heads, page_size, batch_size};
   const long long threads = (long long)batch_size * num_heads * 16;
   return launch_k("append_kv_i4", atom::append_kv_kernel, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, (cudaStream_t)stream, kv,
                   (const uint8_t*)k, (const uint8_t*)v, (const __half2*)k_param, (const __half2*)v_param,
@@ -895,13 +884,12 @@ int atom_init_kv_i4(void* kv_data, void* kv_param, const void* kv_indptr, const 
                     const void* last_page_offset, const void* k, const void* v, const void* k_param,
                     const void* v_param, const void* seqlen_indptr, int total_tokens, int num_layers, int layer_idx,
                     int num_heads, int page_size, int batch_size, void* stream) {
-  int rc = kv_check("init_kv_i4", kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx,
-                    num_heads, page_size, batch_size);
+  atom::KvArgs kv;
+  int rc = kv_args("init_kv_i4", kv_data, kv_param, kv_indptr, kv_indices, last_page_offset, num_layers, layer_idx, num_heads, page_size,
+                   batch_size, &kv);
   if (rc) return rc;
   ATOM_REQUIRE(k && v && k_param && v_param && seqlen_indptr, "init_kv_i4: null k/v/seqlen_indptr");
   if (total_tokens <= 0) return ATOM_OK;
-  atom::KvArgs kv{(uint8_t*)kv_data, (__half2*)kv_param, (const int32_t*)kv_indptr, (const int32_t*)kv_indices,
-                  (const int32_t*)last_page_offset, num_layers, layer_idx, num_heads, page_size, batch_size};
   const long long threads = (long long)total_tokens * num_heads * 16;
   return launch_k("init_kv_i4", atom::append_kv_kernel, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, (cudaStream_t)stream, kv,
                   (const uint8_t*)k, (const uint8_t*)v, (const __half2*)k_param, (const __half2*)v_param,

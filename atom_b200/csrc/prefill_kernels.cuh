@@ -7,7 +7,8 @@
 //     init_kv_i4 scatters into the page pool, page.cuh:165-216): x = nibble * scale - zero, rounded to FP16 as the
 //     decode path sees it;
 //   * RoPE (theta = 1e4, pairs (i, i + 64), llama.py:18-32) on q and k from a (cos, sin) table of the positions;
-//   * flash-attention recurrence (online softmax in FP32, base 2), FP16 tensor-core MMAs with FP32 accumulation.
+//   * flash-attention recurrence (online softmax in FP32, base 2), FP16 tensor-core MMAs with FP32 accumulation: the tile step
+//     attn_tile_step below, which the verify and shared-prefix kernels run too.
 // Two launches: kv_dequant_rope_kernel turns the packed K/V into FP16 once (K rotated), because every K/V tile is reused by
 // all later query tiles of its prompt; prefill_attn_kernel is the attention proper.
 // Tiling: CTA = 64 query rows of one (prompt, head), 4 warps x 16 rows; K/V in 64-token tiles through shared memory
@@ -135,6 +136,129 @@ __device__ __forceinline__ void prefill_ctx_tile(const KvArgs& kv, int b, int L,
 __device__ __forceinline__ int prefill_ctx_len(int, int) { return 0; }                             // <false>: no cache
 __device__ __forceinline__ void prefill_ctx_tile(int, int, int, int, const float2*, __half*, __half*, int) {}
 
+constexpr float ATTN_SCALE_LOG2 = 0.08838834764831845f * 1.4426950408889634f;   // 1/sqrt(128) * log2(e), as the decode kernel
+
+// The consumer of one 64-key tile, shared by the prefill, verify and shared-prefix kernels.  A warp owns 16 query rows of the
+// m16n8k16 fragments; a thread holds rows g and g + 8 (row rr = 0, 1; g = lane / 4) and columns 2t, 2t + 1 of each 8-column
+// block (t = lane % 4).  S = Q K^T from the rotated Q fragments qa and the tile in Ks (keys k0 .. k0 + 63), scaled to base 2;
+// key kpos is kept for row rr where visible(rr, kpos), else -inf.  Then the online softmax in FP32 -- the quad's row maximum,
+// the rescale of (o, l), P rounded to FP16 -- and O += P V from the tile in Vt.  A row that has seen no visible key yet keeps
+// m = -inf; its exponentials are taken against 0, which keeps exp2(-inf - -inf) out of the recurrence (o and l stay 0).
+template <typename Visible>
+__device__ __forceinline__ void attn_tile_step(const uint32_t (&qa)[8][4], const __half* Ks, const __half* Vt, int k0, Visible visible,
+                                               float (&o)[16][4], float& m0, float& m1, float& l0, float& l1) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  float s[8][4];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      const uint32_t b0 = *reinterpret_cast<const uint32_t*>(&Ks[(8 * j + g) * PF_KPITCH + 16 * kk + 2 * t]);
+      const uint32_t b1 = *reinterpret_cast<const uint32_t*>(&Ks[(8 * j + g) * PF_KPITCH + 16 * kk + 8 + 2 * t]);
+      mma_16816(s[j], qa[kk], b0, b1);
+    }
+  }
+  float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      const int kpos = k0 + 8 * j + 2 * t + u;
+      s[j][u] = visible(0, kpos) ? s[j][u] * ATTN_SCALE_LOG2 : -INFINITY;
+      s[j][2 + u] = visible(1, kpos) ? s[j][2 + u] * ATTN_SCALE_LOG2 : -INFINITY;
+      mx0 = fmaxf(mx0, s[j][u]); mx1 = fmaxf(mx1, s[j][2 + u]);
+    }
+  }
+  mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1)); mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+  mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1)); mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+  const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);
+  const float base0 = mn0 == -INFINITY ? 0.f : mn0, base1 = mn1 == -INFINITY ? 0.f : mn1;
+  const float a0 = exp2f(m0 - base0), a1 = exp2f(m1 - base1);
+  m0 = mn0; m1 = mn1;
+  float sum0 = 0.f, sum1 = 0.f;
+  uint32_t pa[4][4];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float p00 = exp2f(s[j][0] - base0), p01 = exp2f(s[j][1] - base0);
+    const float p10 = exp2f(s[j][2] - base1), p11 = exp2f(s[j][3] - base1);
+    sum0 += p00 + p01; sum1 += p10 + p11;
+    pa[j >> 1][(j & 1) * 2 + 0] = pack_h2(p00, p01);
+    pa[j >> 1][(j & 1) * 2 + 1] = pack_h2(p10, p11);
+  }
+  l0 = l0 * a0 + sum0; l1 = l1 * a1 + sum1;
+#pragma unroll
+  for (int i = 0; i < 16; ++i) { o[i][0] *= a0; o[i][1] *= a0; o[i][2] *= a1; o[i][3] *= a1; }
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      const uint32_t b0 = *reinterpret_cast<const uint32_t*>(&Vt[(8 * i + g) * PF_VPITCH + 16 * kk + 2 * t]);
+      const uint32_t b1 = *reinterpret_cast<const uint32_t*>(&Vt[(8 * i + g) * PF_VPITCH + 16 * kk + 8 + 2 * t]);
+      mma_16816(o[i], pa[kk], b0, b1);
+    }
+  }
+}
+
+// Q fragments of a thread's two rows (row rr: q row qr[rr], position pos[rr]) rotated at positions read on the device, so a
+// captured graph replays with new lengths: the angle pos * theta^(-d/64) by FP32 sincosf, the rotation in FP32, rounded to FP16
+// once (the decode kernel's arithmetic)
+__device__ __forceinline__ void rope_q_frags(uint32_t (&qa)[8][4], const __half* const (&qr)[2], const int (&pos)[2], float log2_theta) {
+  const int t = threadIdx.x & 3;
+  const float kFreqStep = log2_theta / 64.f;
+  float2 lo[2][4][2], hi[2][4][2];
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) {
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+      for (int hf = 0; hf < 2; ++hf) {            // columns d = 16 kk + 8 hf + 2 t, d + 1 and their partners d + 64
+        const int d = 16 * kk + 8 * hf + 2 * t;
+        const float2 x = __half22float2(*reinterpret_cast<const __half2*>(qr[rr] + d));
+        const float2 y = __half22float2(*reinterpret_cast<const __half2*>(qr[rr] + d + 64));
+        float s0, c0, s1, c1;
+        sincosf((float)pos[rr] * exp2f(-(float)d * kFreqStep), &s0, &c0);
+        sincosf((float)pos[rr] * exp2f(-(float)(d + 1) * kFreqStep), &s1, &c1);
+        lo[rr][kk][hf] = make_float2(x.x * c0 - y.x * s0, x.y * c1 - y.y * s1);
+        hi[rr][kk][hf] = make_float2(y.x * c0 + x.x * s0, y.y * c1 + x.y * s1);
+      }
+    }
+  }
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        qa[kk][2 * hf + rr] = pack_h2(lo[rr][kk][hf].x, lo[rr][kk][hf].y);
+        qa[kk + 4][2 * hf + rr] = pack_h2(hi[rr][kk][hf].x, hi[rr][kk][hf].y);
+      }
+}
+
+// row sum of l over the quad of threads that share a row
+__device__ __forceinline__ float quad_sum(float x) {
+  x += __shfl_xor_sync(0xffffffffu, x, 1);
+  return x + __shfl_xor_sync(0xffffffffu, x, 2);
+}
+
+// row rr of this thread's o fragments, normalised by its quad-summed l and rounded to FP16, into the row's 128 halves at dst
+__device__ __forceinline__ void attn_store_row(__half* dst, const float (&o)[16][4], int rr, float l) {
+  const int t = threadIdx.x & 3;
+  const float inv = 1.f / l;
+#pragma unroll
+  for (int i = 0; i < 16; ++i)
+    *reinterpret_cast<uint32_t*>(dst + 8 * i + 2 * t) = pack_h2(o[i][2 * rr] * inv, o[i][2 * rr + 1] * inv);
+}
+
+// row rr of this thread's o fragments as an un-normalised partial (m, l, acc[128]) in the DEC_PART layout at dst
+__device__ __forceinline__ void attn_store_part(float* dst, const float (&o)[16][4], int rr, float m, float l) {
+  const int t = threadIdx.x & 3;
+  if (t == 0) *reinterpret_cast<float2*>(dst) = make_float2(m, l);
+#pragma unroll
+  for (int i = 0; i < 16; ++i)
+    *reinterpret_cast<float2*>(dst + 2 + 8 * i + 2 * t) = make_float2(o[i][2 * rr], o[i][2 * rr + 1]);
+}
+
 // q f16 [T, H*128] (pre-RoPE, the q projection's output); kf, vf f16 [T, Hkv*128] from kv_dequant_rope_kernel (H % Hkv == 0);
 // indptr i32 [B+1]: prompt b owns tokens [indptr[b], indptr[b+1]); out f16 [T, H*128]
 // kCtx = false: grid (q tiles, B, H); every prompt is a whole sequence (positions 0 .. L - 1).
@@ -145,13 +269,13 @@ __device__ __forceinline__ void prefill_ctx_tile(int, int, int, int, const float
 // causal tiles: every context key precedes every query, so these tiles need no causal mask, only the first (partial) one a length
 // mask, and the online-softmax state carries on into the prompt's tiles unchanged.  q is rotated at ctx_b + r.
 // Every term of the context path sits behind `if constexpr` or a condition on the constant kCtx, and the cache is a trailing
-// parameter pack (empty for <false>): prefill_attn_kernel<false> compiles to the SASS of the kernel before the context path.
+// parameter pack (empty for <false>): <false> carries none of it.
 // <true> asks for two CTAs per SM: at the three CTAs ptxas otherwise aims for (168 registers) its context producer spills.
 template <bool kCtx, typename... Cache>
 __global__ void __launch_bounds__(PF_THREADS, kCtx ? 2 : 0)
 prefill_attn_kernel(const __half* __restrict__ q, const __half* __restrict__ kf, const __half* __restrict__ vf,
                     const int32_t* __restrict__ indptr, const float2* __restrict__ rope, __half* __restrict__ out, int H,
-                    int Hkv, float scale_log2, Cache... cache) {
+                    int Hkv, Cache... cache) {
   static_assert(sizeof...(Cache) == (kCtx ? 1 : 0), "prefill_attn_kernel<true> takes the cache (one KvArgs), <false> nothing");
   __shared__ __align__(16) __half Ks[PF_BK * PF_KPITCH];
   __shared__ __align__(16) __half Vt[128 * PF_VPITCH];
@@ -169,8 +293,9 @@ prefill_attn_kernel(const __half* __restrict__ q, const __half* __restrict__ kf,
   const size_t row_pitch = (size_t)H * 128;
   const size_t kv_pitch = (size_t)Hkv * 128;          // grouped-query attention: query head h reads KV head h / (H / Hkv)
   const int hk = h / (H / Hkv);
+  const int ctx = prefill_ctx_len(cache..., b, L);
 
-  if constexpr (kCtx) rope += (size_t)prefill_ctx_len(cache..., b, L) * 64;     // row p of the table = position ctx + p
+  if constexpr (kCtx) rope += (size_t)ctx * 64;       // row p of the table = position ctx + p
   // ---- Q fragments of this warp's 16 rows, rotated (FP32 math, rounded to FP16 like `rotary_pos_emb(...).to(q.dtype)`)
   uint32_t qa[8][4];
   {
@@ -204,7 +329,7 @@ prefill_attn_kernel(const __half* __restrict__ q, const __half* __restrict__ kf,
   float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
   const int qrow0 = q0 + warp * 16 + g, qrow1 = qrow0 + 8;
 
-  for (int kt = kCtx ? -((prefill_ctx_len(cache..., b, L) + PF_BK - 1) / PF_BK) : 0; kt <= qt; ++kt) {
+  for (int kt = kCtx ? -((ctx + PF_BK - 1) / PF_BK) : 0; kt <= qt; ++kt) {
     const int k0 = kt * PF_BK;
     __syncthreads();                                  // the previous tile has been consumed
     if (kCtx && kt < 0) {
@@ -228,84 +353,16 @@ prefill_attn_kernel(const __half* __restrict__ q, const __half* __restrict__ kf,
     }
     }
     __syncthreads();
-
-    // ---- S = Q K^T (16 x 64 per warp), FP32
-    float s[8][4];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
-#pragma unroll
-      for (int kk = 0; kk < 8; ++kk) {
-        const uint32_t b0 = *reinterpret_cast<const uint32_t*>(&Ks[(8 * j + g) * PF_KPITCH + 16 * kk + 2 * t]);
-        const uint32_t b1 = *reinterpret_cast<const uint32_t*>(&Ks[(8 * j + g) * PF_KPITCH + 16 * kk + 8 + 2 * t]);
-        mma_16816(s[j], qa[kk], b0, b1);
-      }
-    }
-    if constexpr (kCtx) {                             // the first context tile's slots before the context: no key
-      const int lim = -prefill_ctx_len(cache..., b, L);
-      if (k0 < lim) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-#pragma unroll
-          for (int u = 0; u < 2; ++u)
-            if (k0 + 8 * j + 2 * t + u < lim) s[j][u] = s[j][2 + u] = -INFINITY;
-        }
-      }
-    }
-    // ---- scale, causal / length mask, online softmax (rows qrow0 and qrow1 of this thread)
-    float mx0 = -INFINITY, mx1 = -INFINITY;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-#pragma unroll
-      for (int u = 0; u < 2; ++u) {
-        const int kpos = k0 + 8 * j + 2 * t + u;
-        const bool ok0 = kpos <= qrow0 && kpos < L, ok1 = kpos <= qrow1 && kpos < L;
-        s[j][u] = ok0 ? s[j][u] * scale_log2 : -INFINITY;
-        s[j][2 + u] = ok1 ? s[j][2 + u] * scale_log2 : -INFINITY;
-        mx0 = fmaxf(mx0, s[j][u]); mx1 = fmaxf(mx1, s[j][2 + u]);
-      }
-    }
-    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1)); mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
-    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1)); mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
-    const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);
-    // rows past the prompt end have every key masked in their first tiles: keep exp2(-inf - -inf) out of the recurrence
-    const float base0 = mn0 == -INFINITY ? 0.f : mn0, base1 = mn1 == -INFINITY ? 0.f : mn1;
-    const float a0 = exp2f(m0 - base0), a1 = exp2f(m1 - base1);
-    m0 = mn0; m1 = mn1;
-    float sum0 = 0.f, sum1 = 0.f;
-    uint32_t pa[4][4];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float p00 = exp2f(s[j][0] - base0), p01 = exp2f(s[j][1] - base0);
-      const float p10 = exp2f(s[j][2] - base1), p11 = exp2f(s[j][3] - base1);
-      sum0 += p00 + p01; sum1 += p10 + p11;
-      pa[j >> 1][(j & 1) * 2 + 0] = pack_h2(p00, p01);
-      pa[j >> 1][(j & 1) * 2 + 1] = pack_h2(p10, p11);
-    }
-    l0 = l0 * a0 + sum0; l1 = l1 * a1 + sum1;
-#pragma unroll
-    for (int i = 0; i < 16; ++i) { o[i][0] *= a0; o[i][1] *= a0; o[i][2] *= a1; o[i][3] *= a1; }
-    // ---- O += P V
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {
-        const uint32_t b0 = *reinterpret_cast<const uint32_t*>(&Vt[(8 * i + g) * PF_VPITCH + 16 * kk + 2 * t]);
-        const uint32_t b1 = *reinterpret_cast<const uint32_t*>(&Vt[(8 * i + g) * PF_VPITCH + 16 * kk + 8 + 2 * t]);
-        mma_16816(o[i], pa[kk], b0, b1);
-      }
-    }
+    // causal and prompt-length mask; <true>: the first context tile's slots before the context hold no key.  Rows past the
+    // prompt end have every key masked in their first tiles.
+    attn_tile_step(qa, Ks, Vt, k0, [&](int rr, int kpos) { return (!kCtx || kpos >= -ctx) && kpos <= (rr ? qrow1 : qrow0) && kpos < L; },
+                   o, m0, m1, l0, l1);
   }
 
   // ---- normalise and store
-  l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
-  l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
-  const float i0 = 1.f / l0, i1 = 1.f / l1;
-#pragma unroll
-  for (int i = 0; i < 16; ++i) {
-    if (qrow0 < L) *reinterpret_cast<uint32_t*>(out + (size_t)(t0 + qrow0) * row_pitch + h * 128 + 8 * i + 2 * t) = pack_h2(o[i][0] * i0, o[i][1] * i0);
-    if (qrow1 < L) *reinterpret_cast<uint32_t*>(out + (size_t)(t0 + qrow1) * row_pitch + h * 128 + 8 * i + 2 * t) = pack_h2(o[i][2] * i1, o[i][3] * i1);
-  }
+  l0 = quad_sum(l0); l1 = quad_sum(l1);
+  if (qrow0 < L) attn_store_row(out + (size_t)(t0 + qrow0) * row_pitch + h * 128, o, 0, l0);
+  if (qrow1 < L) attn_store_row(out + (size_t)(t0 + qrow1) * row_pitch + h * 128, o, 1, l1);
 }
 
 }  // namespace atom

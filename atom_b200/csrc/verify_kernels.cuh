@@ -6,10 +6,11 @@
 //   * grid (chunk, KV head, sequence).  The S x G query rows of one (sequence, KV head) -- row r = (token r / G, query head
 //     hkv*G + r % G) -- fit one 64-row m16n8k16 tile, so a CTA streams its chunk of the sequence's pages ONCE for all of them:
 //     64-token tiles dequantised, and K rotated at its absolute positions from the (cos, sin) table, by prefill_attn_kernel<true>'s
-//     context loader (prefill_ctx_tile), as the cascade's prefix pass does; FP32 online softmax with a per-row causal limit.
+//     context loader (prefill_ctx_tile), as the cascade's prefix pass does; the tile step (attn_tile_step) with a per-row causal
+//     limit.
 //     Warps whose 16 rows are all padding (S x G <= 48) load their share of the tile and skip the MMAs.
-//   * q is rotated in FP32 at its own position, read from the page table on the device, as the cascade rotates it: a captured
-//     graph replays the launch with new lengths.  The table covers a bound the caller states.
+//   * q is rotated at its own position, read from the page table on the device, as the cascade rotates it (rope_q_frags): a
+//     captured graph replays the launch with new lengths.  K's table covers a bound the caller states.
 //   * split-KV: the sequence's ceil(len / 64) tiles are cut into nchunks runs of ceil(tiles / nchunks) consecutive tiles (the last
 //     runs may be empty).  With nchunks > 1 each CTA leaves the un-normalised (m, d, acc[128]) of its rows in the FP32 workspace
 //     (the DEC_PART layout, [B*S][Hq][nchunks]) and verify_merge_kernel combines them in chunk order.  The tiling depends on the
@@ -37,7 +38,7 @@ verify_attn_kernel(__half* __restrict__ o, const __half* __restrict__ q, KvArgs 
   if (pdl) { griddep_launch_dependents(); griddep_wait(); }       // q and the tail's K/V come from the preceding kernels
   const int chunk = blockIdx.x, hkv = blockIdx.y, b = blockIdx.z;
   const int len = verify_len(kv, b);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
+  const int tid = threadIdx.x, warp = tid >> 5, g = (tid & 31) >> 2;
   const int Hq = kv.H * G, rows = S * G;
   if (len < S) {             // a page table whose sequence is shorter than its query tokens: zeros, no page is read
     if (chunk == 0 && nchunks == 1)
@@ -49,46 +50,21 @@ verify_attn_kernel(__half* __restrict__ o, const __half* __restrict__ q, KvArgs 
   const int t_begin = chunk * per, t_end = min(tiles, t_begin + per);
   if (t_begin >= t_end) return;
   const bool busy = warp * 16 < rows;                              // warp-uniform: some of this warp's rows are live
-  const float kFreqStep = log2_theta / 64.f;
-  constexpr float kSmScale = 0.08838834764831845f * 1.4426950408889634f;   // 1/sqrt(128) * log2(e), as the decode kernel
 
-  // ---- Q fragments of this warp's 16 rows, rotated in FP32 at len - S + token and rounded to FP16 once; padded rows repeat the
-  // last live row and are never stored
+  // ---- Q fragments of this warp's 16 rows, rotated at len - S + token; padded rows repeat the last live row and are never stored
   const int qrow0 = warp * 16 + g, qrow1 = qrow0 + 8;
   int lim[2], hrow[2], trow[2];
   uint32_t qa[8][4];
   {
-    float2 lo[2][4][2], hi[2][4][2];
+    const __half* qr[2];
 #pragma unroll
     for (int rr = 0; rr < 2; ++rr) {
       const int r = min(rr ? qrow1 : qrow0, rows - 1);
       trow[rr] = r / G; hrow[rr] = hkv * G + r % G;
       lim[rr] = len - S + trow[rr];                                // the row's position: keys at positions <= lim are visible
-      const __half* qr = q + (((size_t)b * S + trow[rr]) * Hq + hrow[rr]) * 128;
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {
-#pragma unroll
-        for (int hf = 0; hf < 2; ++hf) {          // columns d = 16 kk + 8 hf + 2 t, d + 1 and their partners d + 64
-          const int d = 16 * kk + 8 * hf + 2 * t;
-          const float2 x = __half22float2(*reinterpret_cast<const __half2*>(qr + d));
-          const float2 y = __half22float2(*reinterpret_cast<const __half2*>(qr + d + 64));
-          float s0, c0, s1, c1;
-          sincosf((float)lim[rr] * exp2f(-(float)d * kFreqStep), &s0, &c0);
-          sincosf((float)lim[rr] * exp2f(-(float)(d + 1) * kFreqStep), &s1, &c1);
-          lo[rr][kk][hf] = make_float2(x.x * c0 - y.x * s0, x.y * c1 - y.y * s1);
-          hi[rr][kk][hf] = make_float2(y.x * c0 + x.x * s0, y.y * c1 + x.y * s1);
-        }
-      }
+      qr[rr] = q + (((size_t)b * S + trow[rr]) * Hq + hrow[rr]) * 128;
     }
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk)
-#pragma unroll
-      for (int hf = 0; hf < 2; ++hf)
-#pragma unroll
-        for (int rr = 0; rr < 2; ++rr) {
-          qa[kk][2 * hf + rr] = pack_h2(lo[rr][kk][hf].x, lo[rr][kk][hf].y);
-          qa[kk + 4][2 * hf + rr] = pack_h2(hi[rr][kk][hf].x, hi[rr][kk][hf].y);
-        }
+    rope_q_frags(qa, qr, lim, log2_theta);
   }
 
   // the context loader of prefill_attn_kernel<true> with the whole sequence as the "context" of an empty prompt: key position
@@ -106,81 +82,18 @@ verify_attn_kernel(__half* __restrict__ o, const __half* __restrict__ q, KvArgs 
     prefill_ctx_tile(kv, b, 0, hkv, a0 - len, rope_ctx, Ks, Vt, tid);
     __syncthreads();
     if (!busy) continue;
-
-    float s[8][4];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
-#pragma unroll
-      for (int kk = 0; kk < 8; ++kk) {
-        const uint32_t b0f = *reinterpret_cast<const uint32_t*>(&Ks[(8 * j + g) * PF_KPITCH + 16 * kk + 2 * t]);
-        const uint32_t b1f = *reinterpret_cast<const uint32_t*>(&Ks[(8 * j + g) * PF_KPITCH + 16 * kk + 8 + 2 * t]);
-        mma_16816(s[j], qa[kk], b0f, b1f);
-      }
-    }
-    // scale and causal limit (keys past len are past every row's limit)
-    float mx0 = -INFINITY, mx1 = -INFINITY;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-#pragma unroll
-      for (int u = 0; u < 2; ++u) {
-        const int kpos = a0 + 8 * j + 2 * t + u;
-        s[j][u] = kpos <= lim[0] ? s[j][u] * kSmScale : -INFINITY;
-        s[j][2 + u] = kpos <= lim[1] ? s[j][2 + u] * kSmScale : -INFINITY;
-        mx0 = fmaxf(mx0, s[j][u]); mx1 = fmaxf(mx1, s[j][2 + u]);
-      }
-    }
-    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1)); mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
-    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1)); mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
-    const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);
-    // a chunk that starts inside the tail can hold no key for its first rows: keep exp2(-inf - -inf) out of the recurrence
-    const float base0 = mn0 == -INFINITY ? 0.f : mn0, base1 = mn1 == -INFINITY ? 0.f : mn1;
-    const float a_0 = exp2f(m0 - base0), a_1 = exp2f(m1 - base1);
-    m0 = mn0; m1 = mn1;
-    float sum0 = 0.f, sum1 = 0.f;
-    uint32_t pa[4][4];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float p00 = exp2f(s[j][0] - base0), p01 = exp2f(s[j][1] - base0);
-      const float p10 = exp2f(s[j][2] - base1), p11 = exp2f(s[j][3] - base1);
-      sum0 += p00 + p01; sum1 += p10 + p11;
-      pa[j >> 1][(j & 1) * 2 + 0] = pack_h2(p00, p01);
-      pa[j >> 1][(j & 1) * 2 + 1] = pack_h2(p10, p11);
-    }
-    l0 = l0 * a_0 + sum0; l1 = l1 * a_1 + sum1;
-#pragma unroll
-    for (int i = 0; i < 16; ++i) { acc[i][0] *= a_0; acc[i][1] *= a_0; acc[i][2] *= a_1; acc[i][3] *= a_1; }
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {
-        const uint32_t b0f = *reinterpret_cast<const uint32_t*>(&Vt[(8 * i + g) * PF_VPITCH + 16 * kk + 2 * t]);
-        const uint32_t b1f = *reinterpret_cast<const uint32_t*>(&Vt[(8 * i + g) * PF_VPITCH + 16 * kk + 8 + 2 * t]);
-        mma_16816(acc[i], pa[kk], b0f, b1f);
-      }
-    }
+    // causal limit (keys past len are past every row's limit); a chunk that starts inside the tail can hold no key for its first rows
+    attn_tile_step(qa, Ks, Vt, a0, [&](int rr, int kpos) { return kpos <= lim[rr]; }, acc, m0, m1, l0, l1);
   }
   if (!busy) return;
 
-  l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
-  l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  l0 = quad_sum(l0); l1 = quad_sum(l1);
 #pragma unroll
   for (int rr = 0; rr < 2; ++rr) {
     if ((rr ? qrow1 : qrow0) >= rows) continue;
     const size_t row = ((size_t)b * S + trow[rr]) * Hq + hrow[rr];
-    const float m = rr ? m1 : m0, l = rr ? l1 : l0;
-    if (nchunks == 1) {                               // the whole sequence: normalise and store
-      const float inv = 1.f / l;
-#pragma unroll
-      for (int i = 0; i < 16; ++i)
-        *reinterpret_cast<uint32_t*>(o + row * 128 + 8 * i + 2 * t) = pack_h2(acc[i][2 * rr] * inv, acc[i][2 * rr + 1] * inv);
-    } else {                                          // un-normalised partial (m, d, acc[128]) of this chunk
-      float* dst = part + (row * nchunks + chunk) * DEC_PART;
-      if (t == 0) *reinterpret_cast<float2*>(dst) = make_float2(m, l);
-#pragma unroll
-      for (int i = 0; i < 16; ++i)
-        *reinterpret_cast<float2*>(dst + 2 + 8 * i + 2 * t) = make_float2(acc[i][2 * rr], acc[i][2 * rr + 1]);
-    }
+    if (nchunks == 1) attn_store_row(o + row * 128, acc, rr, rr ? l1 : l0);                  // the whole sequence
+    else attn_store_part(part + (row * nchunks + chunk) * DEC_PART, acc, rr, rr ? m1 : m0, rr ? l1 : l0);   // this chunk's partial
   }
 }
 
