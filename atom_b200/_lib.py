@@ -55,6 +55,8 @@ _SIGNATURES = {
     "atom_sample_slot_init": (_I, [_P, _I64, _I, _I, _P, _I, _P]),
     "atom_sample_draft_f16": (_I, [_P, _I64, _I, _I] + [_P] * 8 + [_I, _P, _P, _P, _P]),
     "atom_spec_commit_propose": (_I, [_P] * 4 + [_I, _P, _P] + [_I] * 5 + [_P, _P]),
+    "atom_beam_select_f16": (_I, [_P, _I64, _I, _I, _P, _I, _P, _P, _I, _I] + [_P] * 6),
+    "atom_kv_copy_pages_i4": (_I, [_P, _P] + [_I] * 4 + [_P] * 3 + [_I, _P]),
 }
 
 _lib = None

@@ -30,6 +30,7 @@
 #include "moe_kernels.cuh"
 #include "sample_kernels.cuh"
 #include "spec_kernels.cuh"
+#include "beam_kernels.cuh"
 
 namespace {
 
@@ -1177,6 +1178,76 @@ int atom_sample_slot_init(void* table, int64_t table_ld, int vocab, int slot, co
   return launch_k("sample_slot_init", atom::sample_slot_init_kernel, dim3((unsigned)((table_ld + chunk - 1) / chunk)),
                   dim3(atom::SAMPLE_INIT_THREADS), 0, (cudaStream_t)stream, (uint16_t*)table + (long long)slot * table_ld,
                   (long long)table_ld, vocab, (const int32_t*)prompt, prompt_len);
+}
+
+int atom_beam_select_f16(const void* logits, int64_t ld, int rows, int vocab, const void* row_indptr, int batch, const void* sums,
+                         const int* stop_ids, int num_stop, int width, void* workspace, void* live, void* live_key, void* fin,
+                         void* fin_key, void* stream) {
+  ATOM_REQUIRE((rows == 0 || (logits && sums)) && row_indptr && workspace && live && live_key && fin && fin_key,
+               "beam_select_f16: null pointer argument");
+  ATOM_REQUIRE(rows >= 0 && batch > 0 && vocab > 0 && vocab <= atom::SAMPLE_MAX_CLUSTER * atom::SAMPLE_SLICE_MAX,
+               "beam_select_f16: rows=%d >= 0, batch=%d > 0 and vocab=%d in [1, %d]", rows, batch, vocab,
+               atom::SAMPLE_MAX_CLUSTER * atom::SAMPLE_SLICE_MAX);
+  ATOM_REQUIRE(ld >= vocab || rows <= 1, "beam_select_f16: ld=%lld must be >= vocab=%d", (long long)ld, vocab);
+  ATOM_REQUIRE(width >= 1 && width <= atom::BEAM_MAX_WIDTH, "beam_select_f16: width=%d must be in [1, %d]", width, atom::BEAM_MAX_WIDTH);
+  ATOM_REQUIRE(num_stop >= 0 && num_stop <= atom::BEAM_MAX_STOP && (num_stop == 0 || stop_ids) && vocab > num_stop,
+               "beam_select_f16: num_stop=%d must be in [0, %d] and below vocab=%d", num_stop, atom::BEAM_MAX_STOP, vocab);
+  ATOM_REQUIRE((long long)rows * atom::SAMPLE_MAX_CLUSTER < (1ll << 31), "beam_select_f16: rows=%d too large", rows);
+  ATOM_REQUIRE((reinterpret_cast<uintptr_t>(logits) & 1) == 0 && aligned16(workspace) && aligned4(row_indptr) && aligned4(sums) &&
+               aligned4(live) && aligned4(live_key) && aligned4(fin) && aligned4(fin_key),
+               "beam_select_f16: misaligned pointer (logits 2, workspace 16, the rest 4 bytes)");
+  atom::BeamArgs a{};
+  a.logits = (const __half*)logits; a.ld = (long long)ld; a.V = vocab; a.slice = atom::sample_slice(vocab); a.W = width;
+  a.nstop = num_stop;
+  for (int j = 0; j < num_stop; ++j) {
+    ATOM_REQUIRE(stop_ids[j] >= 0 && stop_ids[j] < vocab, "beam_select_f16: stop id %d outside [0, %d)", stop_ids[j], vocab);
+    for (int q = 0; q < j; ++q) ATOM_REQUIRE(stop_ids[q] != stop_ids[j], "beam_select_f16: stop id %d given twice", stop_ids[j]);
+    a.stop[j] = stop_ids[j];
+  }
+  a.row_indptr = (const int32_t*)row_indptr; a.sums = (const float*)sums; a.R = rows;
+  a.code = (unsigned long long*)workspace;
+  a.lp = (float*)((unsigned long long*)workspace + (size_t)rows * atom::BEAM_LIST);
+  a.live = (int32_t*)live; a.live_key = (float*)live_key; a.fin = (int32_t*)fin; a.fin_key = (float*)fin_key;
+  const cudaStream_t st = (cudaStream_t)stream;
+  const int pdl = pdl_enabled() ? 1 : 0;
+  if (rows > 0) {
+    const int C = atom::sample_cluster(vocab);
+    int rc = ensure_dynamic_smem(atom::beam_row_kernel, (int)atom::beam_row_smem(atom::SAMPLE_SLICE_MAX), "beam_select_f16");
+    if (rc) return rc;
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3((unsigned)(C * rows)); cfg.blockDim = dim3(atom::SAMPLE_THREADS);
+    cfg.dynamicSmemBytes = atom::beam_row_smem(a.slice); cfg.stream = st;
+    cudaLaunchAttribute attr[2];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = C; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr; cfg.numAttrs = 1;
+    if (pdl) {
+      attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+      attr[1].val.programmaticStreamSerializationAllowed = 1;
+      cfg.numAttrs = 2;
+    }
+    cudaError_t e = cudaLaunchKernelEx(&cfg, atom::beam_row_kernel, a, pdl);
+    if (e != cudaSuccess) return fail(ATOM_E_CUDA, "beam_select_f16 launch (cluster %d): %s", C, cudaGetErrorString(e));
+    rc = check_launch("beam_select_f16");
+    if (rc) return rc;
+  }
+  return launch_k("beam_merge", atom::beam_merge_kernel, dim3(batch), dim3(atom::BEAM_MERGE_THREADS), 0, st, a);
+}
+
+int atom_kv_copy_pages_i4(void* kv_data, void* kv_param, int num_pages, int num_layers, int num_heads, int page_size, const void* src,
+                          const void* dst, const void* slots, int n, void* stream) {
+  ATOM_REQUIRE(kv_data && kv_param && src && dst && slots, "kv_copy_pages_i4: null pointer argument");
+  ATOM_REQUIRE(num_pages > 0 && num_layers > 0 && num_heads > 0 && page_size > 0 && n >= 0,
+               "kv_copy_pages_i4: num_pages=%d, num_layers=%d, num_heads=%d, page_size=%d must be positive and n=%d >= 0", num_pages,
+               num_layers, num_heads, page_size, n);
+  ATOM_REQUIRE(aligned16(kv_data) && aligned4(kv_param) && aligned4(src) && aligned4(dst) && aligned4(slots),
+               "kv_copy_pages_i4: misaligned pointer (kv_data 16, the rest 4 bytes)");
+  if (n == 0) return ATOM_OK;
+  const int blocks = num_layers * 2 * num_heads;
+  return launch_k("kv_copy_pages_i4", atom::kv_copy_pages_kernel,
+                  dim3((unsigned)((blocks + atom::KV_COPY_BLOCKS_PER_CTA - 1) / atom::KV_COPY_BLOCKS_PER_CTA), (unsigned)n),
+                  dim3(atom::KV_COPY_THREADS), 0, (cudaStream_t)stream, (uint8_t*)kv_data, (uint32_t*)kv_param, num_pages, blocks,
+                  page_size, (const int32_t*)src, (const int32_t*)dst, (const int32_t*)slots);
 }
 
 }  // extern "C"

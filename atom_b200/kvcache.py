@@ -153,10 +153,11 @@ class KvCacheInt4:
         self._seqlen = n
         return dropped
 
-    def fork(self, n=None) -> "KvCacheInt4":
+    def fork(self, n=None, copies=None) -> "KvCacheInt4":
         """A new sequence holding this one's first `n` tokens (default: all).  It shares the full pages among them; a partly
         filled last page is copied, every layer and K/V block, into a fresh page of its own (one device copy on the current
-        stream).  Both sequences then grow independently."""
+        stream).  Both sequences then grow independently.  copies: a list to defer that copy to, as (src page, dst page, slots),
+        e.g. for ops.copy_kv_pages; it must then run before either sequence writes another token."""
         n = self._seqlen if n is None else int(n)
         if not 0 <= n <= self._seqlen:
             raise ValueError(f"fork: n={n} outside [0, {self._seqlen}]")
@@ -169,8 +170,11 @@ class KvCacheInt4:
         if n % pool.block_len:
             page = pool.alloc_block()
             child._pages.append(page)
-            pool.buf[page].copy_(pool.buf[self._pages[full]])
-            pool.param[page].copy_(pool.param[self._pages[full]])
+            if copies is not None:
+                copies.append((self._pages[full], page, n % pool.block_len))
+            else:
+                pool.buf[page].copy_(pool.buf[self._pages[full]])
+                pool.param[page].copy_(pool.param[self._pages[full]])
         child._seqlen = n
         return child
 

@@ -940,3 +940,108 @@ def spec_commit_propose(tokens, cands, row_indptr, slots, history, lengths, out,
                                                        history.data_ptr(), lengths.data_ptr(), nslots, cap, k, nmin, nmax,
                                                        out.data_ptr(), _stream(history)), "spec_commit_propose")
     return out
+
+
+BEAM_MAX_WIDTH = 8
+BEAM_MAX_STOP = 8
+_BEAM_LIST = BEAM_MAX_WIDTH + BEAM_MAX_STOP
+
+
+def beam_out(batch, width, device):
+    """A packed output buffer for beam_select: int32 [6 * batch * width]."""
+    return torch.empty(6 * int(batch) * int(width), dtype=torch.int32, device=device)
+
+
+def split_beam_out(out, batch, width):
+    """The four views of a packed beam_select buffer (a CUDA tensor or a host array): live [B, W, 2], live_key [B, W] (float32),
+    fin [B, W, 2], fin_key [B, W] (float32)."""
+    n = int(batch) * int(width)
+    if isinstance(out, torch.Tensor):
+        f32 = lambda x: x.view(torch.float32)      # noqa: E731
+    else:
+        import numpy as np
+        f32 = lambda x: x.view(np.float32)         # noqa: E731
+    return (out[:2 * n].reshape(batch, width, 2), f32(out[2 * n:3 * n]).reshape(batch, width),
+            out[3 * n:5 * n].reshape(batch, width, 2), f32(out[5 * n:6 * n]).reshape(batch, width))
+
+
+def beam_select(logits, row_indptr, sums, width, stop_ids=(), *, out=None, workspace=None):
+    """EXTENSION (atom_beam_select_f16; DESIGN section 5.9): one beam-search step.  logits float16 [R, V] (unit stride along V),
+    row_indptr int32 [B + 1] (request i owns rows row_indptr[i] .. row_indptr[i+1]; zero rows pads), sums float32 [R] (each row's
+    beam's running sum), all on one CUDA device; width W in [1, 8]; stop_ids at most 8 host ids in [0, V).  Returns (live [B, W, 2]
+    of (row, token), live_key [B, W], fin [B, W, 2], fin_key [B, W]), padded with -1: each request's live beams and the stop
+    candidates of rank < W, in order (include/atom_b200.h).  out (beam_out) and workspace (uint8 >= R * 192 bytes, 16-byte
+    aligned) may be given, so that a CUDA graph captures no allocation; the four tensors are then views of out."""
+    w = int(width)
+    stops = [int(t) for t in stop_ids]
+    if not 1 <= w <= BEAM_MAX_WIDTH:
+        raise RuntimeError(f"atom_b200.ops.beam_select: width must be in [1, {BEAM_MAX_WIDTH}], got {width}")
+    _req_cuda(row_indptr, sums)
+    if not (isinstance(logits, torch.Tensor) and logits.is_cuda and logits.dtype == torch.float16 and logits.dim() == 2
+            and logits.stride(1) == 1):
+        raise RuntimeError("atom_b200.ops.beam_select: logits must be float16 [R, V] on a CUDA device with unit stride along V")
+    r, v = logits.shape
+    b = row_indptr.numel() - 1
+    dev = logits.device
+    if row_indptr.dtype != torch.int32 or row_indptr.dim() != 1 or b < 1 or row_indptr.device != dev:
+        raise RuntimeError(f"atom_b200.ops.beam_select: row_indptr must be int32 [B + 1] with B >= 1 on {dev}")
+    if sums.dtype != torch.float32 or tuple(sums.shape) != (r,) or sums.device != dev:
+        raise RuntimeError(f"atom_b200.ops.beam_select: sums must be float32 [{r}] on {dev}")
+    if len(stops) > BEAM_MAX_STOP or len(set(stops)) != len(stops) or any(not 0 <= t < v for t in stops) or len(stops) >= v:
+        raise RuntimeError(f"atom_b200.ops.beam_select: stop_ids must be at most {BEAM_MAX_STOP} distinct ids in [0, {v}), fewer "
+                           f"than the vocabulary, got {stop_ids!r}")
+    if out is None:
+        out = beam_out(b, w, dev)
+    elif out.dtype != torch.int32 or out.numel() != 6 * b * w or not out.is_contiguous() or out.device != dev:
+        raise RuntimeError(f"atom_b200.ops.beam_select: out must be contiguous int32 [{6 * b * w}] on {dev}")
+    if workspace is None:
+        workspace = torch.empty(max(1, r) * _BEAM_LIST * 12, dtype=torch.uint8, device=dev)
+    elif workspace.numel() * workspace.element_size() < r * _BEAM_LIST * 12 or not workspace.is_contiguous() or workspace.device != dev:
+        raise RuntimeError(f"atom_b200.ops.beam_select: workspace must hold {r * _BEAM_LIST * 12} contiguous bytes on {dev}")
+    live, live_key, fin, fin_key = split_beam_out(out, b, w)
+    import ctypes
+    arr = (ctypes.c_int * max(1, len(stops)))(*stops)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().atom_beam_select_f16(logits.data_ptr(), logits.stride(0) if r > 1 else v, r, v, row_indptr.data_ptr(), b,
+                                                   sums.data_ptr(), arr, len(stops), w, workspace.data_ptr(), live.data_ptr(),
+                                                   live_key.data_ptr(), fin.data_ptr(), fin_key.data_ptr(), _stream(logits)),
+                   "beam_select")
+    return live, live_key, fin, fin_key
+
+
+def copy_kv_pages(pool, src, dst, slots):
+    """EXTENSION (atom_kv_copy_pages_i4; DESIGN section 5.9): in one launch, copy the first slots[p] token slots of page src[p] to
+    page dst[p] in every layer, K/V and head block of pool.buf and pool.param (a kvcache.KvPoolInt4, or anything with those two
+    tensors).  src, dst, slots: int32 CUDA tensors [n] (read on the device, so a CUDA graph replays with new pairs; src < 0 is
+    padding), or host sequences, which are checked: src != dst, pages in range, slots in [1, page size]."""
+    buf, param = pool.buf, pool.param
+    _req_cuda(buf, param)
+    pages, layers, two, heads, P, half = buf.shape
+    if buf.dtype != torch.uint8 or half != 64 or two != 2 or tuple(param.shape) != (pages, layers, 2, heads, P, 2) or \
+            param.dtype != torch.float16:
+        raise RuntimeError("atom_b200.ops.copy_kv_pages: pool.buf must be uint8 [pages, L, 2, H, P, 64] and pool.param float16 "
+                           "[pages, L, 2, H, P, 2]")
+    dev = buf.device
+    pairs = []
+    for name, x in (("src", src), ("dst", dst), ("slots", slots)):
+        if isinstance(x, torch.Tensor):
+            _req_cuda(x)
+            if x.dtype != torch.int32 or x.dim() != 1 or x.device != dev:
+                raise RuntimeError(f"atom_b200.ops.copy_kv_pages: `{name}` must be int32 [n] on {dev}")
+            pairs.append(x)
+        else:
+            pairs.append(list(x))
+    n = len(pairs[0])
+    if any(len(x) != n for x in pairs):
+        raise RuntimeError("atom_b200.ops.copy_kv_pages: src, dst and slots must have one entry per pair")
+    if not isinstance(pairs[0], torch.Tensor) and not any(isinstance(x, torch.Tensor) for x in pairs):
+        for s, d, k in zip(*pairs):
+            if s >= 0 and (s == d or not 0 <= d < pages or s >= pages or not 1 <= k <= P):
+                raise RuntimeError(f"atom_b200.ops.copy_kv_pages: pair ({s}, {d}, {k}) needs src != dst, pages in [0, {pages}) "
+                                   f"and slots in [1, {P}]")
+    if n == 0:
+        return
+    pairs = [x if isinstance(x, torch.Tensor) else torch.tensor(x, dtype=torch.int32).to(dev) for x in pairs]
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().atom_kv_copy_pages_i4(buf.data_ptr(), param.data_ptr(), pages, layers, heads, P, pairs[0].data_ptr(),
+                                                    pairs[1].data_ptr(), pairs[2].data_ptr(), n, _stream(buf)), "copy_kv_pages")

@@ -152,6 +152,21 @@ class SpeculativeParams:
             raise ValueError(f"need 1 <= num_draft <= 7 and 1 <= ngram_min <= ngram_max <= 16: {self}")
 
 
+@dataclasses.dataclass(frozen=True)
+class BeamSearchParams:
+    """Beam search (DESIGN section 5.9): every request keeps up to `width` live beams, ranked by the FP32 sum of their tokens'
+    log-probabilities (ops.beam_select), and up to `width` finished hypotheses -- a beam that chose a stop id, or a live beam
+    that reached the output length -- scored sum / len^length_penalty in float64.  A request is done when it holds `width`
+    finished hypotheses or its beams reach the output length; its output is the best finished hypothesis.  width = 1 gives the
+    greedy tokens."""
+    width: int = 4
+    length_penalty: float = 0.0
+
+    def __post_init__(self):
+        if not (isinstance(self.width, (int, np.integer)) and 1 <= self.width <= 8) or not np.isfinite(self.length_penalty):
+            raise ValueError(f"need 1 <= width <= 8 and a finite length_penalty: {self}")
+
+
 @dataclasses.dataclass
 class TextGenConfig:
     batch_size: int
@@ -160,6 +175,7 @@ class TextGenConfig:
     sampling: Optional[SamplingParams] = None   # None: greedy (argmax)
     stop_token_ids: Tuple[int, ...] = ()        # a request that emits one of these finishes on it (greedy or sampled)
     speculate: Optional[SpeculativeParams] = None   # None: one token per running request and step
+    beam: Optional[BeamSearchParams] = None         # None: one sequence per request
 
 
 @dataclasses.dataclass
@@ -175,6 +191,8 @@ class TextGenBenchResult:
     logprobs: Optional[List[List[float]]] = None    # with SamplingParams.logprobs and keep_tokens: each token's log-probability
     top_logprobs: Optional[List[List[Tuple[List[int], List[float]]]]] = None    # ... and each token's top-n (ids, logprobs)
     speculative: Optional[dict] = None      # with speculation: TextGenScheduler.spec_stats
+    beam_scores: Optional[np.ndarray] = None    # with beam search: the score of each request's output
+    beam: Optional[dict] = None             # with beam search: TextGenScheduler.beam_stats
 
 
 @dataclasses.dataclass
@@ -189,6 +207,18 @@ class RequestContext:
     logprobs: List[float] = dataclasses.field(default_factory=list)
     top_logprobs: List[tuple] = dataclasses.field(default_factory=list)
     drafts: List[int] = dataclasses.field(default_factory=list)     # with speculation: the next step's drafts
+    beam_sum: float = 0.0                   # with beam search: this beam's FP32 sum of log-probabilities
+    group: Optional["_BeamGroup"] = None    # with beam search: the request this beam belongs to
+
+
+@dataclasses.dataclass(eq=False)
+class _BeamGroup:
+    """A beam-search request: its finished hypotheses (score, arrival, tokens) and timings; its live beams are in the workset."""
+    req_idx: int
+    encode_latency: float
+    decode_start_at: float
+    finished: list = dataclasses.field(default_factory=list)
+    arrivals: int = 0
 
 
 @dataclasses.dataclass(eq=False)
@@ -241,7 +271,7 @@ class TextGenScheduler:
 
     def __init__(self, rs: RequestSet, batch_size: int, pool: KvPoolInt4, device, vocab_size: int = 32000,
                  prefill_chunk: Optional[int] = None, shared_prefix: int = 0, stop_token_ids=(), penalty_slots: bool = False,
-                 num_draft: int = 0):
+                 num_draft: int = 0, beam: Optional[BeamSearchParams] = None):
         if prefill_chunk is not None and int(prefill_chunk) < 1:
             raise ValueError("prefill_chunk must be a positive number of tokens (or None)")
         if int(shared_prefix) < 0:
@@ -270,6 +300,9 @@ class TextGenScheduler:
         if self.num_draft and self._free_slots is None:
             raise ValueError("speculation needs slots (penalty_slots=True): they index the token histories")
         self.S = 1                                  # rows per running request in the admitted step
+        self.beam = beam
+        self.copies: List[tuple] = []               # beam search: the page copies of the last commit's forks, for the next step
+        self.beam_stats = {"page_copies": 0, "copied_slots": 0, "stop_finished": 0}
         self.spec_stats = {"verify_steps": 0, "drafted_tokens": 0, "accepted_tokens": 0, "emitted_tokens": 0,
                            "verify_sequence_steps": 0, "verify_emitted_tokens": 0}
 
@@ -286,6 +319,10 @@ class TextGenScheduler:
         # the prompt's pages plus one spare: the first generated token may open a new page.  Behind a shared prefix of N tokens
         # a fork takes the pages from N // P on: a copy of the partly filled page, if any, and the pages its prompt adds
         n, bl = self.shared_prefix, self.pool.block_len
+        if self.beam is not None:
+            # beam search: the first step forks the prompt into up to W beams, each of which can take one page (a copy of the
+            # partly filled page, or a fresh one for its next token)
+            return (n + prompt_len + bl - 1) // bl - n // bl + self.beam.width
         if self.num_draft:
             # speculating, the spare is room for the first token and for its first step as a running request, which can grow
             # the sequence by K + 1 more tokens
@@ -306,6 +343,8 @@ class TextGenScheduler:
         # running requests may each need a fresh page this step, and the requests being prefilled the pages of the rest of
         # their prompt: keep those in reserve before admitting anyone, so that no admitted request ever waits for a page
         reserve = len(self.workset) + sum(self._outstanding(p) for p in self._prefilling)
+        if self.beam is not None:                   # ... or, with beams, a page for each of up to W beams per running request
+            reserve += self.beam.width * len({id(r.group) for r in self.workset}) - len(self.workset)
         if self.num_draft:                          # ... or, speculating, pages for K + 1 more tokens
             bl = self.pool.block_len
             reserve += sum(-(-(r.kvcache.seqlen + self.num_draft + 1) // bl) - len(r.kvcache.indicies) - 1 for r in self.workset)
@@ -319,8 +358,7 @@ class TextGenScheduler:
             self._new.append((p, p.done, n))
             budget = None if budget is None else budget - n
         root_done = self._root is None or self._root.done == len(self._root.prompt)
-        while root_done and len(self.workset) + len(self._prefilling) < self.batch_size and self.next_req_idx < len(self.rs) and \
-                (budget is None or budget > 0):
+        while root_done and self._room() and self.next_req_idx < len(self.rs) and (budget is None or budget > 0):
             plen = int(self.rs.prompt_lens[self.next_req_idx])
             if self.pool.num_free_blocks - reserve < self._pages_needed(plen):
                 if not self.workset and not self._prefilling:
@@ -348,6 +386,13 @@ class TextGenScheduler:
             r.kvcache.acquire(self.S - 1)
         self._admitted = True
         return len(self._new)
+
+    def _room(self) -> bool:
+        """Whether the batch has room for one more request: a sequence, or with beam search W rows (sequences) from admission."""
+        if self.beam is None:
+            return len(self.workset) + len(self._prefilling) < self.batch_size
+        groups = len({id(r.group) for r in self.workset}) + sum(p.req_idx >= 0 for p in self._prefilling)
+        return (groups + 1) * self.beam.width <= self.batch_size
 
     def next_batch(self) -> StepBatch:
         """The step's model inputs: the prompt chunks (whole prompts without chunking), then the last token of every running
@@ -491,6 +536,115 @@ class TextGenScheduler:
         self.workset = new_workset
         return processed
 
+    # ---- beam search
+    def beam_rows(self) -> List[int]:
+        """Beam search: the rows of last_token_rows() of each request that takes a beam step, as an indptr: one row per prompt
+        this step completes, then the live beams of each running request (contiguous in the workset)."""
+        counts = [1] * len(self._first())
+        prev = None
+        for r in self.workset:
+            if r.group is prev:
+                counts[-1] += 1
+            else:
+                counts.append(1)
+                prev = r.group
+        return np.concatenate([[0], np.cumsum(counts, dtype=np.int64)]).astype(np.int32).tolist()
+
+    def beam_sums(self) -> List[float]:
+        """Beam search: the running sum of every row of last_token_rows() (0 for a prompt's row)."""
+        return [0.0] * len(self._first()) + [r.beam_sum for r in self.workset]
+
+    def take_copies(self) -> List[tuple]:
+        """Beam search: the (src page, dst page, slots) copies the next step must run before any K/V is written."""
+        out, self.copies = self.copies, []
+        return out
+
+    def _offer(self, g: _BeamGroup, tokens: List[int], s) -> None:
+        # the W best by score; a new hypothesis replaces the worst (the latest among equals) only if it is strictly better
+        h = (float(s) / float(len(tokens)) ** self.beam.length_penalty, g.arrivals, tokens)
+        g.arrivals += 1
+        if len(g.finished) < self.beam.width:
+            g.finished.append(h)
+            return
+        worst = min(range(len(g.finished)), key=lambda k: (g.finished[k][0], -g.finished[k][1]))
+        if h[0] > g.finished[worst][0]:
+            g.finished[worst] = h
+
+    def commit_beam(self, live, live_key, fin, fin_key, t1: float, t2: float) -> int:
+        """Beam search: ops.beam_select's result for the requests of beam_rows() (rows index last_token_rows()).  Offers the
+        finished candidates, makes the live ones the request's beams -- the first child of a parent inherits its sequence, any
+        further child is a fork whose partly filled page is copied by the next step (take_copies) -- and finishes the requests
+        that are done.  Returns the number of tokens this step processed."""
+        W = self.beam.width
+        live, fin = np.asarray(live), np.asarray(fin)
+        live_key, fin_key = np.asarray(live_key, np.float32), np.asarray(fin_key, np.float32)
+        processed = sum(n for _, _, n in self._new) + len(self.workset)
+        parents = []                                # per request: (group, its parent beams in row order)
+        for p, s, n in self._new:
+            p.done += n
+            if p.start_at is None:
+                p.start_at = t1
+            if s + n == len(p.prompt):
+                self._prefilling.remove(p)
+                if p.req_idx >= 0:
+                    g = _BeamGroup(p.req_idx, t2 - p.start_at, p.start_at)
+                    parents.append((g, [RequestContext(p.req_idx, p.kvcache, [], group=g)]))
+        for r in self.workset:
+            if parents and parents[-1][0] is r.group:
+                parents[-1][1].append(r)
+            else:
+                parents.append((r.group, [r]))
+        row0 = np.asarray(self.beam_rows()[:-1])
+        assert len(parents) == len(row0)
+        new_workset: List[RequestContext] = []
+        for i, (g, beams) in enumerate(parents):
+            for (row, t), k in zip(fin[i], fin_key[i]):
+                if row >= 0:
+                    self._offer(g, beams[row - row0[i]].output + [int(t)], k)
+            children = [(row - row0[i], int(t), np.float32(k)) for (row, t), k in zip(live[i], live_key[i]) if row >= 0]
+            if len(g.finished) >= W or not children or len(beams[0].output) + 1 >= int(self.rs.output_lens[g.req_idx]):
+                if len(g.finished) < W:
+                    for b, t, k in children:
+                        self._offer(g, beams[b].output + [t], k)
+                for b in beams:
+                    b.kvcache.release()
+                self._finish_group(g, t2)
+                continue
+            kept = {b for b, _, _ in children}
+            for b, beam in enumerate(beams):        # pages return before any are taken
+                if b not in kept:
+                    beam.kvcache.release()
+            inherited = set()
+            for b, t, k in children:
+                parent = beams[b]
+                if b in inherited:
+                    before = len(self.copies)
+                    kv = parent.kvcache.fork(copies=self.copies)
+                    for _, _, slots in self.copies[before:]:
+                        self.beam_stats["page_copies"] += 1
+                        self.beam_stats["copied_slots"] += slots
+                else:
+                    kv = parent.kvcache
+                    inherited.add(b)
+                child = RequestContext(g.req_idx, kv, parent.output + [t], beam_sum=k, group=g)
+                new_workset.append(child)
+            for child in new_workset[len(new_workset) - len(children):]:
+                child.kvcache.acquire_one()
+        self.workset, self._new, self._admitted = new_workset, [], False
+        return processed
+
+    def _finish_group(self, g: _BeamGroup, t2: float) -> None:
+        tokens, score = [], -np.inf
+        if g.finished:
+            score, _, tokens = max(g.finished, key=lambda h: (h[0], -h[1]))
+        if tokens and tokens[-1] in self.stop_token_ids:
+            self.beam_stats["stop_finished"] += 1
+        req = RequestContext(g.req_idx, None, tokens, encode_latency=g.encode_latency, decode_start_at=g.decode_start_at,
+                             decode_latency=t2 - g.decode_start_at, beam_sum=score)
+        self.done.append(req)
+        if self._root is not None and self.finished:
+            self._root.kvcache.release()
+
     @staticmethod
     def _keep_logprobs(req, logprobs, row):
         if logprobs is not None:
@@ -519,6 +673,9 @@ class TextGenScheduler:
         res = TextGenBenchResult(np.array([r.encode_latency for r in done]), np.array([r.decode_latency for r in done]),
                                  duration, steps, [r.output for r in done] if keep_tokens else None)
         res.output_lens = np.array([len(r.output) for r in done], dtype=np.int32)
+        if self.beam is not None:
+            res.beam_scores = np.array([r.beam_sum for r in done], dtype=np.float64)
+            res.beam = dict(self.beam_stats)
         if keep_tokens and any(r.logprobs for r in done):
             res.logprobs = [r.logprobs for r in done]
             res.top_logprobs = [r.top_logprobs for r in done]
@@ -568,11 +725,18 @@ class DecodeGraphRunner:
     H2D copy; a verify step (S > 1) passes BatchLenInfo(decode_len=S, max_len=max_pages * page size) and no groups.  The step
     returns the proposer's output [B, 2K + 3] (and, with logprobs, the sampler's per-row log-probabilities).
 
+    With `beam` (BeamSearchParams) the graphs are keyed on (B rows, prefix groups) and the buffer goes on after the page table
+    and groups with  [copy src(B) | copy dst(B) | copy slots(B) | row_indptr(B+1) | sums(B, FP32 bits)], one H2D copy; the
+    step is `copy_op` (ops.copy_kv_pages: the page copies of the previous commit's forks, padded with src = -1), the model, then
+    `beam_select_op` (ops.beam_select at the runner's width and stop ids) into one packed buffer, read back with one D2H copy.
+
     capture=False runs the same buffers through the model eagerly (the CPU tests use it; it is also the warm-up path)."""
 
     def __init__(self, model: Callable, pool: KvPoolInt4, device, max_pages_per_seq: int, capture: bool = True,
                  sampling: Optional[SamplingParams] = None, sample_op: Callable = None,
-                 speculate: Optional[SpeculativeParams] = None, propose_op: Callable = None, draft_sample_op: Callable = None):
+                 speculate: Optional[SpeculativeParams] = None, propose_op: Callable = None, draft_sample_op: Callable = None,
+                 beam: Optional[BeamSearchParams] = None, stop_token_ids=(), beam_select_op: Callable = None,
+                 copy_op: Callable = None):
         self.model, self.pool, self.device = model, pool, torch.device(device)
         self.max_pages, self.capture = max_pages_per_seq, capture
         self.sampling = sampling
@@ -591,6 +755,12 @@ class DecodeGraphRunner:
                 from . import ops
             self.propose_op = propose_op or ops.spec_commit_propose
             self.draft_sample_op = draft_sample_op or ops.sample_tokens
+        self.beam, self.stop_token_ids = beam, tuple(int(t) for t in stop_token_ids)
+        if beam is not None:
+            if beam_select_op is None or copy_op is None:
+                from . import ops
+            self.beam_select_op = beam_select_op or ops.beam_select
+            self.copy_op = copy_op or ops.copy_kv_pages
 
     def use_history(self, history):
         """The (token histories, lengths) the speculative step commits to and proposes from; graphs captured with others are
@@ -829,6 +999,71 @@ class DecodeGraphRunner:
         return self._launch(e, self._spec_step)
 
 
+    # ---- beam steps
+    def _beam_layout(self, b, ng):
+        o = self._layout(b, ng)[-1]
+        return {"src": o, "dst": o + b, "slots": o + 2 * b, "rip": o + 3 * b, "sums": o + 4 * b + 1, "total": o + 5 * b + 1}
+
+    def _beam_entry(self, b, ng):
+        e = self._entries.get(("beam", b, ng))
+        if e is None:
+            o_ids, o_indptr, o_last, o_ind, o_grp, _ = self._layout(b, ng)
+            o = self._beam_layout(b, ng)
+            host = torch.zeros(o["total"], dtype=torch.int32)
+            if self.device.type == "cuda":
+                host = host.pin_memory()
+            dev = torch.zeros(o["total"], dtype=torch.int32, device=self.device)
+            kv = _StaticKv(self.pool, dev[o_indptr:o_indptr + b + 1], dev[o_ind:o_ind + b * self.max_pages], dev[o_last:o_last + b])
+            if ng:
+                kv.group_indptr = dev[o_grp:o_grp + ng + 1]
+                kv.group_members = dev[o_grp + ng + 1:o_grp + ng + 1 + b]
+                kv.shared_pages = dev[o_grp + ng + 1 + b:o_grp + ng + 1 + 2 * b]
+                kv.group_bounds = (b, self.max_pages)
+            W = self.beam.width
+            e = {"host": host, "dev": dev, "ids": dev[o_ids:o_ids + b], "kv": kv, "blen": BatchLenInfo([], b, self.device),
+                 "graph": None, "out": None, "copy": tuple(dev[o[k]:o[k] + b] for k in ("src", "dst", "slots")),
+                 "rip": dev[o["rip"]:o["rip"] + b + 1], "sums": dev[o["sums"]:o["sums"] + b].view(torch.float32),
+                 "bout": torch.zeros(6 * b * W, dtype=torch.int32, device=self.device),
+                 "ws": torch.zeros(b * 16 * 12, dtype=torch.uint8, device=self.device)}
+            self._entries[("beam", b, ng)] = e
+        return e
+
+    def _beam_step(self, e):
+        self.copy_op(self.pool, *e["copy"])
+        logits, _ = self.model(e["ids"], e["blen"], None, e["kv"])
+        self.beam_select_op(logits, e["rip"], e["sums"], self.beam.width, self.stop_token_ids, out=e["bout"], workspace=e["ws"])
+        return e["bout"]
+
+    def run_beam(self, last_tokens: List[int], kvs: List[KvCacheInt4], copies: List[tuple], row_indptr: List[int],
+                 sums: List[float]):
+        """A beam step over B rows (TextGenScheduler: take_copies, beam_rows, beam_sums).  Returns (live, live_key, fin, fin_key)
+        of the requests of row_indptr, as numpy arrays."""
+        b = len(kvs)
+        groups = prefix_groups(kvs)
+        ng = len(groups)
+        if len(copies) > b:
+            raise RuntimeError(f"{len(copies)} page copies for a step of {b} rows")
+        for src, dst, slots in copies:                  # the kernel skips such pairs: a scheduler fault must not pass silently
+            if src == dst or not (0 <= src < self.pool.capacity and 0 <= dst < self.pool.capacity and 1 <= slots <= self.pool.block_len):
+                raise RuntimeError(f"page copy ({src}, {dst}, {slots}) needs src != dst, pages in range and slots in [1, page size]")
+        e = self._beam_entry(b, ng)
+        o_ids, o_indptr, o_last, o_ind, o_grp, _ = self._layout(b, ng)
+        o = self._beam_layout(b, ng)
+        h = e["host"].numpy()
+        h[o_ids:o_ids + b] = last_tokens
+        self._fill_pages(h, kvs, o_indptr, o_last, o_ind)
+        self._fill_groups(h, e, groups, b, o_grp)
+        n = len(copies)
+        for k, name in enumerate(("src", "dst", "slots")):
+            h[o[name]:o[name] + b] = [c[k] for c in copies] + [-1] * (b - n)
+        nreq = len(row_indptr) - 1
+        h[o["rip"]:o["rip"] + b + 1] = list(row_indptr) + [row_indptr[-1]] * (b - nreq)
+        h[o["sums"]:o["sums"] + b] = np.asarray(sums, np.float32).view(np.int32)
+        out = self._launch(e, self._beam_step)
+        from .ops import split_beam_out
+        return tuple(x[:nreq] for x in split_beam_out(out, b, self.beam.width))
+
+
 def _to_numpy(out):
     return tuple(x.cpu().numpy() for x in out) if isinstance(out, tuple) else out.cpu().numpy()
 
@@ -854,7 +1089,7 @@ def pool_capacity(batch_size: int, maxlen: int, block_len: int, num_draft: int =
 def run_textgen(model: Callable, rs: RequestSet, cfg: TextGenConfig, pool: KvPoolInt4, device, sync: Callable = None,
                 keep_tokens: bool = False, progress: Callable = None, decode_runner: DecodeGraphRunner = None,
                 sample_op: Callable = None, slot_init_op: Callable = None, propose_op: Callable = None,
-                draft_sample_op: Callable = None) -> TextGenBenchResult:
+                draft_sample_op: Callable = None, beam_select_op: Callable = None, copy_op: Callable = None) -> TextGenBenchResult:
     """Drive `model(input_ids, blen, prefill_kv, decode_kv) -> (logits, hidden)` through the whole request set.
     Latencies are wall-clock around the step *including* the device->host read of the next tokens (which synchronises),
     as in the reference.  With a `decode_runner`, steps that carry no prompt tokens are replayed from its CUDA graphs.
@@ -867,7 +1102,12 @@ def run_textgen(model: Callable, rs: RequestSet, cfg: TextGenConfig, pool: KvPoo
     cfg.speculate: token histories of cfg.batch_size slots (ops.spec_history) hold each request's context, set up at admission
     (ops.spec_init_slot); every step samples with `draft_sample_op` (default ops.sample_tokens with drafts, at T = 0 when
     greedy) and then commits and proposes with `propose_op` (default ops.spec_commit_propose); the runner must have been built
-    with the same SpeculativeParams and is given the same histories.  Not with penalties."""
+    with the same SpeculativeParams and is given the same histories.  Not with penalties.
+    cfg.beam: every request keeps up to W beams (TextGenScheduler.commit_beam); each step first runs the page copies of the
+    previous step's forks with `copy_op` (default ops.copy_kv_pages), then the model, then `beam_select_op` (default
+    ops.beam_select) on the rows of every request's beams; the runner must have been built with the same BeamSearchParams and
+    stop ids.  The result's tokens are each request's best hypothesis, beam_scores their scores.  Not with sampling or
+    speculation, and cfg.batch_size (rows) must hold W."""
     sp = cfg.sampling
     if sp is not None and sample_op is None:
         from . import ops
@@ -879,6 +1119,21 @@ def run_textgen(model: Callable, rs: RequestSet, cfg: TextGenConfig, pool: KvPoo
         raise ValueError("speculative decoding cannot be combined with penalties")
     if decode_runner is not None and decode_runner.speculate != spec:
         raise ValueError("decode_runner was built for other speculative parameters than cfg.speculate")
+    beam = cfg.beam
+    if beam is not None:
+        if sp is not None or spec is not None:
+            raise ValueError("beam search cannot be combined with sampling, penalties or speculative decoding")
+        if cfg.batch_size < beam.width:
+            raise ValueError(f"batch_size={cfg.batch_size} rows cannot hold a request of {beam.width} beams")
+        if decode_runner is not None and (decode_runner.beam != beam or
+                                          decode_runner.stop_token_ids != tuple(int(t) for t in cfg.stop_token_ids)):
+            raise ValueError("decode_runner was built for other beam parameters or stop ids than cfg")
+        if beam_select_op is None or copy_op is None:
+            from . import ops
+        beam_select_op = beam_select_op or ops.beam_select
+        copy_op = copy_op or ops.copy_kv_pages
+    elif decode_runner is not None and decode_runner.beam is not None:
+        raise ValueError("decode_runner was built for beam search and cfg.beam is None")
     vocab = _vocab_size(model)
     table = None
     if sp is not None and sp.penalties:
@@ -909,7 +1164,8 @@ def run_textgen(model: Callable, rs: RequestSet, cfg: TextGenConfig, pool: KvPoo
     gsp = sp if sp is not None else SamplingParams(0.0)     # speculating, greedy is the draft sampler at T = 0
     sched = TextGenScheduler(rs, cfg.batch_size, pool, device, vocab_size=vocab, prefill_chunk=cfg.prefill_chunk,
                              shared_prefix=cfg.shared_prefix, stop_token_ids=cfg.stop_token_ids,
-                             penalty_slots=table is not None or spec is not None, num_draft=0 if spec is None else spec.num_draft)
+                             penalty_slots=table is not None or spec is not None, num_draft=0 if spec is None else spec.num_draft,
+                             beam=beam)
     steps = graphed = peak = 0
     t_start = time.perf_counter()
     while not sched.finished:
@@ -923,7 +1179,26 @@ def run_textgen(model: Callable, rs: RequestSet, cfg: TextGenConfig, pool: KvPoo
         peak = max(peak, pool.capacity - pool.num_free_blocks)
         t1 = time.perf_counter()
         logprobs = None
-        if spec is not None and decode_runner is not None and sched.prompt_tokens == 0:
+        if beam is not None:
+            copies = sched.take_copies()
+            if decode_runner is not None and sched.prompt_tokens == 0:
+                next_tokens = decode_runner.run_beam([int(r.output[-1]) for r in sched.workset], [r.kvcache for r in sched.workset],
+                                                     copies, sched.beam_rows(), sched.beam_sums())
+                graphed += 1
+            else:
+                if copies:
+                    copy_op(pool, *([c[k] for c in copies] for k in range(3)))
+                batch = sched.next_batch()
+                ids = torch.tensor(batch.input_ids, dtype=torch.long, device=device)
+                logits, _ = model(ids, batch.blen, batch.prefill_kv, batch.decode_kv)
+                rows = torch.tensor(sched.last_token_rows(), dtype=torch.long, device=logits.device)
+                rip = torch.tensor(sched.beam_rows(), dtype=torch.int32, device=logits.device)
+                next_tokens = ([], [], [], [])
+                if len(rip) > 1:                    # (a step of prompt chunks alone takes no beam step)
+                    sums = torch.tensor(sched.beam_sums(), dtype=torch.float32, device=logits.device)
+                    next_tokens = _to_numpy(tuple(beam_select_op(logits.index_select(0, rows), rip, sums, beam.width,
+                                                                 cfg.stop_token_ids)))
+        elif spec is not None and decode_runner is not None and sched.prompt_tokens == 0:
             out = decode_runner.run_spec(sched.S, sched.decode_ids(), sched.candidates(), [r.kvcache for r in sched.workset],
                                          sched.sample_slots(), sched.sequence_slots())
             next_tokens, logprobs = (out[0], out[1:]) if isinstance(out, tuple) else (out, None)
@@ -976,7 +1251,9 @@ def run_textgen(model: Callable, rs: RequestSet, cfg: TextGenConfig, pool: KvPoo
         if sync is not None:
             sync()
         t2 = time.perf_counter()
-        if spec is not None:
+        if beam is not None:
+            n = sched.commit_beam(*next_tokens, t1, t2)
+        elif spec is not None:
             n = sched.commit_spec(next_tokens, t1, t2, logprobs)
         else:
             n = sched.commit(next_tokens, t1, t2) if logprobs is None else sched.commit(next_tokens, t1, t2, logprobs)
@@ -988,6 +1265,8 @@ def run_textgen(model: Callable, rs: RequestSet, cfg: TextGenConfig, pool: KvPoo
     res.peak_pages = peak
     if spec is not None:
         res.speculative = dict(sched.spec_stats)
+    if beam is not None:                    # a copied slot is 64 bytes of pool.buf and 4 of pool.param per (layer, K|V, head)
+        res.beam["bytes_copied"] = res.beam["copied_slots"] * pool.num_layers * 2 * pool.buf.shape[3] * 68
     return res
 
 
@@ -1011,6 +1290,11 @@ def report(rs: RequestSet, cfg: TextGenConfig, res: TextGenBenchResult) -> dict:
     }
     if cfg.stop_token_ids:
         out["stop_token_ids"] = [int(t) for t in cfg.stop_token_ids]
+    if cfg.beam is not None and res.beam is not None:
+        st = res.beam
+        out["beam"] = {"width": cfg.beam.width, "length_penalty": cfg.beam.length_penalty, "page_copies": st["page_copies"],
+                       "page_copies_per_step": st["page_copies"] / res.steps if res.steps else 0.0,
+                       "bytes_copied": st["bytes_copied"], "stop_finished_requests": st["stop_finished"]}
     if cfg.speculate is not None and res.speculative is not None:
         st, sp = res.speculative, cfg.speculate
         out["speculative"] = {

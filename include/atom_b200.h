@@ -419,6 +419,29 @@ ATOM_API int atom_spec_commit_propose(const void* tokens, const void* cands, con
                                       void* history, void* history_len, int num_slots, int cap, int num_draft, int ngram_min,
                                       int ngram_max, void* out, void* stream);
 
+/* atom_beam_select_f16: one beam-search step (new; DESIGN section 5.9).  logits f16 [rows][ld], sums f32 [rows] (each row's
+ * beam's running sum), row_indptr i32 [batch + 1] (request i owns rows row_indptr[i] .. row_indptr[i+1]; zero rows is allowed),
+ * stop_ids: num_stop <= 8 distinct host ids in [0, vocab), width W in [1, 8].  For every row, lp(t) is bit for bit the
+ * log-probability atom_sample_ex_f16 reports for token t at T = 1 without penalties; a row holding NaN or +inf, or only -inf,
+ * has no candidates, and neither has a token at -inf.  A candidate's key is fl32(sums[row] + lp(t)).  A request's candidates
+ * are ordered by key descending, then row ascending, then the row's order (larger logit, then lower id); walking them at rank
+ * i = 0, 1, ..: a stop id of rank < W is written to fin, one of rank >= W is skipped, any other token is written to live until
+ * there are W.  live and fin i32 [batch][W][2] hold (row, token), live_key and fin_key f32 [batch][W] the keys; unused entries
+ * are -1.  A request of more than W rows gets none.  workspace: 16-byte aligned, rows * 192 bytes.  Two launches (the per-row
+ * lists, then one CTA per request); every device input is read after the preceding kernel has completed.  With rows = 0 only
+ * the second runs (every request gets none), and logits and sums may be null. */
+ATOM_API int atom_beam_select_f16(const void* logits, int64_t ld, int rows, int vocab, const void* row_indptr, int batch,
+                                  const void* sums, const int* stop_ids, int num_stop, int width, void* workspace, void* live,
+                                  void* live_key, void* fin, void* fin_key, void* stream);
+
+/* atom_kv_copy_pages_i4: the page copies of copy-on-write forks in one launch (new; DESIGN section 5.9).  Pair p of src, dst,
+ * slots (i32 [n], read on the device after the preceding kernel has completed) copies the first slots[p] token slots of page
+ * src[p] to page dst[p] in every (layer, K|V, head) block of kv_data (u8 [num_pages][num_layers][2][num_heads][page_size][64])
+ * and kv_param (f16 [...][page_size][2]); the bytes past slots[p] are left untouched.  src < 0 is padding; src == dst, a page
+ * outside [0, num_pages) or slots outside [1, page_size] make the pair a no-op. */
+ATOM_API int atom_kv_copy_pages_i4(void* kv_data, void* kv_param, int num_pages, int num_layers, int num_heads, int page_size,
+                                   const void* src, const void* dst, const void* slots, int n, void* stream);
+
 /* atom_sample_slot_init: set up slot `slot` of a penalty table u16 [*][table_ld] (16-byte aligned, table_ld >= vocab a multiple
  * of 8) for a new request in one launch: zero the row, then set bit 15 of every token in prompt i32 [prompt_len] (ids outside
  * [0, vocab) are ignored). */

@@ -68,6 +68,9 @@ def main():
                     help="speculative decoding with up to K prompt-lookup drafts per sequence and step (0 = off; 1 to 7)")
     ap.add_argument("--ngram-max", type=int, default=3, help="with --speculate: the longest n-gram the proposer matches")
     ap.add_argument("--ngram-min", type=int, default=1, help="with --speculate: the shortest n-gram the proposer matches")
+    ap.add_argument("--beam-width", type=int, default=0, metavar="W",
+                    help="beam search with W beams per request (0 = off; 1 to 8); --batch-size then counts beams")
+    ap.add_argument("--length-penalty", type=float, default=0.0, help="with --beam-width: hypotheses score sum / len^A")
     ap.add_argument("--warmup-batches", type=int, default=1,
                     help="untimed request batches served first (first-use costs: lazy kernel loading, attribute calls, graph "
                          "capture); 0 = time the cold process like the reference's script")
@@ -90,7 +93,8 @@ def main():
     sampling = None if args.temperature is None else tg.SamplingParams(args.temperature, args.top_k, args.top_p, args.seed, **extra)
     spec = tg.SpeculativeParams(args.speculate, args.ngram_max, args.ngram_min) if args.speculate else None
     cfg = tg.TextGenConfig(args.batch_size, prefill_chunk=args.prefill_chunk, shared_prefix=args.shared_prefix, sampling=sampling,
-                           stop_token_ids=tuple(args.stop_token), speculate=spec)
+                           stop_token_ids=tuple(args.stop_token), speculate=spec,
+                           beam=tg.BeamSearchParams(args.beam_width, args.length_penalty) if args.beam_width else None)
     # speculating, a sequence grows by up to K + 1 tokens past its length within a step: those pages too, per sequence
     spec_pages = -(-(args.speculate + 1) // args.block_len) if spec else 0
     shared_pages = -(-args.shared_prefix // args.block_len)           # the system prompt's pages, held once
@@ -100,7 +104,7 @@ def main():
                       args.block_len, device)
     runner = None if args.no_cuda_graphs else tg.DecodeGraphRunner(
         model, pool, device, max_pages_per_seq=(args.maxlen + args.block_len - 1) // args.block_len + 1 + shared_pages + spec_pages,
-        sampling=sampling, speculate=spec)
+        sampling=sampling, speculate=spec, beam=cfg.beam, stop_token_ids=cfg.stop_token_ids)
     if args.warmup_batches > 0:
         wrs = tg.generate_request_set(args.batch_size * args.warmup_batches, args.maxlen)
         tg.run_textgen(model, wrs, cfg, pool, device, sync=torch.cuda.synchronize, decode_runner=runner)
@@ -119,6 +123,11 @@ def main():
     print("duration:", f"{rep['duration_s']:.3f}s")
     print("throughput ((prompt+new)/duration):", f"{rep['throughput_tokens_per_s']:.3f} token/s")
     print("peak KV pages in use:", rep["peak_kv_pages_in_use"], f"of {pool.capacity}")
+    if cfg.beam is not None:
+        b = rep["beam"]
+        print("beam:", f"width {b['width']}, length penalty {b['length_penalty']}, {b['page_copies']} page copies "
+              f"({b['page_copies_per_step']:.2f} per step, {b['bytes_copied'] / 1e6:.1f} MB), {b['stop_finished_requests']} requests "
+              "ended on a stop id")
     if spec is not None:
         s = rep["speculative"]
         print("speculative:", f"{s['verify_steps']} verify steps, {s['accepted_tokens']} of {s['drafted_tokens']} drafts accepted "
