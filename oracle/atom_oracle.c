@@ -125,8 +125,10 @@ static void quant_tail_row(const float *x, int hidden, int row, int scale_ldm,
   }
 }
 
-/* K3: reorder_fp16_i4 (kernels/include/Reorder/Reorder.cuh:64-190) */
-void atom_oracle_reorder_fp16_i4(const h16 *in, int seq_len, int hidden, const int16_t *idx,
+/* K3: reorder_fp16_i4 (kernels/include/Reorder/Reorder.cuh:64-190).
+ * The reorder index is read as uint16_t, as the kernels read it: hidden may reach 65536, so an index >= 32768 is a
+ * column of the row, not an offset before it. */
+void atom_oracle_reorder_fp16_i4(const h16 *in, int seq_len, int hidden, const uint16_t *idx,
                                  int8_t *s8out, uint8_t *s4out, h16 *s8scale, h16 *s4scale) {
   const int ldm = atom_oracle_scale_size(seq_len);
   float *x = (float *)malloc(sizeof(float) * hidden);
@@ -140,9 +142,10 @@ void atom_oracle_reorder_fp16_i4(const h16 *in, int seq_len, int hidden, const i
 /* K4: rmsnorm_fp16_i4 (kernels/include/RMSNorm/RMSNorm.cuh:66-238).
  * Sum of squares follows the reference's order: 128 "threads" each fold hidden/128
  * contiguous elements with fmaf, then tree 128->64->32 and shfl_down 16..1.
- * rstd uses 1/sqrtf (the GPU uses rsqrtf, max 2 ulp) => +-1 LSB tolerance in tests. */
+ * rstd uses 1/sqrtf (the GPU uses rsqrtf, max 2 ulp) => +-1 LSB tolerance in tests.
+ * The reorder index is uint16_t, as in K3. */
 void atom_oracle_rmsnorm_fp16_i4(const h16 *in, const h16 *w, float eps, int seq_len, int hidden,
-                                 const int16_t *idx, int8_t *s8out, uint8_t *s4out,
+                                 const uint16_t *idx, int8_t *s8out, uint8_t *s4out,
                                  h16 *s8scale, h16 *s4scale) {
   const int ldm = atom_oracle_scale_size(seq_len);
   const int ept = hidden / 128;

@@ -60,7 +60,8 @@ def _quant_outputs(m, hidden):
 
 
 def reorder_fp16_i4(x, idx):
-    x, idx = _c(x, np.float16), _c(idx, np.int16)
+    """`idx` holds 16-bit column indices read as unsigned (hidden <= 65536): an int16 array is taken bit for bit."""
+    x, idx = _c(x, np.float16), _c(idx, np.uint16)
     m, h = x.shape
     o8, o4, s8, s4 = _quant_outputs(m, h)
     lib().atom_oracle_reorder_fp16_i4(_p(x), m, h, _p(idx), _p(o8), _p(o4), _p(s8), _p(s4))
@@ -68,7 +69,7 @@ def reorder_fp16_i4(x, idx):
 
 
 def rmsnorm_fp16_i4(x, w, idx, eps):
-    x, w, idx = _c(x, np.float16), _c(w, np.float16), _c(idx, np.int16)
+    x, w, idx = _c(x, np.float16), _c(w, np.float16), _c(idx, np.uint16)
     m, h = x.shape
     o8, o4, s8, s4 = _quant_outputs(m, h)
     lib().atom_oracle_rmsnorm_fp16_i4(_p(x), _p(w), ctypes.c_float(eps), m, h, _p(idx), _p(o8), _p(o4), _p(s8), _p(s4))
